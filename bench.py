@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — rasterizer fwd+bwd Mpix/s @1080p (1M Gaussians) on N B200s.
+"""bench.py — rasterizer fwd+bwd Mpix/s @1080p (1M Gaussians) on N H100s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
@@ -18,7 +18,8 @@ Printed (rank 0, ONE JSON line):
            -> loss -> backward); per step the camera matrices and the target image are
            copied host->device from pinned memory and the loss is read back.
   roofline the dominant kernel: algorithmic bytes per launch (SURVEY.md §8d / DESIGN.md)
-           / its mean launch duration measured live with CUDA events around the launch.
+           / its mean launch duration measured live with CUDA events around the launch, over the
+           H100 SXM data-sheet HBM3 bandwidth (3.35 TB/s).
   cpu_baseline  the CPU oracle (oracle/sfgs_oracle.c, a port: the reference has no CPU
            path) timed on this box's host cores on a bounded sample.
 `--impl reference` times the UNMODIFIED reference through its own stock code path: its pybind module `diff_gauss._C`
@@ -33,9 +34,10 @@ Extra records in the same line (single-GPU run only; they never change `value`):
   ssim          fused-ssim forward(train)+backward at 1x3x1080x1920 with the 72N / 84N-byte roofline of SURVEY 8d, this
                 library next to the reference's compiled kernel (when oracle/_ref has it);
   train_loop    a bounded sample (300 iterations) of the BASELINE configs[2] Stage-1 loop, it/s, either arm with its own packages;
-  next_ops      (this library) the fused appearance path and compute_3D_filter next to their torch formulations;
-  roofline.traffic  dram__bytes_read + dram__bytes_write of the dominant kernel measured in THIS run by an `ncu`
-                subprocess (falls back to profiles/traffic.json and says so in `traffic_source`).
+  next_ops      (this library) the fused appearance path and compute_3D_filter next to their torch formulations.
+`--dump-outputs DIR` (this library only) writes, after the timed steps, what the last timed step computed as float32
+`.npy` files: the four output images at a fixed seeded sample of pixels, and radii and every per-Gaussian gradient at a
+fixed seeded sample of Gaussians (about 48 MB at the default size), so that two builds can be compared output for output.
 Multi-GPU: the headline is the "views" mode — ranks render different cameras of the replicated scene (weak scaling, no
 data-path collective).  In the same invocation every rank then also runs the tile-row sharded mode (ONE frame split by
 balanced bands of tile rows, image all-gather and [P,16] reduce-scatter fused into the kernels over NVLink peer memory,
@@ -48,7 +50,6 @@ import argparse
 import json
 import math
 import os
-import subprocess
 import sys
 import threading
 import time
@@ -72,11 +73,7 @@ METRIC = "rasterizer fwd+bwd Mpix/s @1080p (1M Gaussians)"
 
 # ----------------------------------------------------------------------------- helpers
 def peaks():
-    path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(path):
-        with open(path) as f:
-            return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 class ClockSampler:
@@ -85,8 +82,8 @@ class ClockSampler:
     The clock is measured IN-STREAM, in the un-timed gap between two steps while the previous step's backward
     is still in flight: a one-thread kernel (sfgs_sm_clock_probe) counts SM cycles against %globaltimer for
     ~20 us.  NVML is only touched before the warm-up (max clock) and once right after the last timed step
-    (throttle reasons): polling NVML or nvidia-smi from the host DURING the loop was measured to inflate the
-    median step from 1.8 ms to 3.8-4.7 ms with 30-70 ms outliers on these boxes."""
+    (throttle reasons): polling NVML or nvidia-smi from the host DURING the loop inflates the median step and
+    adds outliers of tens of ms."""
 
     def __init__(self, index: int, dev):
         self.index, self.dev = index, dev
@@ -150,7 +147,7 @@ def algorithmic_bytes(P, V, R, N, M, tiles):
 
 class L2Flusher:
     def __init__(self, dev):
-        self.buf = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 126 MB L2
+        self.buf = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 50 MB L2
 
     def __call__(self):
         self.buf.add_(1)
@@ -234,10 +231,10 @@ def step_ref_stock(d, cam):
 
 def settle(step_fn, flush, dev, min_seconds=0.5, max_seconds=3.0):
     """UNTIMED extra warm-up after the W requested steps.  A freshly set-up loop (or one resumed after the GPU sat idle
-    while the host prepared the next scene) runs its first 0.1-0.3 s in a slow mode on these boxes — steps of 5-8 ms,
-    sometimes bursts of 20-40 ms, then 1.08 ms flat for good (gpurun_out/v1_bench.err, v3_bench.err) — which five
-    warm-up steps do not outlast.  So steps are run four at a time for at least `min_seconds` of wall clock and until a
-    group is within 5 % of the fastest group seen (at most `max_seconds`).  Nothing here is reported."""
+    while the host prepared the next scene) can run its first 0.1-0.3 s in a slow mode — steps several times the
+    steady-state time, sometimes bursts of tens of ms — which five warm-up steps do not outlast.  So steps are run four
+    at a time for at least `min_seconds` of wall clock and until a group is within 5 % of the fastest group seen (at
+    most `max_seconds`).  Nothing here is reported."""
     best, n, t0 = None, 0, time.perf_counter()
     while True:
         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -643,7 +640,7 @@ def next_ops_record(dev):
                                  "algorithmic_bytes": 324 * P, "GBps": round(324 * P / t_fused / 1e6, 1),
                                  "frac_of_hbm_peak": round(324 * P / t_fused / 1e6 / peak, 4),
                                  "tensor_core_flops": 3 * 2 * P * (32 * 128 + 128 * 128 + 128 * 16),
-                                 "note": "tcgen05 kernel (split-bf16 operands, fp32 accumulate in TMEM) vs the reference's statements in torch"}
+                                 "note": "wgmma kernel (split-bf16 operands, fp32 accumulate) vs the reference's statements in torch"}
     # compute_3D_filter: 64 cameras
     rng = np.random.default_rng(2)
     cams = []
@@ -765,41 +762,24 @@ def density_control_record(dev, timeit):
                                   "note": "both include the quantile (torch.quantile) and one host synchronisation; Adam moments moved with the rows"}}
 
 
-def live_traffic(kernel_regex, timeout_s=240):
-    """dram__bytes_read + dram__bytes_write (and issue-slot utilisation) of ONE launch of the dominant kernel, captured in
-    this run by an ncu subprocess over tests/gpu_profile_case.py (same scene, camera and cotangents as the timed loop).
-    Returns None when ncu is unavailable."""
-    import csv
-    import shutil
-    import tempfile
-    ncu = shutil.which("ncu") or "/usr/local/cuda/bin/ncu"
-    if not os.path.exists(ncu):
-        return None
-    with tempfile.TemporaryDirectory() as td:
-        log = os.path.join(td, "t.csv")
-        cmd = [ncu, "--metrics", "dram__bytes_read.sum,dram__bytes_write.sum,sm__issue_active.avg.pct_of_peak_sustained_elapsed,"
-               "smsp__inst_executed.sum,gpu__time_duration.sum", "--clock-control", "none", "-k", f"regex:{kernel_regex}",
-               "-s", "1", "-c", "1", "--csv", "--log-file", log, sys.executable, os.path.join(ROOT, "tests", "gpu_profile_case.py"),
-               "--iters", "2"]
-        try:
-            subprocess.run(cmd, capture_output=True, text=True, timeout=timeout_s, check=True)
-            vals = {}
-            with open(log) as fh:
-                rows = [r for r in csv.reader(l for l in fh if not l.startswith("=="))]
-            h0 = next(i for i, r in enumerate(rows) if "Metric Name" in r and "Metric Value" in r)
-            hdr = rows[h0]
-            for r in rows[h0 + 1:]:
-                row = dict(zip(hdr, r))
-                v = float(row["Metric Value"].replace(",", ""))
-                unit = row.get("Metric Unit", "")
-                scale = {"byte": 1, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}.get(unit, 1)
-                vals[row["Metric Name"]] = v * scale
-            return {"traffic": int(vals["dram__bytes_read.sum"] + vals["dram__bytes_write.sum"]),
-                    "issue_active_pct": round(vals["sm__issue_active.avg.pct_of_peak_sustained_elapsed"], 1),
-                    "warp_instructions": int(vals["smsp__inst_executed.sum"])}
-        except Exception as exc:  # noqa: BLE001
-            print(f"[bench] live ncu capture failed: {type(exc).__name__}: {str(exc)[:200]}", file=sys.stderr)
-            return None
+def dump_outputs(out_dir, f, g, n_pix=1 << 18, n_gauss=1 << 17, seed=0):
+    """The timed path's outputs as float32 .npy files: images at `n_pix` pixels and per-Gaussian arrays at `n_gauss`
+    Gaussians, both index sets drawn once from `seed` (the same rows and pixels for every build of the same workload)."""
+    os.makedirs(out_dir, exist_ok=True)
+    rng = np.random.default_rng(seed)
+    _, color, depth, norm, alpha, radii = f[:6]
+    HW = color.shape[1] * color.shape[2]
+    P = radii.shape[0]
+    pix = torch.from_numpy(np.sort(rng.choice(HW, size=min(n_pix, HW), replace=False))).to(color.device)
+    rows = torch.from_numpy(np.sort(rng.choice(P, size=min(n_gauss, P), replace=False))).to(radii.device)
+    arrays = {name: t.reshape(t.shape[0], HW)[:, pix] for name, t in
+              (("color", color), ("depth", depth), ("norm", norm), ("alpha", alpha))}
+    arrays["radii"] = radii[rows]
+    for name, t in zip(("dL_dmeans2D", "dL_dcolors", "dL_dopacity", "dL_dmeans3D", "dL_dcov3D", "dL_dnorm3D", "dL_dsh",
+                        "dL_dscales", "dL_drotations"), g[:9]):
+        arrays[name] = t[rows]
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().cpu().numpy())
 
 
 # ----------------------------------------------------------------------------- main
@@ -813,8 +793,11 @@ def main():
     ap.add_argument("--P", type=int, default=P_GAUSS)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-clocks", action="store_true", help="do not sample SM clocks during the timed region")
-    ap.add_argument("--no-extras", action="store_true", help="skip the extra frames / ssim / ncu / tile-row records")
+    ap.add_argument("--no-extras", action="store_true", help="skip the extra frames / ssim / tile-row records")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs dumps this library's outputs (--impl ours)")
     steps, warmup = max(1, args.steps), max(3, args.warmup)
 
     rank = int(os.environ.get("RANK", "0"))
@@ -841,9 +824,13 @@ def main():
     flush = L2Flusher(dev)
 
     from sfgs import native
+    last = {}
     if kind == "ours":
         native.lib()
-        step = lambda: step_ours(d, cam)  # noqa: E731
+
+        def step():
+            last["out"] = step_ours(d, cam)      # the last timed step's outputs, for --dump-outputs
+            return last["out"]
     elif kind == "stock":
         step = lambda: step_ref_stock(d, cam)  # noqa: E731
     else:
@@ -855,8 +842,11 @@ def main():
         dist.barrier()
     torch.cuda.synchronize(dev)
     ms, value_info = measure(step, steps, warmup, flush, dev,
-                             between=sampler.sample if (args.impl == "ours" and not args.no_clocks) else None)
+                             between=sampler.sample if (args.impl == "ours" and not args.no_clocks) else None, max_attempts=1)
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *last["out"])
+    last.clear()
     total_ms = torch.tensor([sum(ms)], dtype=torch.float64, device=dev)
     if world > 1:
         dist.barrier()
@@ -872,7 +862,7 @@ def main():
         e2e_obj = E2E(scene, cam, dev, ref_packages()[0])
     else:
         e2e_obj = E2ERefShim(scene, cam, dev)
-    e2e_ms, e2e_info = measure(e2e_obj.step, steps, warmup, flush, dev)
+    e2e_ms, e2e_info = measure(e2e_obj.step, steps, warmup, flush, dev, max_attempts=1)
     e2e_total = torch.tensor([sum(e2e_ms)], dtype=torch.float64, device=dev)
     if world > 1:
         dist.all_reduce(e2e_total, op=dist.ReduceOp.MAX)
@@ -924,7 +914,7 @@ def main():
                    "d2h_bytes_per_step": 4},
            "clocks": clocks}
     out["timing"] = {"value": value_info, "e2e": e2e_info,
-                     "rule": "W warm-up steps, then untimed steps in groups of 4 for >= 0.5 s and until a group is within 5 % of the fastest group (<= 3 s), then exactly K timed steps; a pass whose mean step exceeds 1.05x its fastest step is re-measured (<= 8 passes)"}
+                     "rule": "W warm-up steps, then untimed steps in groups of 4 for >= 0.5 s and until a group is within 5 % of the fastest group (<= 3 s), then exactly K timed steps"}
     out["e2e"]["api"] = {"ours": "diff_gauss.GaussianRasterizer + autograd (this library's drop-in package)",
                          "stock": "the reference's own diff_gauss.GaussianRasterizer + autograd over its own pybind module",
                          "shim": "reference CudaRasterizer::Rasterizer forward/backward behind the ctypes shim"}[kind]
@@ -1003,21 +993,6 @@ def main():
                 out["next_ops"] = next_ops_record(dev)
             except Exception as exc:  # noqa: BLE001
                 out["next_ops"] = {"error": f"{type(exc).__name__}: {exc}"[:300]}
-        if kind == "ours":
-            torch.cuda.synchronize(dev)
-            lt = live_traffic({"render_bwd": "render_bwd", "render_fwd": "render_fwd"}.get(dom, dom))
-            if lt is not None:
-                out["roofline"].update(traffic=lt["traffic"], traffic_source="ncu subprocess in this run (one launch, "
-                                       "dram__bytes_read.sum + dram__bytes_write.sum)")
-                out["roofline"]["limiter"] = (f"instruction issue: {lt['issue_active_pct']}% of issue slots active, "
-                                              f"{lt['warp_instructions']} warp instructions (same ncu capture)")
-            else:
-                tpath = os.path.join(ROOT, "profiles", "traffic.json")
-                if os.path.exists(tpath):
-                    with open(tpath) as fh:
-                        tj = json.load(fh)
-                    out["roofline"].update(traffic=tj.get("kernels", {}).get(dom),
-                                           traffic_source="profiles/traffic.json (committed ncu capture; live capture unavailable)")
     if not args.no_cpu_baseline and world == 1:   # the CPU port is timed on rank 0 of the single-GPU run only
         out["cpu_baseline"] = cpu_baseline(scene, cam)
     print(json.dumps(out))

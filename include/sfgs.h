@@ -1,5 +1,5 @@
 /*
- * sfgs.h — C ABI of the B200-native splat rasterizer (libsfgs.so).
+ * sfgs.h — C ABI of the H100-native splat rasterizer (libsfgs.so).
  *
  * Drop-in boundary for the hot path of jayin92/Skyfall-GS: every entry point
  * below replaces one entry of the reference's native interface.  Citations
@@ -246,7 +246,7 @@ int sfgs_activations_backward(int P, const float* opacity_raw, const float* scal
  * the toned coefficients along normalize(xyz - campos) (utils/sh_utils.py), +0.5, clamp at 0  ->  colors_precomp [P,3].
  * W1 is [128, 3+G+E] row-major (torch.nn.Linear.weight), W2 [128,128], W3 [6,128]; features [P,M,3] with M = 16,
  * gemb [P,G] with G = 24 (4 Fourier frequencies), aemb [E] with E = 32; D = active SH degree.  Tensor-core
- * operands are split bf16 pairs (hi + lo, three tcgen05.mma per product), fp32 accumulation in TMEM; the result is
+ * operands are split bf16 pairs (hi + lo, three wgmma per product), fp32 accumulation in registers; the result is
  * within 1e-4 of the float32 torch evaluation.  features and gemb must be 16-byte aligned. */
 int sfgs_appearance_forward(int P, int D, int M, const float* features, const float* gemb, int G, const float* aemb,
                             int E, const float* W1, const float* b1, const float* W2, const float* b2,

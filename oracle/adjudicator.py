@@ -32,7 +32,7 @@ def build(force: bool = False) -> str:
     os.makedirs(OUT_DIR, exist_ok=True)
     if force or not os.path.exists(LIB) or os.path.getmtime(LIB) < os.path.getmtime(SRC):
         # no fast-math, default FMA contraction: the flags the reference rasterizer is built with (oracle/build_ref.py)
-        cmd = [os.environ.get("NVCC", "nvcc"), "-std=c++17", "-O3", "-gencode", "arch=compute_100a,code=sm_100a",
+        cmd = [os.environ.get("NVCC", "nvcc"), "-std=c++17", "-O3", "-gencode", "arch=compute_90a,code=sm_90a",
                "-Xcompiler", "-fPIC", "-shared", SRC, "-o", LIB]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:

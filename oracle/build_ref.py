@@ -29,7 +29,7 @@ LIB = os.path.join(OUT, "libref_rasterizer.so")
 
 FLAGS = ["-std=c++17", "-O3", "-include", "cstdint", "-include", os.path.join(HERE, "ref_glm_fix.h"),
          "--expt-relaxed-constexpr", "-w",
-         "-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC",
+         "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC",
          "-I", os.path.join(RAST, "third_party", "glm"), "-I", os.path.join(RAST, "cuda_rasterizer"), "-I", KNN]
 
 
@@ -63,7 +63,7 @@ def build(force: bool = False) -> str | None:
 
     with ThreadPoolExecutor(max_workers=5) as ex:
         objs = list(ex.map(cc, srcs.items()))
-    r = subprocess.run([nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"],
+    r = subprocess.run([nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"],
                        capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("reference link failed:\n" + r.stderr)

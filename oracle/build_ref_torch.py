@@ -41,7 +41,7 @@ def built() -> bool:
 def _load(name, sources, build_dir, extra_cuda, include):
     from torch.utils import cpp_extension
     os.makedirs(build_dir, exist_ok=True)
-    os.environ["TORCH_CUDA_ARCH_LIST"] = "10.0a"
+    os.environ["TORCH_CUDA_ARCH_LIST"] = "9.0a"
     cpp_extension.load(name=name, sources=sources, extra_include_paths=include, extra_cuda_cflags=extra_cuda,
                        extra_cflags=["-include", "cstdint"], build_directory=build_dir, is_python_module=False,
                        verbose=False)

@@ -1,4 +1,4 @@
-"""Build recipe for libsfgs.so (sm_100a only).
+"""Build recipe for libsfgs.so (sm_90a only).
 
 Plain nvcc, in-tree output (skyfall-gs_b200/lib/libsfgs.so) so the built
 library travels with the repository snapshot to the GPU box.  No torch headers
@@ -20,7 +20,7 @@ LIB = os.path.join(LIBDIR, "libsfgs.so")
 
 NVCC_FLAGS = [
     "-std=c++17", "-O3", "-lineinfo",
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-Xcompiler", "-fPIC",
 ]
 
@@ -67,7 +67,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         if stale.endswith(".o") and os.path.join(OBJDIR, stale) not in objs:
             os.remove(os.path.join(OBJDIR, stale))
     if jobs or force or _newer(objs, LIB):
-        run([nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"])
+        run([nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"])
     return LIB
 
 

@@ -14,101 +14,121 @@
 // The per-camera embedding `aemb` is the same vector for every Gaussian, so its 32 columns of W1 fold into the bias
 // (b1' = b1 + W1[:, 27:] aemb, computed once per CTA) and layer 1 contracts over K = 27 (padded to 32).
 //
-// Tensor cores: a CTA owns a tile of 128 Gaussians = the M = 128 rows of three tcgen05.mma (kind::f16, split-bf16
-// operands, fp32 accumulate) GEMMs: [128x32]x[32x128], [128x128]x[128x128], [128x128]x[128x16].  Weights are converted to bf16
-// once per CTA and stay in shared memory in the canonical K-major no-swizzle core-matrix layout (8 rows x 16 bytes per
-// core; SBO = 128 B between 8-row groups, LBO = bytes between the two 16-byte K chunks of one MMA); activations never
-// leave the SM: thread m packs row m of the A operand into the same layout, one elected thread issues the MMAs, the
-// fp32 accumulator lives in TMEM (128 lanes x 128 columns) and comes back with tcgen05.ld (lane m -> thread m) for the
-// bias + ReLU + bf16 pack of the next layer.  CTAs are persistent over tiles and run TWO tiles at a time: two groups
-// of 128 threads, each with its own operand buffer, accumulator columns and mbarrier, synchronised only inside the
-// group (named barriers), so one group's epilogue arithmetic overlaps the other group's MMAs and loads.
+// Tensor cores: a CTA owns a tile of 128 Gaussians per warpgroup; each GEMM — [128x32]x[32x128], [128x128]x[128x128],
+// [128x128]x[128x16] — runs as two m64 halves of wgmma.mma_async (bf16 operands from shared memory, fp32 accumulate in
+// registers).  Weights are converted to bf16 once per CTA and stay in shared memory in the canonical K-major
+// no-swizzle core-matrix layout (8 rows x 16 bytes per core; SBO = 128 B between 8-row groups, LBO = bytes between
+// the two 16-byte K chunks of one k16 step); activations never leave the SM: thread m packs row m of the A operand
+// into the same layout, the warpgroup issues the MMAs, and each thread applies bias + ReLU + bf16 pack to the
+// accumulator fragment it holds, writing the next layer's A operand in place.  CTAs are persistent over tiles and
+// run TWO tiles at a time: two warpgroups, each with its own operand buffer, synchronised only inside the group
+// (named barriers), so one group's epilogue arithmetic overlaps the other group's MMAs and loads.
 //
 // Precision: the multiplier head of a trained model is O(1) (h ~ 100 before the x0.01), so plain bf16 operands
 // (2^-9 relative) would leave ~1e-2 in the colours (measured on the golden vectors: 8e-3).  Every operand is therefore
 // carried as TWO bf16 values, x = hi + lo with lo = bf16(x - hi) (16 mantissa bits together), and every product is
 // three tensor-core MMAs into the same fp32 accumulator:  A W ~= Ah Wh + Ah Wl + Al Wh  (the dropped Al Wl term is
-// 2^-18 relative).  The GEMMs stay on tcgen05 at 3x the MMA count — still far below the kernel's HBM time — and the
-// colours agree with the reference's float32 modules to 1e-4 (tests/test_appearance.py).  Everything after the MLP is
-// float32.
+// 2^-18 relative).  The GEMMs stay on the tensor cores at 3x the MMA count — still far below the kernel's HBM time —
+// and the colours agree with the reference's float32 modules to 1e-4 (tests/test_appearance.py).  Everything after
+// the MLP is float32.
 #include <cuda_bf16.h>
 #include "sfgs_common.cuh"
 
 namespace {
 
-constexpr int AP_THREADS = 256;       // two groups of 128 threads, each with its own tile in flight
+constexpr int AP_THREADS = 256;       // two warpgroups, each with its own tile in flight
 constexpr int AP_GROUPS = 2;
 constexpr int AP_M = 128;            // Gaussians per tile
 constexpr int AP_H = 128;            // hidden width
 constexpr int AP_K1 = 32;            // 3 + 24 padded
-constexpr int AP_N3 = 16;            // 6 outputs padded to the smallest N of an M = 128 MMA
+constexpr int AP_N3 = 16;            // 6 outputs padded to a multiple of the MMA's N granularity
 constexpr int AP_G = 24, AP_E = 32;  // Fourier features per Gaussian, per-camera embedding size
-constexpr int AP_TMEM_COLS = 256;      // 128 accumulator columns per group
 
 struct alignas(128) ApSmem {                       // [2] = {hi, lo} halves of the split operands
   __nv_bfloat16 A[AP_GROUPS][2][AP_H / 8][AP_M / 8][8][8];   // 2 x 64 KB  activations, K-major cores: [k chunk][row group][row][8 k]
   __nv_bfloat16 W1[2][AP_K1 / 8][AP_H / 8][8][8];   // 16 KB  [k chunk][n group][n][8 k]
   __nv_bfloat16 W2[2][AP_H / 8][AP_H / 8][8][8];    // 64 KB
   __nv_bfloat16 W3[2][AP_H / 8][AP_N3 / 8][8][8];   //  8 KB
+  float h3[AP_GROUPS][AP_M][8];                     //  8 KB  layer-3 outputs, row m -> thread m
   float b1[AP_H], b2[AP_H], b3[8];
-  unsigned long long bar[AP_GROUPS];
-  uint32_t tmem_base;
 };
+static_assert(sizeof(ApSmem) <= 227 * 1024, "appearance tile buffers exceed the shared memory of one SM");
+
+using ApTile = __nv_bfloat16[2][AP_H / 8][AP_M / 8][8][8];
 
 __device__ __forceinline__ uint64_t smem_desc(const void* p, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  // UMMA shared-memory matrix descriptor, no swizzle ("interleave"): start >> 4 in [0,14), LBO >> 4 in [16,30),
-  // SBO >> 4 in [32,46), version 1 in [46,48), layout type 0 in [61,64)
+  // wgmma shared-memory matrix descriptor, no swizzle: start >> 4 in [0,14), LBO >> 4 in [16,30), SBO >> 4 in [32,46),
+  // base offset 0, swizzle mode 0 in [62,64)
   const uint32_t a = (uint32_t)__cvta_generic_to_shared(p);
   return (uint64_t)((a >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) |
-         ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | (1ull << 46);
+         ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32);
 }
-// instruction descriptor: D = F32 (1 << 4), A = B = BF16 (1 << 7, 1 << 10), both K-major, N >> 3 at [17,23), M >> 4 at [24,29)
-__host__ __device__ constexpr uint32_t instr_desc(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// D (+)= A B with A = 64 x 16 and B = 16 x N, both K-major in shared memory; D is the warpgroup's register fragment:
+// d[4 j + 2 r + e] is row 16 (warp % 4) + lane / 4 + 8 r, column 8 j + 2 (lane % 4) + e
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+               "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+               " %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+               " %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"
+               " %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+               "%64, %65, p, 1, 1, 0, 0;\n\t}\n"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                 "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+                 "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                 "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+                 "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+                 "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+                 "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+                 "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+               : "l"(da), "l"(db), "r"(accumulate) : "memory");
 }
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-  const uint32_t zero = 0;   // disable-output-lane mask: none
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-               "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, {%5, %5, %5, %5}, p;\n\t}\n"
-               ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate), "r"(zero) : "memory");
+__device__ __forceinline__ void wgmma_n16(float (&d)[8], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+               "{%0, %1, %2, %3, %4, %5, %6, %7}, "
+               "%8, %9, p, 1, 1, 0, 0;\n\t}\n"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+               : "l"(da), "l"(db), "r"(accumulate) : "memory");
 }
-__device__ __forceinline__ void umma_commit(unsigned long long* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];"
-               ::"r"((uint32_t)__cvta_generic_to_shared(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned long long* bar, uint32_t parity) {
-  const uint32_t a = (uint32_t)__cvta_generic_to_shared(bar);
-  uint32_t ok;
-  uint32_t spins = 0;
-  do {
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"
-                 : "=r"(ok) : "r"(a), "r"(parity) : "memory");
-    if (!ok && ++spins > (1u << 24)) __trap();      // a lost completion becomes a launch failure, never a hung GPU
-  } while (!ok);
-}
-// 32 consecutive fp32 columns of this thread's TMEM lane
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float v[32]) {
-  uint32_t r[32];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-               "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-               "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                 "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-                 "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-                 "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-               : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+
+// One m64 half of a layer, split-bf16: acc = Ah Wh + Ah Wl + Al Wh over K = 16 KSTEPS.  a_hi / a_lo point at the
+// half's first core matrix in K chunk 0 (K chunks of A are AP_M x 8 elements apart); w_hi / w_lo at W's K chunk 0.
+template <int N, int KSTEPS>
+__device__ __forceinline__ void mma_half(float (&acc)[N / 2], const __nv_bfloat16* a_hi, const __nv_bfloat16* a_lo,
+                                         const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo) {
 #pragma unroll
-  for (int i = 0; i < 32; i++) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float v[8]) {
-  uint32_t r[8];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+  for (int i = 0; i < N / 2; i++) acc[i] = 0.f;
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 #pragma unroll
-  for (int i = 0; i < 8; i++) v[i] = __uint_as_float(r[i]);
+  for (int ks = 0; ks < KSTEPS; ks++) {
+    const uint64_t ah = smem_desc(a_hi + ks * 2 * AP_M * 8, AP_M * 16, 128), al = smem_desc(a_lo + ks * 2 * AP_M * 8, AP_M * 16, 128);
+    const uint64_t wh = smem_desc(w_hi + ks * 2 * N * 8, N * 16, 128), wl = smem_desc(w_lo + ks * 2 * N * 8, N * 16, 128);
+    if constexpr (N == 128) {
+      wgmma_n128(acc, ah, wh, ks > 0); wgmma_n128(acc, ah, wl, 1); wgmma_n128(acc, al, wh, 1);
+    } else {
+      wgmma_n16(acc, ah, wh, ks > 0); wgmma_n16(acc, ah, wl, 1); wgmma_n16(acc, al, wh, 1);
+    }
+  }
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+}
+// relu(acc + bias) of this thread's fragment -> split bf16 into the A operand (rows row0 + lane/4 + {0, 8})
+__device__ __forceinline__ void store_hidden(const float (&acc)[64], const float* bias, ApTile& A, int row0, int lane) {
+#pragma unroll
+  for (int j = 0; j < AP_H / 8; j++) {
+    const int col = 8 * j + 2 * (lane & 3);
+    const float b0 = bias[col], b1 = bias[col + 1];
+#pragma unroll
+    for (int r = 0; r < 2; r++) {
+      const int row = row0 + (lane >> 2) + 8 * r;
+      const float x0 = fmaxf(acc[4 * j + 2 * r] + b0, 0.f), x1 = fmaxf(acc[4 * j + 2 * r + 1] + b1, 0.f);
+      const __nv_bfloat162 hi = __floats2bfloat162_rn(x0, x1);
+      const __nv_bfloat162 lo = __floats2bfloat162_rn(x0 - __low2float(hi), x1 - __high2float(hi));
+      *reinterpret_cast<__nv_bfloat162*>(&A[0][j][row >> 3][row & 7][col & 7]) = hi;
+      *reinterpret_cast<__nv_bfloat162*>(&A[1][j][row >> 3][row & 7][col & 7]) = lo;
+    }
+  }
 }
 __device__ __forceinline__ uint4 pack8(const float* v) {
   __nv_bfloat162 a = __floats2bfloat162_rn(v[0], v[1]), b = __floats2bfloat162_rn(v[2], v[3]);
@@ -138,22 +158,13 @@ appearance_fwd_kernel(int P, int D, const float* __restrict__ features /*[P,16,3
                       const float* __restrict__ means3D, const float* __restrict__ campos, float* __restrict__ colors) {
   extern __shared__ __align__(128) unsigned char ap_smem[];
   ApSmem& S = *reinterpret_cast<ApSmem*>(ap_smem);
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const int grp = tid >> 7, t = tid & 127;       // group and row inside the group's tile
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int grp = tid >> 7, t = tid & 127;       // warpgroup and row inside the group's tile
+  const int wrow = 16 * ((tid >> 5) & 3);        // first accumulator row of this warp inside an m64 half
   constexpr int IN = 3 + AP_G + AP_E;     // 59 columns of W1
   auto group_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(1 + grp) : "memory"); };
 
-  // ---- once per CTA: TMEM, barrier, weights -> bf16 core-matrix layout, folded bias
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                 ::"r"((uint32_t)__cvta_generic_to_shared(&S.tmem_base)), "r"(AP_TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"((uint32_t)__cvta_generic_to_shared(&S.bar[0])) : "memory");
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"((uint32_t)__cvta_generic_to_shared(&S.bar[1])) : "memory");
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
+  // ---- once per CTA: weights -> bf16 core-matrix layout, folded bias
   for (int i = tid; i < AP_H * AP_K1; i += AP_THREADS) {          // W1[n][k], k < 27 (colour 3 + Fourier 24), zero padded
     const int n = i / AP_K1, k = i - n * AP_K1;
     split_store(&S.W1[0][k >> 3][n >> 3][n & 7][k & 7], &S.W1[1][k >> 3][n >> 3][n & 7][k & 7], k < 3 + AP_G ? W1[n * IN + k] : 0.f);
@@ -174,15 +185,9 @@ appearance_fwd_kernel(int P, int D, const float* __restrict__ features /*[P,16,3
     S.b2[tid] = b2[tid];
     if (tid < 8) S.b3[tid] = tid < 6 ? b3[tid] : 0.f;
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> visible to the MMA's async proxy
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_all = S.tmem_base;
-  const uint32_t tmem = tmem_all + (uint32_t)(grp * 128);                   // this group's 128 accumulator columns
-  const uint32_t tmem_lane = tmem + ((uint32_t)((warp & 3) * 32) << 16);    // a warp reaches the lane quarter warp % 4
-  auto& A = S.A[grp];
-  unsigned long long* bar = &S.bar[grp];
-  uint32_t phase = 0;
+  ApTile& A = S.A[grp];
   const float cx = campos[0], cy = campos[1], cz = campos[2];
 
   const int ntiles = (P + AP_M - 1) / AP_M;
@@ -227,92 +232,39 @@ appearance_fwd_kernel(int P, int D, const float* __restrict__ features /*[P,16,3
         *reinterpret_cast<uint4*>(&A[1][kc][t >> 3][t & 7][0]) = lo;
       }
     }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> visible to the MMA's async proxy
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    group_sync();
-    // ---- layer 1: [128 x 32] x [32 x 128]
-    if (t == 0) {
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-      for (int ks = 0; ks < AP_K1 / 16; ks++) {
-        const uint64_t ah = smem_desc(&A[0][2 * ks][0][0][0], 2048, 128), al = smem_desc(&A[1][2 * ks][0][0][0], 2048, 128);
-        const uint64_t wh = smem_desc(&S.W1[0][2 * ks][0][0][0], 2048, 128), wl = smem_desc(&S.W1[1][2 * ks][0][0][0], 2048, 128);
-        umma_bf16(tmem, ah, wh, instr_desc(AP_M, AP_H), ks > 0);
-        umma_bf16(tmem, ah, wl, instr_desc(AP_M, AP_H), 1);
-        umma_bf16(tmem, al, wh, instr_desc(AP_M, AP_H), 1);
-      }
-      umma_commit(bar);
-    }
-    mbar_wait(bar, phase); phase ^= 1;
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    // ---- h1 = relu(acc + b1') -> A (K = 128)
-#pragma unroll
-    for (int c0 = 0; c0 < AP_H; c0 += 32) {
-      float v[32];
-      tmem_ld32(tmem_lane + c0, v);
-#pragma unroll
-      for (int i = 0; i < 32; i++) v[i] = fmaxf(v[i] + S.b1[c0 + i], 0.f);
-#pragma unroll
-      for (int q = 0; q < 4; q++) {
-        uint4 hi, lo;
-        split8(v + 8 * q, hi, lo);
-        *reinterpret_cast<uint4*>(&A[0][(c0 >> 3) + q][t >> 3][t & 7][0]) = hi;
-        *reinterpret_cast<uint4*>(&A[1][(c0 >> 3) + q][t >> 3][t & 7][0]) = lo;
-      }
-    }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     group_sync();
-    // ---- layer 2: [128 x 128] x [128 x 128]
-    if (t == 0) {
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-      for (int ks = 0; ks < AP_H / 16; ks++) {
-        const uint64_t ah = smem_desc(&A[0][2 * ks][0][0][0], 2048, 128), al = smem_desc(&A[1][2 * ks][0][0][0], 2048, 128);
-        const uint64_t wh = smem_desc(&S.W2[0][2 * ks][0][0][0], 2048, 128), wl = smem_desc(&S.W2[1][2 * ks][0][0][0], 2048, 128);
-        umma_bf16(tmem, ah, wh, instr_desc(AP_M, AP_H), ks > 0);
-        umma_bf16(tmem, ah, wl, instr_desc(AP_M, AP_H), 1);
-        umma_bf16(tmem, al, wh, instr_desc(AP_M, AP_H), 1);
+    // ---- layers 1 and 2: [128 x 32] x [32 x 128], then [128 x 128] x [128 x 128]; h = relu(acc + b) -> A (K = 128).
+    // A half's output rows overwrite only that half's input rows, which its own MMAs have finished reading.
+#pragma unroll 1
+    for (int layer = 0; layer < 2; layer++) {
+#pragma unroll 1
+      for (int half = 0; half < 2; half++) {
+        float acc[64];
+        if (layer == 0)
+          mma_half<AP_H, AP_K1 / 16>(acc, &A[0][0][8 * half][0][0], &A[1][0][8 * half][0][0], &S.W1[0][0][0][0][0], &S.W1[1][0][0][0][0]);
+        else
+          mma_half<AP_H, AP_H / 16>(acc, &A[0][0][8 * half][0][0], &A[1][0][8 * half][0][0], &S.W2[0][0][0][0][0], &S.W2[1][0][0][0][0]);
+        group_sync();      // the whole warpgroup is past its wait before any row of the half is rewritten
+        store_hidden(acc, layer == 0 ? S.b1 : S.b2, A, 64 * half + wrow, lane);
       }
-      umma_commit(bar);
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      group_sync();
     }
-    mbar_wait(bar, phase); phase ^= 1;
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+    // ---- layer 3: [128 x 128] x [128 x 16]; columns 0..7 of row m -> h3[m]
+#pragma unroll 1
+    for (int half = 0; half < 2; half++) {
+      float acc[8];
+      mma_half<AP_N3, AP_H / 16>(acc, &A[0][0][8 * half][0][0], &A[1][0][8 * half][0][0], &S.W3[0][0][0][0][0], &S.W3[1][0][0][0][0]);
 #pragma unroll
-    for (int c0 = 0; c0 < AP_H; c0 += 32) {
-      float v[32];
-      tmem_ld32(tmem_lane + c0, v);
-#pragma unroll
-      for (int i = 0; i < 32; i++) v[i] = fmaxf(v[i] + S.b2[c0 + i], 0.f);
-#pragma unroll
-      for (int q = 0; q < 4; q++) {
-        uint4 hi, lo;
-        split8(v + 8 * q, hi, lo);
-        *reinterpret_cast<uint4*>(&A[0][(c0 >> 3) + q][t >> 3][t & 7][0]) = hi;
-        *reinterpret_cast<uint4*>(&A[1][(c0 >> 3) + q][t >> 3][t & 7][0]) = lo;
-      }
+      for (int r = 0; r < 2; r++)
+        *reinterpret_cast<float2*>(&S.h3[grp][64 * half + wrow + (lane >> 2) + 8 * r][2 * (lane & 3)]) =
+            make_float2(acc[2 * r], acc[2 * r + 1]);
     }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     group_sync();
-    // ---- layer 3: [128 x 128] x [128 x 16]
-    if (t == 0) {
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-      for (int ks = 0; ks < AP_H / 16; ks++) {
-        const uint64_t ah = smem_desc(&A[0][2 * ks][0][0][0], 2048, 128), al = smem_desc(&A[1][2 * ks][0][0][0], 2048, 128);
-        const uint64_t wh = smem_desc(&S.W3[0][2 * ks][0][0][0], 256, 128), wl = smem_desc(&S.W3[1][2 * ks][0][0][0], 256, 128);
-        umma_bf16(tmem, ah, wh, instr_desc(AP_M, AP_N3), ks > 0);
-        umma_bf16(tmem, ah, wl, instr_desc(AP_M, AP_N3), 1);
-        umma_bf16(tmem, al, wh, instr_desc(AP_M, AP_N3), 1);
-      }
-      umma_commit(bar);
-    }
-    mbar_wait(bar, phase); phase ^= 1;
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
     float h[8];
-    tmem_ld8(tmem_lane, h);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");   // the next tile's MMAs overwrite these columns
+#pragma unroll
+    for (int i = 0; i < 8; i++) h[i] = S.h3[grp][t][i];
 
     // ---- tone map + SH evaluation (fp32), scene/gaussian_model.py:60-69, gaussian_renderer/__init__.py:109-117
     float off[3], mul[3];
@@ -351,13 +303,8 @@ appearance_fwd_kernel(int P, int D, const float* __restrict__ features /*[P,16,3
       colors[3 * (size_t)g + 1] = fmaxf(rgb[1] + 0.5f, 0.f);
       colors[3 * (size_t)g + 2] = fmaxf(rgb[2] + 0.5f, 0.f);
     }
-    group_sync();      // every lane has read its accumulator columns and A before the next tile rewrites them
+    group_sync();      // every thread has read h3 and every MMA has finished with A before the next tile rewrites them
   }
-
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0)
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_all), "r"(AP_TMEM_COLS) : "memory");
 }
 
 }  // namespace
@@ -382,11 +329,11 @@ extern "C" int sfgs_appearance_forward(int P, int D, int M, const float* feature
   cudaGetDevice(&dev);
   if (once.first_use() || (dev >= 0 && dev < 64 && sms[dev] == 0)) {
     cudaFuncSetAttribute(appearance_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ApSmem));
-    int n = 148;
+    int n = 132;
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
     if (dev >= 0 && dev < 64) sms[dev] = n;
   }
-  const int nsm = (dev >= 0 && dev < 64 && sms[dev] > 0) ? sms[dev] : 148;
+  const int nsm = (dev >= 0 && dev < 64 && sms[dev] > 0) ? sms[dev] : 132;
   const int ntiles = (P + AP_M - 1) / AP_M;
   const int pairs = (ntiles + AP_GROUPS - 1) / AP_GROUPS;
   const int grid = pairs < nsm ? pairs : nsm;                // persistent: one CTA (two tile groups) per SM

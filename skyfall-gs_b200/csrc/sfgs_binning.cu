@@ -151,7 +151,7 @@ scatter_keys_kernel(const uint4* __restrict__ tmp, const uint2* __restrict__ ran
 // One CTA per tile, two launches over the same grid: a light variant (128 threads x 8 keys, 1024-key window) for
 // the common short lists and a heavy one (256 threads x 16 keys, 4096-key window, global radix fallback beyond
 // that); a CTA whose tile belongs to the other class exits at once.  Lists inside the window are sorted by the
-// shared-memory merge sort below (it replaced a bitonic network: 0.146 -> 0.135 ms on the benchmark frame).
+// shared-memory merge sort below.
 
 // Shared-memory sort buffers hold key i at PADIDX(i): one pad word per 16 keys.  A thread owns VT consecutive keys, so
 // without the pad the 32 lanes of a warp hit the same bank pair on every access (stride VT * 8 bytes = 64 or 128 bytes:
@@ -503,7 +503,7 @@ static void launch_tile_sorts(const GeomLayout& g, const ImageLayout& im, const 
       im.tiles, im.ranges, im.hdr, b.keys, b.point_list, g.rec, im.tiles_x, b.inst_mask);
   // lists beyond the warp class: a persistent grid (three resident CTAs per SM) that returns at once when the frame's
   // longest list (header word written by the scan) is inside the warp class
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   { int v = 0; if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && v > 0) sms = v; }
   const int grid_cta = im.tiles < 3 * sms ? im.tiles : 3 * sms;

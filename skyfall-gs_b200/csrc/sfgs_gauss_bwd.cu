@@ -502,9 +502,8 @@ void sfgs_launch_gauss_bwd(const sfgs_backward_args* a, const GeomLayout& g, flo
       a->scale_modifier, cov3D_ptr, g.rec, a->norm3D_precomp, a->viewmatrix, a->projmatrix, focal_x, focal_y,         \
       a->tan_fovx, a->tan_fovy, a->kernel_size, a->cam_pos, acc, a->dL_dmean2D, a->dL_dconic, a->dL_dopacity,         \
       a->dL_dcolor, a->dL_ddepth, a->dL_dmean3D, a->dL_dcov3D, a->dL_dnorm3D, a->dL_dsh, a->dL_dscale, a->dL_drot
-  // resident CTAs per SM of the SH-writing variant: 5 (96 registers).  Measured on the benchmark frame: 6 / 7 CTAs (80 / 72
-  // registers, 100-180 bytes of spills) take 0.152 / 0.170 ms instead of 0.131, 4 CTAs (127 registers) 0.128 ms; issuing
-  // the first pass's loads before the zero fill (to overlap their round trip with the fill's stores) 0.134 ms.
+  // resident CTAs per SM of the SH-writing variant: 5 (96 registers); 6 / 7 CTAs would cap it at 80 / 72 registers and
+  // spill, 4 CTAs leave fewer warps to hide the gathers.
   if (a->M > 0 && a->dL_dsh != nullptr) {
     gauss_bwd_kernel<true, 5><<<blocks, GB_THREADS, 0, st>>>(GB_ARGS);
   } else {

@@ -28,7 +28,7 @@ struct Sym3 { float c0, c1, c2, c3, c4, c5; };
 __device__ __forceinline__ void rot_from_quat(float r, float x, float y, float z, float R[3][3]) {
   // R[c][k]: column c, row k, same element order as the glm::mat3 constructor call.
   // The products below are pinned with explicit round-to-nearest intrinsics to the exact
-  // mul / fma split the reference's sm_100a binary uses for this block (read off its SASS:
+  // mul / fma split the reference's compiled binary uses for this block (read off its SASS:
   // xy, yz and ry are fused into the add, rz, rx and xz are rounded products), because
   // cov3D feeds the radius and therefore the tile/key indexing that must match bit for bit.
   const float yy = __fmul_rn(y, y), zz = __fmul_rn(z, z);
@@ -140,7 +140,7 @@ __device__ __forceinline__ float4 cov2d_project(float mx, float my, float mz,
 // The clamp flag (colour < 0 before the clamp) is CONTROL FLOW of the backward pass: a colour within an ulp of zero
 // that lands on the other side flips dL/dSH of that channel between 0 and its full value (seen once in a 5M-Gaussian
 // frame while the colour itself only differed by 1e-7).  So this routine is evaluated exactly like the reference's
-// binary evaluates it — every multiply / add / fused multiply-add below is the one in the reference's sm_100a SASS
+// binary evaluates it — every multiply / add / fused multiply-add below is the one in the reference's compiled SASS
 // (read off oracle/_ref, preprocessCUDA<3>, section after the three IEEE divisions of the view direction), pinned
 // with round-to-nearest intrinsics so the compiler cannot contract it differently: colours, and therefore the clamp
 // flags, are bit-identical to the reference (tests: rgb compared bit for bit on every visible Gaussian).

@@ -20,8 +20,8 @@
 //     butterfly per (warp, record) of the first version of this kernel (~45 % fewer issued instructions).
 //     A chunk is filled across staging batches (the record's parameters travel with it), so phase 2 always
 //     runs on 16 records except once at the end of the tile.
-//   combine: each (block, record) pair ends in four red.global.add.v4.f32 (measured: the L2 sustains
-//     ~320 G vector reductions/s, tools/red_bench.cu, so the ~16 M issued per frame hide behind the math):
+//   combine: each (block, record) pair ends in four red.global.add.v4.f32 (tools/red_bench.cu times such traffic on
+//     its own; the ~16 M issued per frame hide behind the math):
 //     ~200x fewer global atomics than the reference and no block-wide barrier besides the staging one.
 #include "sfgs_common.cuh"
 #include <cstdlib>
@@ -359,7 +359,7 @@ render_bwd_kernel(const uint2* __restrict__ ranges, const char* __restrict__ bin
 // Chunks are always full except the last one of a warp.  A record that none of the warp's 32 pixels blends (0.6 % on
 // the benchmark frame: the reach mask is conservative) occupies a slot with zeros.
 // (T is recovered back to front as T_j = T_{j+1} * rcp.approx(1 - alpha_{j+1}).  Refining the reciprocal with a Newton step
-// was measured: +0.008 ms and NO change in the error statistics against the float64 adjudicator — the worst elements are
+// costs time and does NOT change the error statistics against the float64 adjudicator — the worst elements are
 // summation-order noise of ill-conditioned sums, which vary by 5x between runs of either implementation, not T drift.)
 constexpr int W4_CH = 16;
 struct alignas(16) WarpSmem {

@@ -7,7 +7,7 @@
 // tested entry, n_contrib = index of the last applied entry, colour gets
 // T*background, depth/normal/alpha have zero background.
 //
-// B200 mapping: each warp owns an 8x4 pixel block; the tile's sorted Gaussian
+// Mapping: each warp owns an 8x4 pixel block; the tile's sorted Gaussian
 // list is streamed through a 2-stage cp.async ring of packed 64-byte blend
 // records, so the inner loop touches shared memory only (the reference gathers
 // colour/depth/normal from global memory per pixel).  Each record carries the
@@ -41,9 +41,9 @@ __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_gr
 
 // ---- optional TMA staging: one bulk copy (cp.async.bulk, SASS UBLKCP) per 64-byte blend record, completion by
 // mbarrier (each staging warp posts its byte count with one arrive.expect_tx; the phase completes when all eight
-// warps have arrived and all announced bytes have landed).  Measured on B200: parity-green but 5 % SLOWER than the
-// cp.async path (0.322 vs 0.305 ms): UBLKCP is a uniform-datapath instruction, so a warp whose 32 lanes gather 32
-// scattered records issues 32 serialised bulk copies where LDGSTS issues 4 vector instructions.  TMA pays for
+// warps have arrived and all announced bytes have landed).  Parity-green, but a uniform-datapath bulk copy per record
+// means a warp whose 32 lanes gather 32 scattered records issues 32 serialised bulk copies where LDGSTS issues 4
+// vector instructions.  TMA pays for
 // tiles, not for 64-byte gathers — the default stays cp.async; build with -DSFGS_TMA_STAGING=1 to reproduce.
 #ifndef SFGS_TMA_STAGING
 #define SFGS_TMA_STAGING 0

@@ -2,16 +2,17 @@
 //
 // Replaces fusedssim / fusedssim_backward of the reference's fused-ssim submodule (SSIM/ssim.h:7-26; what they
 // compute: 11-tap sigma = 1.5 separable Gaussian window with "same" zero padding, C1/C2 passed by the caller,
-// only img1 differentiable).  The kernels are new, designed around what Blackwell offers for a tile-movement
-// problem of this shape:
+// only img1 differentiable).  The kernels are new, designed around what Hopper offers for a tile-movement problem of
+// this shape:
 //
 //   * the zero-padded (tile + 5-pixel halo) boxes of the input planes are fetched by TMA
 //     (cp.async.bulk.tensor.3d, one elected thread, completion on an mbarrier): the tensor map's out-of-bounds
 //     fill IS the "same" zero padding, so there is no per-pixel bounds test and no address arithmetic on the load
 //     side at all;
-//   * the five windowed moments E[x], E[y], E[x^2], E[y^2], E[xy] are carried as two packed pairs + one scalar and
-//     the window is applied with the sm_100 packed-fp32 instructions (add/mul/fma.f32x2 -> FADD2/FMUL2/FFMA2):
-//     (x, y) and (x^2, y^2) share their filter weight, so 2/5 of the filter arithmetic issues disappear;
+//   * the five windowed moments E[x], E[y], E[x^2], E[y^2], E[xy] are carried as two pairs + one scalar:
+//     (x, y) and (x^2, y^2) share their filter weight, which is loaded once per tap for both lanes of a pair; the
+//     pair arithmetic is written with the round-to-nearest intrinsics, so no multiply is contracted into an add and
+//     every lane is rounded exactly like a separate multiply / add / fused multiply-add;
 //   * 64x32-pixel tiles (1.5x halo read amplification against L2; 2.6x for the reference's 16x16 tiles), the
 //     horizontal pass register-blocked four outputs per thread from 128-bit shared-memory loads, the vertical pass
 //     streaming down 2 columns x 4 rows per thread with the partial sums in registers;
@@ -28,8 +29,8 @@
 namespace {
 
 constexpr int TW = 64, TH = 32, HALO = 5;
-// A TMA box must START on a 16-byte boundary of the row (a box at x0 - 5 raises "illegal instruction"; measured with
-// tools/tma_probe.cu), so the box is fetched from x0 - HX with HX = 8 and is 64 + 2*8 = 80 floats wide: output column c
+// The TMA box starts on a 16-byte boundary of the row (x0 - 8 rather than x0 - 5), so it is fetched from x0 - HX with
+// HX = 8 and is 64 + 2*8 = 80 floats wide: output column c
 // reads box columns c + 3 .. c + 13.  Rows have no such constraint (the box starts at y0 - 5).
 constexpr int HX = 8;
 constexpr int BOX_W = TW + 2 * HX;        // 80 floats = 320 bytes per row
@@ -45,11 +46,12 @@ __constant__ float c_w[11] = {0.001028380123898387f, 0.0075987582094967365f, 0.0
                               0.0075987582094967365f, 0.001028380123898387f};
 
 using u64 = unsigned long long;
-__device__ __forceinline__ u64 pk(float a, float b) { u64 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
-__device__ __forceinline__ void upk(u64 v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) { u64 d; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c)); return d; }
-__device__ __forceinline__ u64 add2(u64 a, u64 b) { u64 d; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-__device__ __forceinline__ u64 mul2(u64 a, u64 b) { u64 d; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
+using f2 = float2;
+__device__ __forceinline__ f2 pk(float a, float b) { return make_float2(a, b); }
+__device__ __forceinline__ void upk(f2 v, float& a, float& b) { a = v.x; b = v.y; }
+__device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ f2 add2(f2 a, f2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ f2 mul2(f2 a, f2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 
 __device__ __forceinline__ void mbar_init(u64* bar, unsigned count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"((unsigned)__cvta_generic_to_shared(bar)), "r"(count) : "memory");
@@ -162,7 +164,7 @@ ssim_fwd_kernel(const __grid_constant__ Maps4 tm, int H, int W, int planes, floa
       X[4 * q] = a.x; X[4 * q + 1] = a.y; X[4 * q + 2] = a.z; X[4 * q + 3] = a.w;
       Y[4 * q] = b.x; Y[4 * q + 1] = b.y; Y[4 * q + 2] = b.z; Y[4 * q + 3] = b.w;
     }
-    u64 P1[14], P2[14];
+    f2 P1[14], P2[14];
     float PXY[14];
 #pragma unroll
     for (int i = 0; i < 14; i++) {
@@ -173,13 +175,13 @@ ssim_fwd_kernel(const __grid_constant__ Maps4 tm, int H, int W, int planes, floa
 #pragma unroll
     for (int j = 0; j < 4; j++) {
       const float wc = c_w[HALO];
-      const u64 wc2 = pk(wc, wc);
-      u64 a1 = mul2(P1[j + HALO], wc2), a2 = mul2(P2[j + HALO], wc2);
+      const f2 wc2 = pk(wc, wc);
+      f2 a1 = mul2(P1[j + HALO], wc2), a2 = mul2(P2[j + HALO], wc2);
       float a5 = PXY[j + HALO] * wc;
 #pragma unroll
       for (int d = 1; d <= HALO; d++) {
         const float w = c_w[HALO - d];
-        const u64 w2 = pk(w, w);
+        const f2 w2 = pk(w, w);
         a1 = fma2(add2(P1[j + HALO - d], P1[j + HALO + d]), w2, a1);
         a2 = fma2(add2(P2[j + HALO - d], P2[j + HALO + d]), w2, a2);
         a5 = fmaf(PXY[j + HALO - d] + PXY[j + HALO + d], w, a5);
@@ -201,24 +203,24 @@ ssim_fwd_kernel(const __grid_constant__ Maps4 tm, int H, int W, int planes, floa
   // ---- vertical pass: 2 columns x 4 output rows per thread, streaming down the 14 rows it needs
   const int cg = t & 31, rg = t >> 5;         // column group (2 columns), row group (4 rows)
   const int lx = 2 * cg, ly = 4 * rg;
-  u64 v1[4][2], v2[4][2];
+  f2 v1[4][2], v2[4][2];
   float v5[4][2];
 #pragma unroll
   for (int r = 0; r < 4; r++)
 #pragma unroll
-    for (int c = 0; c < 2; c++) { v1[r][c] = 0ull; v2[r][c] = 0ull; v5[r][c] = 0.f; }
+    for (int c = 0; c < 2; c++) { v1[r][c] = pk(0.f, 0.f); v2[r][c] = pk(0.f, 0.f); v5[r][c] = 0.f; }
 #pragma unroll
   for (int i = 0; i < 14; i++) {              // box row ly + i feeds output row ly + r with weight c_w[i - r]
     const float4 a = *reinterpret_cast<const float4*>(&S.h12[ly + i][lx]);
     const float4 b = *reinterpret_cast<const float4*>(&S.h34[ly + i][lx]);
     const float2 c5 = *reinterpret_cast<const float2*>(&S.h5[ly + i][lx]);
-    const u64 a0 = pk(a.x, a.y), a1 = pk(a.z, a.w), b0 = pk(b.x, b.y), b1 = pk(b.z, b.w);
+    const f2 a0 = pk(a.x, a.y), a1 = pk(a.z, a.w), b0 = pk(b.x, b.y), b1 = pk(b.z, b.w);
 #pragma unroll
     for (int r = 0; r < 4; r++) {
       const int k = i - r;
       if (k >= 0 && k <= 10) {
         const float w = c_w[k];
-        const u64 w2 = pk(w, w);
+        const f2 w2 = pk(w, w);
         v1[r][0] = fma2(a0, w2, v1[r][0]); v1[r][1] = fma2(a1, w2, v1[r][1]);
         v2[r][0] = fma2(b0, w2, v2[r][0]); v2[r][1] = fma2(b1, w2, v2[r][1]);
         v5[r][0] = fmaf(c5.x, w, v5[r][0]); v5[r][1] = fmaf(c5.y, w, v5[r][1]);
@@ -336,7 +338,7 @@ ssim_bwd_kernel(const __grid_constant__ Maps4 tm, int H, int W, int planes, cons
 
   for (int u = t; u < BOX_H * (TW / 4); u += SSIM_THREADS) {
     const int row = u >> 4, xg = u & 15;
-    u64 P[14];
+    f2 P[14];
     float Q[14];
 #pragma unroll
     for (int q = 0; q < 5; q++) {             // box columns 4xg .. 4xg+19, of which 4xg+3 .. 4xg+16 are used
@@ -357,7 +359,7 @@ ssim_bwd_kernel(const __grid_constant__ Maps4 tm, int H, int W, int planes, cons
 #pragma unroll
     for (int j = 0; j < 4; j++) {
       const float wc = c_w[HALO];
-      u64 a1 = mul2(P[j + HALO], pk(wc, wc));
+      f2 a1 = mul2(P[j + HALO], pk(wc, wc));
       float a2 = Q[j + HALO] * wc;
 #pragma unroll
       for (int d = 1; d <= HALO; d++) {
@@ -378,23 +380,23 @@ ssim_bwd_kernel(const __grid_constant__ Maps4 tm, int H, int W, int planes, cons
 
   const int cg = t & 31, rg = t >> 5;
   const int lx = 2 * cg, ly = 4 * rg;
-  u64 v01[4][2];
+  f2 v01[4][2];
   float v2[4][2];
 #pragma unroll
   for (int r = 0; r < 4; r++)
 #pragma unroll
-    for (int c = 0; c < 2; c++) { v01[r][c] = 0ull; v2[r][c] = 0.f; }
+    for (int c = 0; c < 2; c++) { v01[r][c] = pk(0.f, 0.f); v2[r][c] = 0.f; }
 #pragma unroll
   for (int i = 0; i < 14; i++) {
     const float4 a = *reinterpret_cast<const float4*>(&S.h01[ly + i][lx]);
     const float2 c2 = *reinterpret_cast<const float2*>(&S.h2[ly + i][lx]);
-    const u64 a0 = pk(a.x, a.y), a1 = pk(a.z, a.w);
+    const f2 a0 = pk(a.x, a.y), a1 = pk(a.z, a.w);
 #pragma unroll
     for (int r = 0; r < 4; r++) {
       const int k = i - r;
       if (k >= 0 && k <= 10) {
         const float w = c_w[k];
-        const u64 w2 = pk(w, w);
+        const f2 w2 = pk(w, w);
         v01[r][0] = fma2(a0, w2, v01[r][0]); v01[r][1] = fma2(a1, w2, v01[r][1]);
         v2[r][0] = fmaf(c2.x, w, v2[r][0]); v2[r][1] = fmaf(c2.y, w, v2[r][1]);
       }
@@ -461,8 +463,8 @@ int sm_count() {
   static int n[64] = {0};
   int dev = 0;
   cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64) return 148;
-  if (n[dev] == 0) { int v = 148; cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev); n[dev] = v > 0 ? v : 148; }
+  if (dev < 0 || dev >= 64) return 132;
+  if (n[dev] == 0) { int v = 132; cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev); n[dev] = v > 0 ? v : 132; }
   return n[dev];
 }
 

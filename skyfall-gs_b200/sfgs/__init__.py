@@ -1,4 +1,4 @@
-"""sfgs — Python host side of the B200-native splat rasterizer.
+"""sfgs — Python host side of the H100-native splat rasterizer.
 
 `sfgs.native` binds the C ABI (include/sfgs.h) with ctypes; `sfgs.rasterizer`
 implements, on top of it, the three functions of the reference's pybind module

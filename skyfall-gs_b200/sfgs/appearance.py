@@ -9,7 +9,7 @@ replaces, in gaussian_renderer/__init__.py:105-118,
     dir_pp_normalized = ...; colors_toned = eval_sh(pc.active_sh_degree, colors_toned, dir_pp_normalized)
     colors_precomp = torch.clamp_min(colors_toned + 0.5, 0.0)
 
-Forward: one tcgen05 tensor-core kernel (csrc/sfgs_appearance.cu, `sfgs_appearance_forward`).  Backward: not fused yet —
+Forward: one wgmma tensor-core kernel (csrc/sfgs_appearance.cu, `sfgs_appearance_forward`).  Backward: not fused yet —
 the autograd function recomputes the same expression with torch ops (`reference_colors`, float32) and differentiates
 that, so gradients are those of the torch formulation; the fused forward pays off for evaluation / video renders
 (render_video.py, metrics) and halves the appearance cost of a training step.

@@ -18,7 +18,7 @@ scripts/run_jax.py:52-87).  Design:
   alternative.
 
 The host logic (partitioning, padded gather/assembly, reduction) is backend-agnostic and covered by
-world-size-2 gloo tests on CPU tensors; on B200s the backend is NCCL over NVLink/NVSwitch.
+world-size-2 gloo tests on CPU tensors; on H100s the backend is NCCL over NVLink/NVSwitch.
 """
 from __future__ import annotations
 

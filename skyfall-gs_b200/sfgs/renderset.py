@@ -5,7 +5,7 @@ targets x 6 orbit cameras x 2 samples, 1024 x 1024; train.py:360-525, utils/came
 arguments/__init__.py:232-256) before each view goes through FlowEdit and MoGe.  The views are independent, so the set
 shards by VIEW: every rank holds the scene, renders a contiguous share of the views (forward only, fused normal
 normalisation), and only the results — 8-bit colour and float depth — are gathered on rank 0.  There is no exchange
-inside a frame; the single collective is the gather of finished images (backend-agnostic: NCCL on the B200s, gloo in the
+inside a frame; the single collective is the gather of finished images (backend-agnostic: NCCL on the H100s, gloo in the
 CPU tests).  The diffusion / depth models themselves are out of scope (no weights, no network).
 """
 from __future__ import annotations

@@ -1,4 +1,4 @@
-"""Generate tests/golden/*.npz from the UNMODIFIED reference CUDA rasterizer (oracle/_ref) on a B200.
+"""Generate tests/golden/*.npz from the UNMODIFIED reference CUDA rasterizer (oracle/_ref) on a GPU.
 
 Run on the GPU box (the reference cannot execute in the CPU-only container):
     gpurun -- 'python tests/golden/make_golden.py gpurun_out/golden'

@@ -1,6 +1,9 @@
 """Shared helpers for the parity tests (test infrastructure)."""
 from __future__ import annotations
 
+import hashlib
+import os
+
 import numpy as np
 import torch
 
@@ -120,7 +123,7 @@ ADJ_FLOOR = 1e-5      # north_star: 1e-5 abs on gradient tensors
 
 
 def adjudicate_gradients(d, cam, sh_degree, bg, I, out_alpha, radii, cot, ours, ref, tag, kernel_size=0.1,
-                         scale_modifier=1.0, colors=None, factors=None, floor=ADJ_FLOOR):
+                         scale_modifier=1.0, colors=None, factors=None, floor=ADJ_FLOOR, ref_stats=None):
     """The gradient gate of the parity tests.
 
     The reference's backward is itself an approximation (float atomics in a run-dependent order, transmittance
@@ -134,9 +137,8 @@ def adjudicate_gradients(d, cam, sh_degree, bg, I, out_alpha, radii, cot, ours, 
     ref: one run of the reference's gradients, or a list of runs (every statistic: the largest over the runs).
     ours: one run of this library's gradients, or a list of runs (mean / p99.9: the largest over the runs; the worst
     element: the median over the runs — see oracle.adjudicator.error_report).
-    Returns the report (also appended to gpurun_out/adjudication.jsonl when that directory exists)."""
-    import json
-    import os
+    ref_stats: instead of `ref`, the reference build's statistics per tensor as stored by RefFacts.adjudicate.
+    Returns the report."""
     from oracle import adjudicator as A
     factors = factors or ADJ_FACTORS
     f64 = A.backward_f64(I, d["means3D"], radii, d["shs"], d["scales"], d["rotations"], scale_modifier,
@@ -144,11 +146,10 @@ def adjudicate_gradients(d, cam, sh_degree, bg, I, out_alpha, radii, cot, ours, 
                          sh_degree, bg, out_alpha, cot, colors_precomp=colors)
     keys = [k for k in A.GRAD_KEYS if not (colors is not None and k == "sh")]
     rep = A.error_report(ours, ref, f64, keys)
+    if ref_stats is not None:
+        for k in rep:
+            rep[k]["ref"] = ref_stats[k]
     print(f"\n[adjudication] {tag}\n" + A.format_report(rep))
-    out_dir = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out")
-    if os.path.isdir(out_dir):
-        with open(os.path.join(out_dir, "adjudication.jsonl"), "a") as fh:
-            fh.write(json.dumps({"case": tag, "report": rep}) + "\n")
     failures = []
     for k, r in rep.items():
         for stat, factor in factors.items():
@@ -157,3 +158,100 @@ def adjudicate_gradients(d, cam, sh_degree, bg, I, out_alpha, radii, cot, ours, 
                 failures.append(f"{k}.{stat}: ours {r['ours'][stat]:.3e} > {factor} x ref {r['ref'][stat]:.3e} + {floor}")
     assert not failures, f"{tag}: " + "; ".join(failures)
     return rep
+
+
+# ----------------------------------------------------------------------------- recorded reference facts
+REF_FACTS_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference")
+SAMPLE = 8192          # elements of a tolerance-compared tensor kept per fact
+
+
+def _canon(t):
+    """Bytes that identify a tensor's values exactly: float32 as their bit patterns, everything widened to int64."""
+    t = t.detach().contiguous()
+    if t.dtype.is_floating_point:
+        t = t.float().view(torch.int32)
+    return t.to(torch.int64).cpu().numpy().tobytes() + str(tuple(t.shape)).encode()
+
+
+def _sample_index(n, name):
+    seed = int.from_bytes(hashlib.sha256(name.encode()).digest()[:8], "little")
+    return np.sort(np.random.default_rng(seed).choice(n, size=min(n, SAMPLE), replace=False))
+
+
+class RefFacts:
+    """What a parity test compares against the original rasterizer, kept small enough to live in the repository.
+
+    Live (the original's CUDA build is in oracle/_ref): every comparison runs against the original's values, and with
+    SFGS_RECORD_REFERENCE=1 what it compared against is stored in tests/golden/reference/<tag>.npz.  Replay (no
+    original build): the stored facts stand in for it.  A quantity compared bit for bit is stored as the SHA-256 digest
+    of its values, so replay still compares it bit for bit; a quantity compared within a tolerance as its values at a
+    fixed seeded sample of elements; a scalar as itself; a gradient comparison as the original build's error
+    statistics against the float64 adjudicator (helpers.adjudicate_gradients)."""
+
+    def __init__(self, tag, live=None):
+        from oracle import ref_cuda
+        self.tag = tag
+        self.path = os.path.join(REF_FACTS_DIR, tag + ".npz")
+        self.live = ref_cuda.available() if live is None else live
+        self.record = self.live and os.environ.get("SFGS_RECORD_REFERENCE") == "1"
+        self.facts = {}
+        if not self.live:
+            assert os.path.exists(self.path), f"no recorded reference facts for {tag} ({self.path})"
+            with np.load(self.path) as z:
+                self.facts = {k: z[k] for k in z.files}
+
+    def _put(self, key, value):
+        if self.record:
+            self.facts[key] = np.asarray(value)
+            os.makedirs(REF_FACTS_DIR, exist_ok=True)
+            np.savez_compressed(self.path, **self.facts)
+
+    def value(self, name, fn):
+        """A number of the original's run: computed by `fn` when live, else the stored one."""
+        if self.live:
+            v = fn()
+            self._put("value/" + name, v)
+            return v
+        return self.facts["value/" + name].item()
+
+    def same(self, name, ours, ref_fn):
+        """`ours` equals the original's tensor bit for bit."""
+        if self.live:
+            ref = ref_fn()
+            ok = _canon(ours) == _canon(ref)
+            self._put("same/" + name, hashlib.sha256(_canon(ref)).hexdigest())
+        else:
+            ok = hashlib.sha256(_canon(ours)).hexdigest() == str(self.facts["same/" + name])
+        assert ok, f"{self.tag}: {name} differs from the original"
+
+    def close(self, name, ours, ref_fn, atol, rtol=0.0):
+        """|ours - original| <= atol + rtol |original| (every element live; the stored sample on replay)."""
+        o = ours.detach().reshape(-1).double()
+        idx = _sample_index(o.numel(), self.tag + "/" + name)
+        if self.live:
+            ref = ref_fn().detach().reshape(-1).double()
+            self._put("close/" + name, ref[torch.from_numpy(idx).to(ref.device)].float().cpu().numpy())
+        else:
+            ref = torch.from_numpy(self.facts["close/" + name]).to(o.device)
+            o = o[torch.from_numpy(idx).to(o.device)]
+        err = float(((o - ref).abs() - rtol * ref.abs()).max()) if o.numel() else 0.0
+        assert err <= atol, (self.tag, name, err, atol)
+
+    def adjudicate(self, d, cam, sh_degree, bg, I_ours, out_alpha, radii, cot, ours, ref_fn, tag, **kw):
+        """helpers.adjudicate_gradients against the original's gradient runs (`ref_fn` returns (internals, out_alpha,
+        radii, list of runs)) when live; against its stored error statistics, on this library's forward intermediates
+        (asserted bit-identical on indexing by the caller), on replay."""
+        if self.live:
+            I, alpha, rad, runs = ref_fn()
+            rep = adjudicate_gradients(d, cam, sh_degree, bg, I, alpha, rad, cot, ours, runs, tag, **kw)
+            for k, r in rep.items():
+                for stat, v in r["ref"].items():
+                    self._put(f"adj/{k}/{stat}", v)
+            return rep
+        stats = {}
+        for key, v in self.facts.items():
+            if key.startswith("adj/"):
+                _, k, stat = key.split("/")
+                stats.setdefault(k, {})[stat] = float(v)
+        return adjudicate_gradients(d, cam, sh_degree, bg, I_ours, out_alpha, radii, cot, ours, None, tag,
+                                    ref_stats=stats, **kw)

@@ -3,7 +3,7 @@
 Golden vectors: tests/golden/appearance_ref.npz, produced by the reference's OWN EmbeddingModel and eval_sh
 (tests/golden/make_appearance_golden.py, float32 and float64).
   * CPU: the torch formulation in sfgs/appearance.py (used for the backward pass) equals the reference modules' output;
-  * GPU: the tcgen05 kernel equals it within the stated bf16 tolerance, for every SH degree, ragged P, and the
+  * GPU: the wgmma kernel equals it within the stated bf16 tolerance, for every SH degree, ragged P, and the
     gradients of the autograd wrapper are those of the torch formulation.
 """
 import os

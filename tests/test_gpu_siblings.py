@@ -5,6 +5,8 @@ import numpy as np
 import pytest
 import torch
 
+import helpers as Hh
+
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
@@ -69,10 +71,10 @@ def test_dist_cuda2_matches_bruteforce_and_reference(cuda_device):
         want = knn_oracle.dist2_knn3(pts)
         assert np.allclose(got, want, rtol=2e-6, atol=1e-12), name
     from oracle import ref_cuda
-    if ref_cuda.available():
-        pts = torch.from_numpy(clouds["uniform"].astype(np.float32)).to(dev)
-        # same 3-NN set; the squared distance may contract differently (1 ulp)
-        assert torch.allclose(distCUDA2(pts), ref_cuda.knn(pts), rtol=1e-6, atol=0)
+    F = Hh.RefFacts("dist_cuda2")
+    pts = torch.from_numpy(clouds["uniform"].astype(np.float32)).to(dev)
+    # same 3-NN set; the squared distance may contract differently (1 ulp)
+    F.close("uniform", distCUDA2(pts), lambda: ref_cuda.knn(pts), atol=0.0, rtol=1e-6)
 
 
 def test_expf_replica_is_bit_exact(cuda_device):
@@ -103,9 +105,7 @@ def test_expf_replica_is_bit_exact(cuda_device):
 
 def _ref_fused_ssim():
     from oracle import build_ref_torch
-    if not build_ref_torch.built():
-        pytest.skip("oracle/_ref torch extensions not built")
-    return build_ref_torch.import_reference_packages()[1]
+    return build_ref_torch.import_reference_packages()[1] if build_ref_torch.built() else None
 
 
 @pytest.mark.parametrize("shape", [(5, 5, 1080, 1920), (1, 3, 1080, 1920), (2, 3, 270, 333), (1, 1, 17, 19), (1, 2, 64, 4),
@@ -116,40 +116,52 @@ def test_fused_ssim_against_the_reference_cuda_kernel(cuda_device, shape):
     the training shape and on sizes that are off the tile grid, odd, narrower than a tile or not 16-byte rows (the
     non-TMA load path).  The reference kernel is compiled with --use_fast_math (approximate divisions): the map agrees
     within 1e-5 (the image tolerance of the north star), and for the end-to-end value and gradient a float64 torch
-    evaluation decides whose error a deviation is (ours <= 2x the reference kernel's)."""
+    evaluation decides whose error a deviation is (ours <= 2x the reference kernel's).  Where the reference's build is
+    absent, what a run on an H100 recorded stands in for it (helpers.RefFacts); the backward kernel alone, fed the
+    reference's derivative maps, is then not compared (the maps themselves and the end-to-end gradient are)."""
     ref = _ref_fused_ssim()
+    F = Hh.RefFacts("fused_ssim_" + "x".join(str(n) for n in shape), live=ref is not None)
     from fused_ssim import fused_ssim, fusedssim, fusedssim_backward
     dev = cuda_device
     g = torch.Generator(device="cpu").manual_seed(sum(shape))
     a = torch.rand(shape, generator=g).to(dev)
     b = (a + 0.2 * torch.randn(shape, generator=g).to(dev)).clamp(0, 1) if shape[2] > 20 else torch.rand(shape, generator=g).to(dev)
     C1, C2 = 0.01 ** 2, 0.03 ** 2
-    m0, d0, e0, f0 = ref.fusedssim(C1, C2, a, b, True)
+    r = ref.fusedssim(C1, C2, a, b, True) if F.live else None
     m1, d1, e1, f1 = fusedssim(C1, C2, a, b, True)
     # the value map is O(1); the derivative maps reach ~1/C2 and dm_dmu1 is a difference of terms far larger than the
     # result (the reference sums four of them with approximate divisions), so they are compared relative to the
     # largest magnitude in the tensor
-    for name, x, y, rel in (("ssim_map", m1, m0, 1e-5), ("dm_dmu1", d1, d0, 2e-5), ("dm_dsigma1_sq", e1, e0, 2e-5),
-                            ("dm_dsigma12", f1, f0, 2e-5)):
-        tol = rel * max(1.0, float(y.abs().max()))
-        assert float((x - y).abs().max()) <= tol, (name, float((x - y).abs().max()), tol)
+    for i, (name, x, rel) in enumerate((("ssim_map", m1, 1e-5), ("dm_dmu1", d1, 2e-5), ("dm_dsigma1_sq", e1, 2e-5),
+                                        ("dm_dsigma12", f1, 2e-5))):
+        tol = rel * max(1.0, F.value(name + "_absmax", lambda: float(r[i].abs().max())))
+        F.close(name, x, lambda: r[i], tol)
     dL = torch.randn(shape, generator=g).to(dev)
-    g0 = ref.fusedssim_backward(C1, C2, a, b, dL, d0, e0, f0)
-    g1 = fusedssim_backward(C1, C2, a, b, dL, d0, e0, f0)         # same derivative maps in: isolates the backward kernel
-    assert float((g1 - g0).abs().max()) <= 2e-6 * max(1.0, float(g0.abs().max()))
+    if F.live:
+        m0, d0, e0, f0 = r
+        g0 = ref.fusedssim_backward(C1, C2, a, b, dL, d0, e0, f0)
+        g1 = fusedssim_backward(C1, C2, a, b, dL, d0, e0, f0)         # same derivative maps in: isolates the backward kernel
+        assert float((g1 - g0).abs().max()) <= 2e-6 * max(1.0, float(g0.abs().max()))
+        del r, m0, d0, e0, f0, g0, g1
     # the public entry point end to end; whose error a deviation is, is decided by a float64 torch evaluation
     x0, x1 = a.clone().requires_grad_(True), a.clone().requires_grad_(True)
-    v0, v1 = ref.fused_ssim(x0, b), fused_ssim(x1, b)
-    v0.backward(); v1.backward()
-    assert abs(v0.item() - v1.item()) < 2e-6
+    v1 = fused_ssim(x1, b)
+    v1.backward()
+    if F.live:
+        v0 = ref.fused_ssim(x0, b)
+        v0.backward()
+    v0_item = F.value("value", lambda: v0.item())
+    assert abs(v0_item - v1.item()) < 2e-6
     if a.numel() <= 20_000_000:
         xd = a.double().requires_grad_(True)
         vd = torch_ssim_map(xd, b.double()).mean()
         vd.backward()
-        e_ours, e_ref = float((x1.grad.double() - xd.grad).abs().max()), float((x0.grad.double() - xd.grad).abs().max())
-        assert abs(v1.item() - vd.item()) <= 2 * abs(v0.item() - vd.item()) + 1e-6
+        e_ours = float((x1.grad.double() - xd.grad).abs().max())
+        e_ref = F.value("grad_err_vs_f64", lambda: float((x0.grad.double() - xd.grad).abs().max()))
+        assert abs(v1.item() - vd.item()) <= 2 * abs(v0_item - vd.item()) + 1e-6
         assert e_ours <= 2 * e_ref + 1e-9 * float(xd.grad.abs().max()) + 1e-12, (e_ours, e_ref)
     else:
-        assert float((x0.grad - x1.grad).abs().max()) <= 2e-5 * float(x0.grad.abs().max()) + 1e-12
+        F.close("grad", x1.grad, lambda: x0.grad, 2e-5 * F.value("grad_absmax", lambda: float(x0.grad.abs().max())) + 1e-12)
     if shape[2] > 10 and shape[3] > 10:
-        assert abs(ref.fused_ssim(a, b, padding="valid", train=False).item() - fused_ssim(a, b, padding="valid", train=False).item()) < 2e-6
+        v_valid = F.value("value_valid", lambda: ref.fused_ssim(a, b, padding="valid", train=False).item())
+        assert abs(v_valid - fused_ssim(a, b, padding="valid", train=False).item()) < 2e-6

@@ -1,6 +1,6 @@
 """Pin the CPU oracle (oracle/sfgs_oracle.c) against the UNMODIFIED reference CUDA rasterizer.
 
-tests/golden/ref_*.npz were produced on a B200 by the reference's own code (oracle/_ref, built from
+tests/golden/ref_*.npz were produced by the reference's own code (oracle/_ref, built from
 /root/reference by oracle/build_ref.py) with tests/golden/make_golden.py.  No GPU is needed here."""
 import os
 

@@ -1,11 +1,12 @@
 """SURVEY.md §8 row a1 / §8b: the reference's OWN caller runs unmodified on the drop-in packages.
 
 `gaussian_renderer.render()` (gaussian_renderer/__init__.py:19-164) and `scene.gaussian_model.GaussianModel`
-(scene/gaussian_model.py) are imported from /root/reference as they are — nothing is copied or edited — with
+(scene/gaussian_model.py) are imported from the original project's tree ($SFGS_REFERENCE) as they are — nothing is
+copied or edited — with
 `skyfall-gs_b200/` on sys.path so that `from diff_gauss import ...` (gaussian_renderer/__init__.py:14) and
 `from simple_knn._C import distCUDA2` (scene/gaussian_model.py:25) resolve to this repository's packages.
 
-There is no GPU in this container, so the native layer below the pybind boundary (`diff_gauss._C`, i.e.
+The test needs no GPU: the native layer below the pybind boundary (`diff_gauss._C`, i.e.
 sfgs.rasterizer over libsfgs.so) is replaced by a RECORDING FAKE that
   * checks every positional argument of `rasterize_gaussians` / `rasterize_gaussians_backward` for position, python
     type, dtype and shape against the reference's binding (RAST/rasterize_points.h:17-73, .cu:35-243), and
@@ -16,9 +17,9 @@ opacity / scale, rotation normalise, appearance MLP), this repository's `diff_ga
 reference's `add_densification_stats`, which consumes `viewspace_points.grad` (scene/gaussian_model.py:744-749).
 
 The test fails if any name, argument order, default, dtype or return arity drifts from what
-gaussian_renderer/__init__.py:132-140 and the reference's diff_gauss/__init__.py expect.  (/root/reference does not
-exist on the GPU box, so there the same call sequence runs on the real kernels as a restatement:
-tests/test_gpu_parity.py::test_training_loop_with_all_three_ops.)
+gaussian_renderer/__init__.py:132-140 and the reference's diff_gauss/__init__.py expect.  Where the original tree is
+absent the tests skip; the same call sequence runs on the real kernels as a restatement in
+tests/test_gpu_parity.py::test_training_loop_with_all_three_ops.
 """
 import os
 import sys
@@ -31,12 +32,12 @@ REF = os.environ.get("SFGS_REFERENCE", "/root/reference")
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PKG = os.path.join(ROOT, "skyfall-gs_b200")
 
-pytestmark = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "gaussian_renderer")),
-                                reason="the reference tree is only present in the build container")
+needs_reference = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "gaussian_renderer")),
+                                     reason="the original project's source tree ($SFGS_REFERENCE) is not present")
 
 
 class _CudaToCpu(torch.overrides.TorchFunctionMode):
-    """Redirect explicit CUDA placements of the reference code to the CPU (no GPU in this container)."""
+    """Redirect explicit CUDA placements of the reference code to the CPU (the test runs without a GPU)."""
 
     @staticmethod
     def _fix(v):
@@ -191,6 +192,7 @@ def _camera(W=80, H=48):
                                  camera_center=torch.from_numpy(c.campos), uid=1)
 
 
+@needs_reference
 @pytest.mark.parametrize("appearance", [False, True])
 def test_reference_render_and_model_run_unmodified_on_the_dropin(reference_stack, appearance):
     render, GaussianModel, rec = reference_stack
@@ -234,6 +236,7 @@ def test_reference_render_and_model_run_unmodified_on_the_dropin(reference_stack
     assert torch.allclose(pc.xyz_gradient_accum_abs[vis], vsp.grad[vis, 2:].norm(dim=-1, keepdim=True))
 
 
+@needs_reference
 def test_reference_callers_of_the_sibling_ops_resolve_to_the_dropins(reference_stack):
     """train.py:42 `from fused_ssim import fused_ssim` and scene/gaussian_model.py:25 `from simple_knn._C import distCUDA2`."""
     import fused_ssim
