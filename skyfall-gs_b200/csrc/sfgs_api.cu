@@ -338,6 +338,7 @@ int sfgs_rasterize_backward(const sfgs_backward_args* a) {
     return fail(SFGS_E_BADARG, "backward: null output");
   if (do_gauss && !a->radii) return fail(SFGS_E_BADARG, "backward: radii missing");
   if (do_gauss && a->M > 0 && a->shs && !a->dL_dsh) return fail(SFGS_E_BADARG, "backward: dL_dsh missing");
+  if (a->ED < 0 || a->ED > SFGS_MAX_EXTRA) return fail(SFGS_E_BADARG, "backward: ED out of range");
   // extra-attribute gradients are accumulated by the blend stage only and are never exchanged between ranks: the
   // two-phase (multi-GPU) form would return them partial or uninitialised
   if (a->ED > 0 && phase != 0) return fail(SFGS_E_UNSUPPORTED, "backward: extra_attrs are not supported by the two-phase backward");

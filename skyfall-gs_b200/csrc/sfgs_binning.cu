@@ -107,24 +107,24 @@ tile_scan_kernel(int tiles, const uint32_t* __restrict__ tile_count, uint2* __re
 // (depth, id) is unique inside a tile, so the order is the order of depth_bits << 32 | id.  The sort kernels then touch
 // no Gaussian data at all; round 1/2a gathered 56 MB of records inside the sort CTAs to form the masks there.
 // With P >= 2^24 the key stays depth_bits << 32 | id and the sort kernels compute the masks as before.
-// SCATTER_ITEMS: instances per thread (independent loads in flight).  With the mask the kernel needs ~36 live floats per
-// instance in flight: one instance per thread keeps it at 60 registers (four CTAs per SM).
-template <bool PACK, int SCATTER_ITEMS>
+// ITEMS: instances per thread (independent loads in flight).  With the mask the kernel needs ~36 live floats per
+// instance in flight, so the packed path runs two per thread; the unpacked path forms no mask and runs four.
+template <bool PACK, int ITEMS>
 __global__ void __launch_bounds__(256)
 scatter_keys_kernel(const uint4* __restrict__ tmp, const uint2* __restrict__ ranges, uint32_t* __restrict__ tile_count,
                     const uint32_t* __restrict__ hdr, const float* __restrict__ rec, int gx, uint64_t* __restrict__ keys) {
   if (hdr[HDR_OVERFLOW]) return;
   const uint32_t R = hdr[HDR_R];
-  const uint32_t i0 = blockIdx.x * (256u * SCATTER_ITEMS) + threadIdx.x;
-  uint4 t[SCATTER_ITEMS];
-  uint32_t start[SCATTER_ITEMS], slot[SCATTER_ITEMS];
-  float4 r0[SCATTER_ITEMS];
-  float2 r1[SCATTER_ITEMS];
+  const uint32_t i0 = blockIdx.x * (256u * ITEMS) + threadIdx.x;
+  uint4 t[ITEMS];
+  uint32_t start[ITEMS], slot[ITEMS];
+  float4 r0[ITEMS];
+  float2 r1[ITEMS];
 #pragma unroll
-  for (int u = 0; u < SCATTER_ITEMS; u++)
+  for (int u = 0; u < ITEMS; u++)
     if (i0 + 256u * u < R) t[u] = tmp[i0 + 256u * u];
 #pragma unroll
-  for (int u = 0; u < SCATTER_ITEMS; u++)
+  for (int u = 0; u < ITEMS; u++)
     if (i0 + 256u * u < R) {
       // the slot inside the tile bucket: the histogram the preprocess built is counted back down (any order will do,
       // the bucket is sorted next); the returning atomic is in flight while the reach mask is formed
@@ -136,7 +136,7 @@ scatter_keys_kernel(const uint4* __restrict__ tmp, const uint2* __restrict__ ran
       }
     }
 #pragma unroll
-  for (int u = 0; u < SCATTER_ITEMS; u++)
+  for (int u = 0; u < ITEMS; u++)
     if (i0 + 256u * u < R) {
       uint32_t lo = t[u].x;
       if (PACK) {
@@ -482,13 +482,9 @@ void sfgs_launch_scatter(const GeomLayout& g, const ImageLayout& im, const Binni
                          unsigned long long capacity, cudaStream_t st) {
   SFGS_COUNT_LAUNCH();
   if (capacity == 0) return;
-  // instances per thread of the mask-forming scatter (default 2; SFGS_SCATTER_ITEMS=1|2|4 for A/B measurements)
-  static const int items = [] { const char* e = getenv("SFGS_SCATTER_ITEMS"); return e ? atoi(e) : 2; }();
   auto blocks_for = [&](int it) { return (unsigned)((capacity + 256ull * it - 1) / (256ull * it)); };
-  if (!sfgs_keys_packed(P)) scatter_keys_kernel<false, 4><<<blocks_for(4), 256, 0, st>>>(b.tmp, im.ranges, im.tile_count, im.hdr, g.rec, im.tiles_x, b.keys);
-  else if (items == 4) scatter_keys_kernel<true, 4><<<blocks_for(4), 256, 0, st>>>(b.tmp, im.ranges, im.tile_count, im.hdr, g.rec, im.tiles_x, b.keys);
-  else if (items == 2) scatter_keys_kernel<true, 2><<<blocks_for(2), 256, 0, st>>>(b.tmp, im.ranges, im.tile_count, im.hdr, g.rec, im.tiles_x, b.keys);
-  else scatter_keys_kernel<true, 1><<<blocks_for(1), 256, 0, st>>>(b.tmp, im.ranges, im.tile_count, im.hdr, g.rec, im.tiles_x, b.keys);
+  if (sfgs_keys_packed(P)) scatter_keys_kernel<true, 2><<<blocks_for(2), 256, 0, st>>>(b.tmp, im.ranges, im.tile_count, im.hdr, g.rec, im.tiles_x, b.keys);
+  else scatter_keys_kernel<false, 4><<<blocks_for(4), 256, 0, st>>>(b.tmp, im.ranges, im.tile_count, im.hdr, g.rec, im.tiles_x, b.keys);
 }
 
 template <bool PACK>

@@ -22,7 +22,6 @@
 // tensor map; they take the same kernels with a cooperative bounds-checked tile load instead of TMA.
 #include <cuda.h>
 #include <cudaTypedefs.h>
-#include <cstdlib>
 #include <mutex>
 #include "sfgs_common.cuh"
 
@@ -453,11 +452,7 @@ bool make_map(CUtensorMap* m, const float* base, int planes, int H, int W) {
             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-bool tma_enabled() {   // SFGS_SSIM_TMA=0 forces the cooperative tile load (debugging / A-B timing)
-  static const bool on = [] { const char* e = getenv("SFGS_SSIM_TMA"); return !(e && e[0] == '0'); }();
-  return on;
-}
-bool tma_ok(const void* p, int W) { return tma_enabled() && (W % 4) == 0 && (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+bool tma_ok(const void* p, int W) { return (W % 4) == 0 && (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 int sm_count() {
   static int n[64] = {0};

@@ -17,27 +17,31 @@ def to_torch(scene: S.Scene, cam: S.Camera, device):
                 projmatrix=t(cam.projmatrix), campos=t(cam.campos))
 
 
-def run_ours_forward(d, cam, sh_degree, bg, kernel_size=0.1, scale_modifier=1.0, colors=None, debug=False):
+def run_ours_forward(d, cam, sh_degree, bg, kernel_size=0.1, scale_modifier=1.0, colors=None, debug=False,
+                     extras=None):
     from sfgs import rasterizer as R
     e = torch.empty(0, device=d["means3D"].device)
     sh = e if colors is not None else d["shs"]
     col = colors if colors is not None else e
+    ex, ED = (extras, int(extras.shape[1])) if extras is not None else (e, 0)
     out = R.rasterize_gaussians(bg, d["means3D"], col, d["opacities"], d["scales"], d["rotations"], scale_modifier,
-                                e, e, e, 0, d["viewmatrix"], d["projmatrix"], cam.tanfovx, cam.tanfovy, kernel_size,
+                                e, e, ex, ED, d["viewmatrix"], d["projmatrix"], cam.tanfovx, cam.tanfovy, kernel_size,
                                 cam.height, cam.width, sh, sh_degree, d["campos"], False, debug)
     keys = ("num_rendered", "color", "depth", "norm", "alpha", "radii", "extra", "geom", "binning", "img")
     return dict(zip(keys, out))
 
 
 def run_ours_backward(d, cam, sh_degree, bg, fwd, cot, kernel_size=0.1, scale_modifier=1.0, colors=None, debug=False,
-                      **kw):
+                      extras=None, dL_extra=None, **kw):
     from sfgs import rasterizer as R
     e = torch.empty(0, device=d["means3D"].device)
     sh = e if colors is not None else d["shs"]
     col = colors if colors is not None else e
-    out = R.rasterize_gaussians_backward(bg, d["means3D"], fwd["radii"], col, d["scales"], d["rotations"], e,
+    ex = extras if extras is not None else e
+    dex = dL_extra if dL_extra is not None else e
+    out = R.rasterize_gaussians_backward(bg, d["means3D"], fwd["radii"], col, d["scales"], d["rotations"], ex,
                                          scale_modifier, e, e, d["viewmatrix"], d["projmatrix"], cam.tanfovx,
-                                         cam.tanfovy, kernel_size, cot[0], cot[1], cot[2], cot[3], e, sh, sh_degree,
+                                         cam.tanfovy, kernel_size, cot[0], cot[1], cot[2], cot[3], dex, sh, sh_degree,
                                          d["campos"], fwd["geom"], fwd["num_rendered"], fwd["binning"], fwd["img"],
                                          fwd["alpha"], debug, **kw)
     if kw.get("phase") == 1:

@@ -74,6 +74,9 @@ def test_new_option_validation_without_gpu():
     b.phase = 1                                   # phase 1 needs the pixel cotangents and a caller-owned acc (or peers)
     for f in ("dL_dpix", "dL_dpix_depth", "dL_dpix_norm", "dL_dpix_alpha", "accum_alphas"):
         setattr(b, f, ptr)
+    b.ED = 35                                     # more extra channels than SFGS_MAX_EXTRA
+    assert L.sfgs_rasterize_backward(C.byref(b)) == -2 and "ED out of range" in native.last_error()
+    b.ED = 0
     assert L.sfgs_rasterize_backward(C.byref(b)) == -2 and "acc" in native.last_error()
     peers = (C.c_void_p * 2)(C.cast(dummy, C.c_void_p), C.cast(dummy, C.c_void_p))
     b.acc_peers, b.n_peers, b.peer_slice = C.cast(peers, C.POINTER(C.c_void_p)), 2, 3     # 2*3 < P

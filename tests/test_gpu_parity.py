@@ -217,6 +217,38 @@ def test_against_cpu_oracle(cuda_device):
         assert np.abs(a - b).max() <= 1e-4 + 2e-4 * np.abs(b).max(), k
 
 
+@pytest.mark.parametrize("ED", [1, 34])
+def test_extra_attrs_vs_cpu_oracle(cuda_device, ED):
+    """extra_attrs (ED channels, 34 = SFGS_MAX_EXTRA) on an image that is not a multiple of the tile: the extras and
+    their gradients against the CPU oracle, and every other forward output bit-identical to the same call without
+    extras (both run one blend loop)."""
+    from oracle import cpu_oracle as O
+    dev = cuda_device
+    scene, cam = S.blob_scene(2500, seed=41), S.simple_camera(190, 150)
+    bg = np.array([0.3, 0.1, 0.2], np.float32)
+    bg_t = torch.from_numpy(bg).to(dev)
+    rng = np.random.default_rng(ED)
+    extras = rng.uniform(-1, 1, (scene.P, ED)).astype(np.float32)
+    dL_extra = rng.uniform(-1, 1, (ED, cam.height, cam.width)).astype(np.float32)
+    d = Hh.to_torch(scene, cam, dev)
+    f0 = Hh.run_ours_forward(d, cam, 3, bg_t)
+    f = Hh.run_ours_forward(d, cam, 3, bg_t, extras=torch.from_numpy(extras).to(dev))
+    for k in ("color", "depth", "norm", "alpha"):
+        assert torch.equal(bits(f[k]), bits(f0[k])), k
+    n_contrib = lambda fw: Hh.our_internals(fw, scene.P, cam.height, cam.width)["n_contrib"]  # noqa: E731
+    assert torch.equal(n_contrib(f), n_contrib(f0))
+    o = O.forward(scene.means3D, scene.scales, scene.rotations, scene.opacities, scene.shs, 3, cam.viewmatrix,
+                  cam.projmatrix, cam.campos, cam.width, cam.height, cam.tanfovx, cam.tanfovy, bg, extras=extras)
+    assert np.abs(f["extra"].cpu().numpy() - o["extra"]).max() <= 5e-5   # glibc expf vs CUDA expf, as above
+    cot = S.cotangents(cam.width, cam.height, seed=6)
+    gb = Hh.run_ours_backward(d, cam, 3, bg_t, f, [torch.from_numpy(c).to(dev) for c in cot],
+                              extras=torch.from_numpy(extras).to(dev), dL_extra=torch.from_numpy(dL_extra).to(dev))
+    og = O.backward(o, *cot, dL_extra=dL_extra)
+    for k in ("extra", "means2D", "opacity", "means3D"):
+        a, b = gb[k].cpu().numpy().astype(np.float64), og[k].astype(np.float64)
+        assert np.abs(a - b).max() <= 1e-4 + 2e-4 * np.abs(b).max(), k
+
+
 def test_edge_cases(cuda_device):
     dev = cuda_device
     from sfgs import rasterizer as R
