@@ -13,15 +13,18 @@
 //   phase 1  pixel-parallel (lane = pixel): the per-pixel recursion over the chunk's records in slot order.  The
 //            reference's eight per-channel accumulators collapse into the scalar form
 //                dL/dalpha_j = T_j (g_j - A_j),  g_j = <dL/dpix, attr_j>,  A_j = a_{j+1} g_{j+1} + (1 - a_{j+1}) A_{j+1}
-//            (the channel-sum of accum_rec/accum_red/accum_ren/accum_rea, backward.cu:660-711).  Per pair only two
-//            numbers leave the lane:  w = alpha*T  and  h = G * dL/dalpha ; they are parked in a per-warp
-//            shared-memory tile [pixel][slot].  Slot k is a compile-time constant after unrolling, so record
-//            parameters, list position and the (w, h) hand-over all sit at immediate offsets;
+//            (the channel-sum of accum_rec/accum_red/accum_ren/accum_rea, backward.cu:660-711), carried as one
+//            register C = A of the next active record.  Per pair only two numbers leave the lane:  w = alpha*T  and
+//            h = G * dL/dalpha ; they are parked in a per-warp shared-memory tile [pixel][slot].  Slot k is a
+//            compile-time constant after unrolling, so record parameters, list position and the (w, h) hand-over all
+//            sit at immediate offsets;
 //   phase 2  record-parallel (lane = slot of the chunk x half of the block's pixels): all 14 per-Gaussian sums are
 //            linear in (w, h):
 //                sum w*dL/dpix_c (7 channels),  sum h*{1, dx, dy, dx^2, dx dy, dy^2},  sum |..| for the abs-gradient,
 //            so each lane streams down its record's column of the tile accumulating in registers — no cross-lane
-//            reduction except one 16-lane exchange between the two pixel halves;
+//            reduction except one 16-lane exchange between the two pixel halves.  The loop is fully unrolled and
+//            sums h against the pixels' compile-time offsets from the centre of their 8x2 half; the moments about
+//            the record's centre follow once per chunk by binomial expansion;
 //   combine  each (block, record) pair ends in four red.global.add.v4.f32 (tools/red_bench.cu times such traffic on
 //            its own; the ~16 M issued per frame hide behind the math): ~200x fewer global atomics than the reference.
 //
@@ -30,13 +33,19 @@
 // (T is recovered back to front as T_j = T_{j+1} * rcp.approx(1 - alpha_{j+1}).  Refining the reciprocal with a Newton step
 // costs time and does NOT change the error statistics against the float64 adjudicator — the worst elements are
 // summation-order noise of ill-conditioned sums, which vary by 5x between runs of either implementation, not T drift.)
+// (Numerics of the expansion in phase 2: for a record whose centre is (DX, DY) from the half's centre, sum h dx^2
+// formed as DX^2 sum h - 2 DX sum h x + sum h x^2 carries rounding error of about eps (|DX| + |x|)^2 sum|h|, where the
+// direct sum over the pixels carries eps (DX - x)^2 sum|h|.  With the origin at the half's first pixel (offsets 0..7)
+// the expansion's error was several times the direct sum's for the many small records centred inside the block, and
+// the float64-adjudicated conic gradients (cov3D, scales, rotations) exceeded the reference build's error.  Centred
+// offsets (+-3.5 .. +-0.5, rows +-0.5) bring it back within the reference's error.)
 #include "sfgs_common.cuh"
 
 namespace {
 
 constexpr int BWD_THREADS = 256;
 constexpr int BWD_WARPS = BWD_THREADS / 32;
-constexpr int PIXF = 12;          // floats per pixel-table row: dLc[3], dLd, dLn[3], px, py, pad[3]
+constexpr int PIXF = 8;           // floats per pixel-table row: dLc[3], dLd, dLn[3], half centre (see below)
 
 // PEER: the target may be another GPU's memory reached over NVLink and every GPU of the node adds into it, so the
 // reduction must be system-scope; otherwise the default (device) scope
@@ -63,7 +72,7 @@ struct alignas(16) WarpSmem {
                                 //        record carries its list position (bits of a uint32)
   uint32_t gid[2][W4_CH];       // Gaussian id of each slot
   float2 wh[32][W4_CH + 1];     // 4.25 KB phase-1 -> phase-2 hand-over, [pixel][slot], padded
-  float pix[32][PIXF];          // 1.5 KB  per-pixel cotangents and coordinates
+  float pix[32][PIXF];          // 1 KB    per-pixel cotangents
   uint32_t list[64];            // ring of collected list positions
 };
 
@@ -141,8 +150,10 @@ render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict_
   {
     float4* pt = reinterpret_cast<float4*>(&S.pix[lane][0]);
     pt[0] = make_float4(dLc0, dLc1, dLc2, dLd);
-    pt[1] = make_float4(dLn0, dLn1, dLn2, pixfx);
-    pt[2] = make_float4(pixfy, 0.f, 0.f, 0.f);
+    // the free word: the centre of the lane's 8x2 half of the block, its x in even lanes and its y in odd ones;
+    // phase 2 reads it from the half's pixels 0 and 1
+    pt[1] = make_float4(dLn0, dLn1, dLn2, (lane & 1) ? pixfy - (float)((lane >> 3) & 1) + 0.5f
+                                                     : pixfx - (float)(lane & 7) + 3.5f);
   }
   __syncwarp();
 
@@ -157,9 +168,10 @@ render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict_
       last_extra[ch] = 0.f;
     }
 
-  float A = 0.f, g_last = 0.f, last_alpha = 0.f;
-  const float ddelx_dx = 0.5 * W;
-  const float ddely_dy = 0.5 * H;
+  // C = the A of the next active record, advanced at each active record as C' = alpha g + (1 - alpha) C (the
+  // reference keeps A, g_last and last_alpha and forms this only at the next record); last_alpha is kept for the
+  // extras' recursion only
+  float C = 0.f, last_alpha = 0.f;
   const SfgsExpConsts ek = sfgs_exp_consts(hdr[HDR_ZERO]);
   const unsigned lt_mask = (1u << lane) - 1u;
 
@@ -203,7 +215,11 @@ render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict_
     return n;
   };
 
-  // ---- phase 2: lane (k = lane & 15, half = lane >> 4) sums slot k of the chunk over pixels half*16 .. +15
+  // ---- phase 2: lane (k = lane & 15, half = lane >> 4) sums slot k of the chunk over pixels half*16 .. +15.  The
+  // half is 8 x 2 pixels; in coordinates centred on it, its pixel i sits at the compile-time offset
+  // (x, y) = ((i & 7) - 3.5, (i >> 3) - 0.5).  The loop sums h against those constants, and the moments about the
+  // record's centre (dx = DX - x, dy = DY - y, where (DX, DY) = record centre - half centre) follow once per chunk
+  // (see the numerics note at the top).
   const int ck = lane & (W4_CH - 1), chalf = lane >> 4;
   auto phase2 = [&](int n, int buf) {
     __syncwarp();
@@ -212,24 +228,41 @@ render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict_
     const float4 ra = S.rec[buf][slot][0];      // mx, my, con.x, con.y
     const float4 rb = S.rec[buf][slot][1];      // con.z, opac, depth
     const uint32_t gid = S.gid[buf][slot];
+    const float2* whp = &S.wh[chalf * 16][ck];
+    const float4* pix = reinterpret_cast<const float4*>(&S.pix[chalf * 16][0]);
+    const float DX = ra.x - pix[1].w, DY = ra.y - pix[3].w;
+    // abs-gradient term |h| (|u| + |v|), u = (W/2)(con.x dx + con.y dy), v = (H/2)(con.y dx + con.z dy): affine in
+    // the pixel offset, so each is one FFMA from its row's base.  au .. bv are the conic scaled by d(ndc)/d(pixel)
+    // (W/2 or H/2; 0.5 con is exact)
+    const float au = 0.5f * ra.z * W, bu = 0.5f * ra.w * W, av = 0.5f * ra.w * H, bv = 0.5f * rb.x * H;
+    const float u0 = fmaf(au, DX, bu * DY), v0 = fmaf(av, DX, bv * DY);
+    const float urow[2] = {fmaf(bu, 0.5f, u0), fmaf(bu, -0.5f, u0)}, vrow[2] = {fmaf(bv, 0.5f, v0), fmaf(bv, -0.5f, v0)};
     float s0 = 0, s1 = 0, s2 = 0, s3 = 0, s4 = 0, s5 = 0, s6 = 0;      // sum w * dL/dpix_c
-    float sh = 0, shx = 0, shy = 0, shxx = 0, shxy = 0, shyy = 0, sab = 0;
-    const int pbase = chalf * 16;
-#pragma unroll 4
+    float h1[2] = {0, 0}, hx[2] = {0, 0}, sxx = 0;                    // per row: sum h * {1, x}; sum h x^2
+    float sab = 0;
+#pragma unroll
     for (int i = 0; i < 16; i++) {
-      const float2 wh = S.wh[pbase + i][ck];
-      const float4 p0 = *reinterpret_cast<const float4*>(&S.pix[pbase + i][0]);
-      const float4 p1 = *reinterpret_cast<const float4*>(&S.pix[pbase + i][4]);
-      const float pyv = S.pix[pbase + i][8];
+      const float x = (float)(i & 7) - 3.5f;
+      const int r = i >> 3;
+      const float2 wh = whp[i * (W4_CH + 1)];
+      const float4 p0 = pix[2 * i], p1 = pix[2 * i + 1];
       s0 = fmaf(wh.x, p0.x, s0); s1 = fmaf(wh.x, p0.y, s1); s2 = fmaf(wh.x, p0.z, s2); s3 = fmaf(wh.x, p0.w, s3);
       s4 = fmaf(wh.x, p1.x, s4); s5 = fmaf(wh.x, p1.y, s5); s6 = fmaf(wh.x, p1.z, s6);
-      const float dx = ra.x - p1.w, dy = ra.y - pyv;
-      const float hx = wh.y * dx, hy = wh.y * dy;
-      sh += wh.y; shx += hx; shy += hy;
-      shxx = fmaf(hx, dx, shxx); shxy = fmaf(hx, dy, shxy); shyy = fmaf(hy, dy, shyy);
-      const float t7 = fmaf(ra.z, hx, ra.w * hy), t8 = fmaf(rb.x, hy, ra.w * hx);
-      sab = fmaf(fabsf(t7), ddelx_dx, sab); sab = fmaf(fabsf(t8), ddely_dy, sab);
+      h1[r] += wh.y;
+      hx[r] = fmaf(wh.y, x, hx[r]);
+      sxx = fmaf(wh.y, x * x, sxx);
+      const float u = fmaf(-au, x, urow[r]), v = fmaf(-av, x, vrow[r]);
+      sab = fmaf(fabsf(wh.y), fabsf(u) + fabsf(v), sab);
     }
+    // sums of h * {1, x, y, x^2, x y, y^2} over the half (y = -0.5 in row 0, +0.5 in row 1) ...
+    float sh = h1[0] + h1[1];
+    const float sx = hx[0] + hx[1], sy = 0.5f * (h1[1] - h1[0]);
+    const float sxy = 0.5f * (hx[1] - hx[0]), syy = 0.25f * sh;
+    // ... and about the centre: sum h dx = DX sum h - sum h x, sum h dx^2 = DX sum h dx - (DX sum h x - sum h x^2), ...
+    float shx = fmaf(DX, sh, -sx), shy = fmaf(DY, sh, -sy);
+    float shxx = fmaf(DX, shx, -fmaf(DX, sx, -sxx));
+    float shxy = fmaf(DX, shy, -fmaf(DY, sx, -sxy));
+    float shyy = fmaf(DY, shy, -fmaf(DY, sy, -syy));
 #define XH(v) v += __shfl_xor_sync(0xffffffffu, v, 16)
     XH(s0); XH(s1); XH(s2); XH(s3); XH(s4); XH(s5); XH(s6);
     XH(sh); XH(shx); XH(shy); XH(shxx); XH(shxy); XH(shyy); XH(sab);
@@ -243,11 +276,11 @@ render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict_
       } else {
         dst = acc + (size_t)gid * 16;
       }
-      if (chalf == 0) {
+      if (lane < 16) {
         red_add_v4<PEER>(dst, make_float4(s0, s1, s2, s3));
-        red_add_v4<PEER>(dst + 4, make_float4(s4, s5, s6, -ddelx_dx * o * fmaf(ra.z, shx, ra.w * shy)));
+        red_add_v4<PEER>(dst + 4, make_float4(s4, s5, s6, -o * fmaf(au, shx, bu * shy)));
       } else {
-        red_add_v4<PEER>(dst + 8, make_float4(-ddely_dy * o * fmaf(rb.x, shy, ra.w * shx), fabsf(o) * sab,
+        red_add_v4<PEER>(dst + 8, make_float4(-o * fmaf(bv, shy, av * shx), fabsf(o) * sab,
                                               -0.5f * o * shxx, -0.5f * o * shxy));
         red_add_v4<PEER>(dst + 12, make_float4(-0.5f * o * shyy, sh, 0.f, 0.f));
       }
@@ -275,8 +308,9 @@ render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict_
       const float4 rd = S.rec[buf][k][3];       // ny, nz
       // 1 - alpha is in [0.01, 1]: the approximate reciprocal (1 ulp, one MUFU) needs no range fix-up; it is shared
       // by the T recovery and the background term
+      const float one_m_alpha = 1.f - alpha;
       float inv_1ma;
-      asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(inv_1ma) : "f"(1.f - alpha));
+      asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(inv_1ma) : "f"(one_m_alpha));
       const float Tn = T * inv_1ma;
       // two independent chains: halves the dependent-FMA latency of the dot product
       float g = rc.x * dLc0, g2 = rc.w * dLn0;
@@ -284,8 +318,7 @@ render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict_
       g += rc.z * dLc2; g2 += rd.y * dLn2;
       g += rb.z * dLd;  g2 += dLa;
       g += g2;
-      const float An = last_alpha * g_last + (1.f - last_alpha) * A;
-      float dL_dalpha_T = g - An;                 // dL/dalpha / T
+      float dL_dalpha_T = g - C;                  // dL/dalpha / T
       if constexpr (HAS_EXTRA) {
         const uint32_t gid = S.gid[buf][k];
         for (int ch = 0; ch < ED; ch++) {
@@ -296,14 +329,14 @@ render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict_
           last_extra[ch] = active ? ex : last_extra[ch];
           if (active) atomicAdd(&dL_dextras[(size_t)gid * ED + ch], alpha * Tn * dL_dpixel_extra[ch]);
         }
+        last_alpha = active ? alpha : last_alpha;
       }
       const float dL_dalpha = fmaf(tb, inv_1ma, Tn * dL_dalpha_T);
       const float w_out = active ? alpha * Tn : 0.f;
       const float h_out = active ? G * dL_dalpha : 0.f;
       T = active ? Tn : T;
-      A = active ? An : A;
-      g_last = active ? g : g_last;
-      last_alpha = active ? alpha : last_alpha;
+      // the roundings of forming A from (A, g_last, last_alpha) at the next record: (1 - alpha) * C, then one FMA
+      C = active ? fmaf(alpha, g, __fmul_rn(one_m_alpha, C)) : C;
       S.wh[lane][k] = make_float2(w_out, h_out);
     };
     auto slot = [&](const int k) {
@@ -324,7 +357,7 @@ render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict_
       for (int k = 0; k < n_cur; k++) slot(k);
     }
     phase2(n_cur, buf);
-    buf ^= 1;
+    buf = 1 - buf;                                  // (as buf ^= 1, ptxas spills in two of the three instantiations)
     n_cur = n_next;
   }
 }
