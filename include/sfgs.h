@@ -244,8 +244,9 @@ int sfgs_activations_backward(int P, const float* opacity_raw, const float* scal
  * kernel: EmbeddingModel.forward (scene/gaussian_model.py:45-69: [P,59] -> 128 -> 128 -> 6 MLP on [min(dc,1) | Fourier
  * features | per-camera embedding], x0.01, offset/C0 on the DC term, per-channel multiplier, clamp at 1), eval_sh of
  * the toned coefficients along normalize(xyz - campos) (utils/sh_utils.py), +0.5, clamp at 0  ->  colors_precomp [P,3].
- * W1 is [128, 3+G+E] row-major (torch.nn.Linear.weight), W2 [128,128], W3 [6,128]; features [P,M,3] with M = 16,
- * gemb [P,G] with G = 24 (4 Fourier frequencies), aemb [E] with E = 32; D = active SH degree.  Tensor-core
+ * W1 is [128, 3+G+E] row-major (torch.nn.Linear.weight), W2 [128,128], W3 [6,128]; features [P,M,3] with M = 1, 4,
+ * 9 or 16 ((max_sh_degree+1)^2), gemb [P,G] with G = 24 (4 Fourier frequencies), aemb [E] with E = 32; D = active SH
+ * degree, 0..3.  Another M, G or E returns SFGS_E_UNSUPPORTED; (D+1)^2 > M returns SFGS_E_BADARG.  Tensor-core
  * operands are split bf16 pairs (hi + lo, three wgmma per product), fp32 accumulation in registers; the result is
  * within 1e-4 of the float32 torch evaluation.  features and gemb must be 16-byte aligned. */
 int sfgs_appearance_forward(int P, int D, int M, const float* features, const float* gemb, int G, const float* aemb,

@@ -2,14 +2,19 @@
 //
 // Replaces, for the forward pass, gaussian_renderer/__init__.py:105-118 + EmbeddingModel.forward
 // (scene/gaussian_model.py:45-69) + eval_sh (utils/sh_utils.py) — in torch: a [P,59] concat, three Linear layers with
-// [P,128] fp32 intermediates, a repeat, a [P,48] tone map, a [P,3,16] transpose, the SH evaluation and four clamps,
-// ~25 kernels and ~2.5 KB of HBM traffic per Gaussian — by one kernel that reads each Gaussian's 48 SH features, 24
-// Fourier features and position once and writes its 3 colours (324 B per Gaussian):
+// [P,128] fp32 intermediates, a repeat, a [P,3M] tone map, a [P,3,M] transpose, the SH evaluation and four clamps,
+// ~25 kernels and ~2.5 KB of HBM traffic per Gaussian at M = 16 — by one kernel that reads each Gaussian's 3M SH
+// features, 24 Fourier features and position once and writes its 3 colours (324 B per Gaussian at M = 16):
 //
 //   inp    = [min(features[:3], 1) | gemb | aemb]                      (59 = 3 + 24 + 32)
 //   h      = W3 relu(W2 relu(W1 inp + b1) + b2) + b3 ;  offset, mul = 0.01 h[:3], 0.01 h[3:]
-//   toned  = min(min(features, 1) * mul[ch] + [offset/C0 on the DC term], 1)           ([16,3] per Gaussian)
+//   toned  = min(min(features, 1) * mul[ch] + [offset/C0 on the DC term], 1)            ([M,3] per Gaussian)
 //   colour = max(eval_sh(D, toned, normalize(xyz - campos)) + 0.5, 0)
+//
+// M = (max_sh_degree + 1)^2 is a template parameter (1, 4, 9 or 16).  Layer 1 reads only the three DC values, so the
+// GEMMs do not depend on it; M sets the feature row stride (3M floats), the L2 prefetch span and the length of the
+// tone-map / eval_sh loop.  Rows are loaded as float4 only when M % 4 == 0: 12- and 108-byte rows are not 16-byte
+// aligned.
 //
 // The per-camera embedding `aemb` is the same vector for every Gaussian, so its 32 columns of W1 fold into the bias
 // (b1' = b1 + W1[:, 27:] aemb, computed once per CTA) and layer 1 contracts over K = 27 (padded to 32).
@@ -150,8 +155,9 @@ __device__ __forceinline__ void split_store(__nv_bfloat16* hi, __nv_bfloat16* lo
   *lo = __float2bfloat16(x - __bfloat162float(h));
 }
 
+template <int M>
 __global__ void __launch_bounds__(AP_THREADS, 1)
-appearance_fwd_kernel(int P, int D, const float* __restrict__ features /*[P,16,3]*/, const float* __restrict__ gemb /*[P,24]*/,
+appearance_fwd_kernel(int P, int D, const float* __restrict__ features /*[P,M,3]*/, const float* __restrict__ gemb /*[P,24]*/,
                       const float* __restrict__ aemb /*[32]*/, const float* __restrict__ W1 /*[128,59]*/,
                       const float* __restrict__ b1, const float* __restrict__ W2 /*[128,128]*/, const float* __restrict__ b2,
                       const float* __restrict__ W3 /*[6,128]*/, const float* __restrict__ b3,
@@ -197,10 +203,11 @@ appearance_fwd_kernel(int P, int D, const float* __restrict__ features /*[P,16,3
     if (tl >= ntiles) return;
     const int r0 = tl * AP_M;
     const unsigned rows = (unsigned)((P - r0) < AP_M ? (P - r0) : AP_M);
-    const float* pf = features + (size_t)r0 * 48;
+    const float* pf = features + (size_t)r0 * (3 * M);     // r0 * 12M bytes: 16-byte aligned, as r0 is a multiple of 128
     const float* pg = gemb + (size_t)r0 * AP_G;
     const float* pm = means3D + (size_t)r0 * 3;
-    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(pf), "r"(rows * 192u) : "memory");
+    const unsigned fb = (rows * (12u * M)) & ~15u;           // zero only for M = 1 and a single row
+    if (M % 4 == 0 || fb) asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(pf), "r"(fb) : "memory");
     asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(pg), "r"(rows * (unsigned)(AP_G * 4)) : "memory");
     const unsigned mb = (rows * 12u) & ~15u;
     if (mb && (reinterpret_cast<uintptr_t>(pm) & 15) == 0)
@@ -214,7 +221,7 @@ appearance_fwd_kernel(int P, int D, const float* __restrict__ features /*[P,16,3
     // ---- A0: row m = [min(dc, 1) (3) | Fourier features (24) | 0 (5)]
     {
       float in[AP_K1];
-      const float* f = features + (size_t)gi * 48;
+      const float* f = features + (size_t)gi * (3 * M);
       in[0] = fminf(f[0], 1.f); in[1] = fminf(f[1], 1.f); in[2] = fminf(f[2], 1.f);
       const float4* g4 = reinterpret_cast<const float4*>(gemb + (size_t)gi * AP_G);
 #pragma unroll
@@ -285,18 +292,23 @@ appearance_fwd_kernel(int P, int D, const float* __restrict__ features /*[P,16,3
     bas[14] = SH_C3_5 * z * (xx - yy); bas[15] = SH_C3_6 * x * (xx - 3.f * yy);
     const int ncoef = (D + 1) * (D + 1);
     float rgb[3] = {0.f, 0.f, 0.f};
-    const float4* f4 = reinterpret_cast<const float4*>(features + (size_t)gi * 48);
+    auto tone_sh = [&](int j, float e) {                               // features[k][ch], j = 3 k + ch
+      const int k = j / 3, ch = j - 3 * k;
+      float tv = fminf(e, 1.f) * mul[ch] + (k == 0 ? off[ch] : 0.f);
+      tv = fminf(tv, 1.f);
+      if (k < ncoef) rgb[ch] = fmaf(bas[k], tv, rgb[ch]);
+    };
+    const float* fr = features + (size_t)gi * (3 * M);
+    if constexpr (M % 4 == 0) {
+      const float4* f4 = reinterpret_cast<const float4*>(fr);
 #pragma unroll
-    for (int q = 0; q < 12; q++) {
-      const float4 v = f4[q];
-      const float e[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-      for (int u = 0; u < 4; u++) {
-        const int j = 4 * q + u, k = j / 3, ch = j - 3 * k;          // features[k][ch]
-        float tv = fminf(e[u], 1.f) * mul[ch] + (k == 0 ? off[ch] : 0.f);
-        tv = fminf(tv, 1.f);
-        if (k < ncoef) rgb[ch] = fmaf(bas[k], tv, rgb[ch]);
+      for (int q = 0; q < 3 * M / 4; q++) {
+        const float4 v = f4[q];
+        tone_sh(4 * q, v.x); tone_sh(4 * q + 1, v.y); tone_sh(4 * q + 2, v.z); tone_sh(4 * q + 3, v.w);
       }
+    } else {
+#pragma unroll
+      for (int j = 0; j < 3 * M; j++) tone_sh(j, fr[j]);
     }
     if (valid) {
       colors[3 * (size_t)g] = fmaxf(rgb[0] + 0.5f, 0.f);
@@ -317,18 +329,25 @@ extern "C" int sfgs_appearance_forward(int P, int D, int M, const float* feature
                                        float* colors, void* stream) {
   if (P < 0) return sfgs_set_error(SFGS_E_BADARG, "appearance_forward: P < 0", 0);
   if (P == 0) return SFGS_OK;
-  if (M != 16 || G != AP_G || E != AP_E || D < 0 || D > 3)
-    return sfgs_set_error(SFGS_E_UNSUPPORTED, "appearance_forward: built for 16 SH coefficients, 24 Fourier features, a 32-wide embedding", 0);
+  if ((M != 1 && M != 4 && M != 9 && M != 16) || G != AP_G || E != AP_E || D < 0 || D > 3)
+    return sfgs_set_error(SFGS_E_UNSUPPORTED,
+                          "appearance_forward: built for 1, 4, 9 or 16 SH coefficients, 24 Fourier features, a 32-wide embedding", 0);
+  if ((D + 1) * (D + 1) > M)
+    return sfgs_set_error(SFGS_E_BADARG, "appearance_forward: active SH degree D needs (D+1)^2 <= M coefficients", 0);
   if (!features || !gemb || !aemb || !W1 || !b1 || !W2 || !b2 || !W3 || !b3 || !means3D || !campos || !colors)
     return sfgs_set_error(SFGS_E_BADARG, "appearance_forward: null pointer", 0);
   if ((reinterpret_cast<uintptr_t>(features) & 15) || (reinterpret_cast<uintptr_t>(gemb) & 15))
     return sfgs_set_error(SFGS_E_BADARG, "appearance_forward: features / gemb must be 16-byte aligned", 0);
+  using Kernel = void (*)(int, int, const float*, const float*, const float*, const float*, const float*, const float*,
+                          const float*, const float*, const float*, const float*, const float*, float*);
+  const Kernel kernels[4] = {appearance_fwd_kernel<1>, appearance_fwd_kernel<4>, appearance_fwd_kernel<9>, appearance_fwd_kernel<16>};
+  const Kernel kernel = kernels[M == 1 ? 0 : M == 4 ? 1 : M == 9 ? 2 : 3];
   static SfgsPerDeviceOnce once;
   static int sms[64] = {0};
   int dev = 0;
   cudaGetDevice(&dev);
   if (once.first_use() || (dev >= 0 && dev < 64 && sms[dev] == 0)) {
-    cudaFuncSetAttribute(appearance_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ApSmem));
+    for (const Kernel k : kernels) cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ApSmem));
     int n = 132;
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
     if (dev >= 0 && dev < 64) sms[dev] = n;
@@ -338,8 +357,8 @@ extern "C" int sfgs_appearance_forward(int P, int D, int M, const float* feature
   const int pairs = (ntiles + AP_GROUPS - 1) / AP_GROUPS;
   const int grid = pairs < nsm ? pairs : nsm;                // persistent: one CTA (two tile groups) per SM
   SFGS_COUNT_LAUNCH();
-  appearance_fwd_kernel<<<grid, AP_THREADS, sizeof(ApSmem), (cudaStream_t)stream>>>(P, D, features, gemb, aemb, W1, b1, W2, b2,
-                                                                                  W3, b3, means3D, campos, colors);
+  kernel<<<grid, AP_THREADS, sizeof(ApSmem), (cudaStream_t)stream>>>(P, D, features, gemb, aemb, W1, b1, W2, b2, W3, b3,
+                                                                   means3D, campos, colors);
   const cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? SFGS_OK : sfgs_set_error(SFGS_E_CUDA, "appearance_forward", (int)e);
 }

@@ -9,10 +9,14 @@ replaces, in gaussian_renderer/__init__.py:105-118,
     dir_pp_normalized = ...; colors_toned = eval_sh(pc.active_sh_degree, colors_toned, dir_pp_normalized)
     colors_precomp = torch.clamp_min(colors_toned + 0.5, 0.0)
 
+for any SH width the model stores: features [P, M, 3] with M = (max_sh_degree + 1)^2 = 1, 4, 9 or 16 (the README's
+training commands use --sh_degree 1, M = 4), at any active degree D with (D + 1)^2 <= M.
+
 Forward: one wgmma tensor-core kernel (csrc/sfgs_appearance.cu, `sfgs_appearance_forward`).  Backward: not fused yet —
 the autograd function recomputes the same expression with torch ops (`reference_colors`, float32) and differentiates
-that, so gradients are those of the torch formulation; the fused forward pays off for evaluation / video renders
-(render_video.py, metrics) and halves the appearance cost of a training step.
+that, so gradients are those of the torch formulation.  The fused forward pays off where no backward follows
+(evaluation and video renders: render_video.py, metrics).  In a training step the recompute repeats the torch forward,
+so the step pays the fused forward on top of the torch forward and backward (DESIGN.md §7).
 """
 from __future__ import annotations
 
@@ -100,8 +104,10 @@ class _Appearance(torch.autograd.Function):
 
 
 def fused_appearance_colors(features, gemb, aemb, mlp, xyz, campos, active_sh_degree):
-    """features [P,16,3] (pc.get_features), gemb [P,24] (pc._embeddings), aemb [32] (the camera's appearance
-    embedding), mlp = pc.appearance_mlp.mlp (nn.Sequential Linear-ReLU-Linear-ReLU-Linear) or its six tensors."""
+    """features [P,M,3] (pc.get_features, M = (pc.max_sh_degree + 1)^2 = 1, 4, 9 or 16), gemb [P,24]
+    (pc._embeddings), aemb [32] (the camera's appearance embedding), mlp = pc.appearance_mlp.mlp (nn.Sequential
+    Linear-ReLU-Linear-ReLU-Linear) or its six tensors; active_sh_degree D needs (D + 1)^2 <= M.  Another M, or a D
+    the width cannot hold, raises native.SfgsError."""
     if isinstance(mlp, (tuple, list)):
         W1, b1, W2, b2, W3, b3 = mlp
     else:
