@@ -191,6 +191,17 @@ typedef struct sfgs_backward_args {
 
 int sfgs_rasterize_backward(const sfgs_backward_args* a);
 
+/* The same backward with bit-reproducible outputs: no floating-point atomics or reductions; every per-Gaussian sum
+ * runs in an order fixed by the inputs alone (not by scheduling, SM count or addresses), and the cross-tile sums are
+ * formed in float64.  Same struct, same validation, plus:
+ *   phase 0 and phase 1 (the blend adjoint) need `radii` and `scratch_alloc`: the extra scratch is
+ *     4 P + 524 R bytes (+ alignment; R = instances of the forward), on top of the P*16 floats of `acc` when that is
+ *     not given;
+ *   phase 2 runs the per-Gaussian adjoint, which has no reduction, exactly as sfgs_rasterize_backward does;
+ *   acc_peers (system-scope reductions) and ED > 0 (extra_attrs) return SFGS_E_UNSUPPORTED before any CUDA work.
+ * The outputs equal sfgs_rasterize_backward's up to the rounding of the sums' order. */
+int sfgs_rasterize_backward_deterministic(const sfgs_backward_args* a);
+
 /* ---- markVisible --------------------------------------------------------- */
 int sfgs_mark_visible(int P, const float* means3D, const float* viewmatrix,
                       const float* projmatrix, unsigned char* present, void* stream);

@@ -12,6 +12,8 @@
 //            The binning buffer is sized from a running estimate instead and the
 //            tail of the pipeline is re-run in the rare case it was too small.
 // Backward = zero accumulators -> tile blend adjoint -> per-Gaussian adjoint.
+// Deterministic backward = clear the written flags -> ORDERED blend adjoint (partial rows, no reductions) ->
+//            fixed-order float64 sum of each Gaussian's rows into acc (sfgs_bwd_order.cu) -> per-Gaussian adjoint.
 #include <cstdio>
 #include <cstring>
 #include <atomic>
@@ -33,7 +35,13 @@ void sfgs_launch_tile_sort(const GeomLayout& g, const ImageLayout& im, const Bin
 void sfgs_launch_render_fwd(const sfgs_forward_args* a, const GeomLayout& g, const ImageLayout& im,
                             const BinningLayout& b, cudaStream_t st);
 void sfgs_launch_render_bwd(const sfgs_backward_args* a, const GeomLayout& g, const ImageLayout& im,
-                            const BinningLayout& b, float* acc, cudaStream_t st);
+                            const BinningLayout& b, float* acc, float* part, unsigned char* written, cudaStream_t st);
+size_t sfgs_order_scratch_bytes(int P, long long R);
+SfgsOrderScratch sfgs_order_scratch(char* base, int P, long long R);
+void sfgs_launch_order_prepare(int P, const GeomLayout& g, const ImageLayout& im, const BinningLayout& b,
+                               const int* radii, int band0, int band1, const SfgsOrderScratch& o, cudaStream_t st);
+void sfgs_launch_order_reduce(int P, const GeomLayout& g, const int* radii, bool all_rows, const SfgsOrderScratch& o,
+                              float* acc, cudaStream_t st);
 int sfgs_launch_activations_fwd(int P, const float* opacity_raw, const float* scaling_raw, const float* rotation_raw,
                                 const double* filter_3D, float* opacity, float* scales, float* rotations,
                                 cudaStream_t st);
@@ -122,7 +130,8 @@ int fail(int code, const char* what, cudaError_t e = cudaSuccess) {
   } while (0)
 
 // ---- optional per-stage device timing (bench.py's roofline uses it; off by default) ----
-enum { ST_FWD_ZERO = 0, ST_PREPROCESS, ST_SCAN, ST_EMIT, ST_SORT, ST_RENDER_FWD, ST_BWD_ZERO, ST_RENDER_BWD, ST_GAUSS_BWD, ST_COUNT };
+enum { ST_FWD_ZERO = 0, ST_PREPROCESS, ST_SCAN, ST_EMIT, ST_SORT, ST_RENDER_FWD, ST_BWD_ZERO, ST_RENDER_BWD, ST_GAUSS_BWD,
+       ST_BWD_ORDER, ST_COUNT };
 struct StageProf {
   bool on = false;
   struct Span { cudaEvent_t a, b; int stage; };
@@ -178,6 +187,8 @@ struct PinnedHdr {
 };
 constexpr int MAX_DEVICES = 64;
 thread_local PinnedHdr t_hdr_dev[MAX_DEVICES];
+
+int rasterize_backward(const sfgs_backward_args* a, bool deterministic);
 
 }  // namespace
 
@@ -323,9 +334,20 @@ int sfgs_rasterize_forward(const sfgs_forward_args* a) {
   return (int)R;
 }
 
-int sfgs_rasterize_backward(const sfgs_backward_args* a) {
+int sfgs_rasterize_backward(const sfgs_backward_args* a) { return rasterize_backward(a, false); }
+int sfgs_rasterize_backward_deterministic(const sfgs_backward_args* a) { return rasterize_backward(a, true); }
+
+}  // extern "C"
+
+namespace {
+
+int rasterize_backward(const sfgs_backward_args* a, bool deterministic) {
   if (!a) return fail(SFGS_E_BADARG, "backward: null args");
   if (a->P < 0 || a->width <= 0 || a->height <= 0) return fail(SFGS_E_BADARG, "backward: bad sizes");
+  if (deterministic && a->acc_peers != nullptr)
+    return fail(SFGS_E_UNSUPPORTED, "backward_deterministic: acc_peers (system-scope reductions) have no deterministic implementation");
+  if (deterministic && a->ED > 0)
+    return fail(SFGS_E_UNSUPPORTED, "backward_deterministic: extra_attrs have no deterministic implementation");
   if (a->P == 0) return SFGS_OK;
   const int phase = a->phase;
   if (phase < 0 || phase > 2) return fail(SFGS_E_BADARG, "backward: phase must be 0, 1 or 2");
@@ -352,6 +374,10 @@ int sfgs_rasterize_backward(const sfgs_backward_args* a) {
   if (phase == 0 && !a->acc && !a->scratch_alloc) return fail(SFGS_E_BADARG, "backward: null scratch allocator");
   if (a->acc && (reinterpret_cast<uintptr_t>(a->acc) & 15)) return fail(SFGS_E_BADARG, "backward: acc must be 16-byte aligned");
   if (a->rotations && (reinterpret_cast<uintptr_t>(a->rotations) & 15)) return fail(SFGS_E_BADARG, "backward: rotations must be 16-byte aligned");
+  // the ordered blend adjoint places each partial by the Gaussian's tile rectangle (radii) in scratch_alloc's memory
+  const bool ordered = deterministic && do_blend;
+  if (ordered && !a->radii) return fail(SFGS_E_BADARG, "backward_deterministic: radii missing");
+  if (ordered && !a->scratch_alloc) return fail(SFGS_E_BADARG, "backward_deterministic: null scratch allocator");
   cudaStream_t st = (cudaStream_t)a->stream;
   const bool debug = a->debug != 0;
   const int P = a->P;
@@ -370,13 +396,37 @@ int sfgs_rasterize_backward(const sfgs_backward_args* a) {
   const float focal_x = a->width / (2.0f * a->tan_fovx);
 
   float* acc = a->acc;
-  if (!acc && !peer) {
-    const size_t abytes = (size_t)P * 16 * sizeof(float) + SFGS_ALIGN;
+  const long long R = a->R > 0 ? a->R : 0;
+  SfgsOrderScratch order = {};
+  // one scratch_alloc call: the allocator may hand out the memory of an earlier call's buffer again
+  if ((!acc && !peer) || ordered) {
+    const size_t acc_bytes = !acc ? sfgs_align_up((size_t)P * 16 * sizeof(float)) : 0;
+    const size_t abytes = acc_bytes + (ordered ? sfgs_order_scratch_bytes(P, R) : 0) + SFGS_ALIGN;
     char* aptr = a->scratch_alloc(a->scratch_user, abytes);
     if (!aptr) return fail(SFGS_E_ALLOC, "backward: scratch allocator returned NULL");
-    acc = (float*)sfgs_align_ptr(aptr);
+    char* base = sfgs_align_ptr(aptr);
+    if (!acc) acc = (float*)base;
+    if (ordered) order = sfgs_order_scratch(base + acc_bytes, P, R);
   }
-  if (do_blend) {
+  if (ordered) {
+    // every row of acc the per-Gaussian adjoint reads (phase 0) or the caller sums across ranks (phase 1) is
+    // written once by the reduction, so nothing is cleared but the written flags
+    PROF_BEGIN(ST_BWD_ZERO);
+    if (R > 0) CU(cudaMemsetAsync(order.written, 0, (size_t)R * BWD_BLOCKS, st));
+    PROF_END();
+    if (R > 0) {
+      PROF_BEGIN(ST_RENDER_BWD);
+      sfgs_launch_render_bwd(a, g, im, b, acc, order.part, order.written, st);
+      PROF_END();
+      STAGE_CHECK("render_bwd");
+    }
+    const SfgsBand band = sfgs_band(a->tile_row_begin, a->tile_row_end, im.tiles_y);
+    PROF_BEGIN(ST_BWD_ORDER);
+    sfgs_launch_order_prepare(P, g, im, b, a->radii, band.b0, band.b1, order, st);
+    sfgs_launch_order_reduce(P, g, a->radii, phase == 1, order, acc, st);
+    PROF_END();
+    STAGE_CHECK("bwd_order");
+  } else if (do_blend) {
     // cleared right before the blend adjoint: the memset also makes the accumulator lines L2-resident for the
     // kernel's vector reductions (cleared earlier, those lines would have left L2 by the time the reductions arrive)
     PROF_BEGIN(ST_BWD_ZERO);
@@ -389,7 +439,7 @@ int sfgs_rasterize_backward(const sfgs_backward_args* a) {
     PROF_END();
     if (a->R > 0) {
       PROF_BEGIN(ST_RENDER_BWD);
-      sfgs_launch_render_bwd(a, g, im, b, acc, st);
+      sfgs_launch_render_bwd(a, g, im, b, acc, nullptr, nullptr, st);
       PROF_END();
       STAGE_CHECK("render_bwd");
     }
@@ -402,6 +452,10 @@ int sfgs_rasterize_backward(const sfgs_backward_args* a) {
   }
   return SFGS_OK;
 }
+
+}  // namespace
+
+extern "C" {
 
 int sfgs_activations_forward(int P, const float* opacity_raw, const float* scaling_raw, const float* rotation_raw,
                              const double* filter_3D, float* opacity, float* scales, float* rotations, void* stream) {

@@ -27,6 +27,9 @@
 //            the record's centre follow once per chunk by binomial expansion;
 //   combine  each (block, record) pair ends in four red.global.add.v4.f32 (tools/red_bench.cu times such traffic on
 //            its own; the ~16 M issued per frame hide behind the math): ~200x fewer global atomics than the reference.
+//            The ORDERED instantiation (the deterministic backward, sfgs_bwd_order.cu) stores the pair's 16 words with
+//            plain 16-byte stores to its own row of a partial table instead, row (sorted instance) * 8 + block, and
+//            sets that row's written flag; a later pass adds the rows of each Gaussian in a fixed order.
 //
 // Chunks are always full except the last one of a warp.  A record that none of the warp's 32 pixels blends (0.6 % on
 // the benchmark frame: the reach mask is conservative) occupies a slot with zeros.
@@ -79,7 +82,10 @@ struct alignas(16) WarpSmem {
 // HAS_EXTRA: also the adjoint of the ED channels of `extras` [P,ED] (extra_attrs; Skyfall-GS never passes them):
 // phase 1 keeps the reference's per-pixel recursion of the extras and adds one global atomicAdd per (pixel, Gaussian,
 // channel) into dL_dextras, so this instantiation is a slow path.
-template <bool PEER, bool HAS_EXTRA>
+// ORDERED: no reduction at all.  The 16 words of a (block, record) pair go to row (range.x + list position) * 8 + wid
+// of `part` [R*8,16] and written[row] is set; exactly one warp owns each row.  `acc` is not touched.  The slot's gid
+// word carries the sorted instance range.x + list position instead of the Gaussian id (nothing else reads it here).
+template <bool PEER, bool HAS_EXTRA, bool ORDERED = false>
 __global__ void __launch_bounds__(BWD_THREADS, 3)
 render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict__ binning_base,
                        const uint32_t* __restrict__ hdr, int W, int H, int band0,
@@ -89,7 +95,8 @@ render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict_
                        const float* __restrict__ dL_dpixel_norms, const float* __restrict__ dL_dpixel_alphas,
                        const float* __restrict__ norm_raw, float* __restrict__ acc /* [P,16] zero-initialised */,
                        const PeerTable peers, const float* __restrict__ extras,
-                       const float* __restrict__ dL_dpixel_extras, float* __restrict__ dL_dextras, int ED) {
+                       const float* __restrict__ dL_dpixel_extras, float* __restrict__ dL_dextras, int ED,
+                       float* __restrict__ part, unsigned char* __restrict__ written) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   WarpSmem& S = reinterpret_cast<WarpSmem*>(smem_raw)[wid];
@@ -201,7 +208,7 @@ render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict_
       if (hf == 0) {
         cp_async16(&S.rec[buf][r][0], src);
         cp_async16(&S.rec[buf][r][2], src + 8);
-        S.gid[buf][r] = id;
+        S.gid[buf][r] = ORDERED ? range.x + pos : id;     // ORDERED: the sorted instance, which names the row
       } else {
         cp_async16(&S.rec[buf][r][3], src + 12);
         cp_async8(&S.rec[buf][r][1], src + 4);
@@ -267,7 +274,19 @@ render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict_
     XH(s0); XH(s1); XH(s2); XH(s3); XH(s4); XH(s5); XH(s6);
     XH(sh); XH(shx); XH(shy); XH(shxx); XH(shxy); XH(shyy); XH(sab);
 #undef XH
-    if (have_rec) {
+    if (ORDERED && have_rec) {
+      const float o = rb.y;
+      const size_t row = (size_t)gid * BWD_WARPS + wid;
+      float4* dst = reinterpret_cast<float4*>(part + row * 16);
+      if (lane < 16) {
+        dst[0] = make_float4(s0, s1, s2, s3);
+        dst[1] = make_float4(s4, s5, s6, -o * fmaf(au, shx, bu * shy));
+        written[row] = 1;
+      } else {
+        dst[2] = make_float4(-o * fmaf(bv, shy, av * shx), fabsf(o) * sab, -0.5f * o * shxx, -0.5f * o * shxy);
+        dst[3] = make_float4(-0.5f * o * shyy, sh, 0.f, 0.f);
+      }
+    } else if (have_rec) {
       const float o = rb.y;
       float* dst;
       if (PEER) {   // the sums of Gaussian gid live on rank gid / per: the reduction itself is the reduce-scatter
@@ -357,7 +376,9 @@ render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict_
       for (int k = 0; k < n_cur; k++) slot(k);
     }
     phase2(n_cur, buf);
-    buf = 1 - buf;                                  // (as buf ^= 1, ptxas spills in two of the three instantiations)
+    // (as buf ^= 1, ptxas spills in two of the three default instantiations; as 1 - buf, it spills one word in the
+    // ORDERED one)
+    buf = ORDERED ? buf ^ 1 : 1 - buf;
     n_cur = n_next;
   }
 }
@@ -365,7 +386,7 @@ render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict_
 }  // namespace
 
 void sfgs_launch_render_bwd(const sfgs_backward_args* a, const GeomLayout& g, const ImageLayout& im,
-                            const BinningLayout& b, float* acc, cudaStream_t st) {
+                            const BinningLayout& b, float* acc, float* part, unsigned char* written, cudaStream_t st) {
   const SfgsBand band = sfgs_band(a->tile_row_begin, a->tile_row_end, im.tiles_y);
   const int band0 = band.b0, band1 = band.b1;
   if (band1 <= band0) return;
@@ -376,6 +397,7 @@ void sfgs_launch_render_bwd(const sfgs_backward_args* a, const GeomLayout& g, co
     cudaFuncSetAttribute(render_bwd_warp_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     cudaFuncSetAttribute(render_bwd_warp_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     cudaFuncSetAttribute(render_bwd_warp_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(render_bwd_warp_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   }
   PeerTable pt = {};
   const bool peer = a->acc_peers != nullptr && a->n_peers > 0;
@@ -383,13 +405,15 @@ void sfgs_launch_render_bwd(const sfgs_backward_args* a, const GeomLayout& g, co
     for (int r = 0; r < a->n_peers && r < 8; r++) pt.p[r] = a->acc_peers[r];
     pt.per = a->peer_slice;
   }
-  // peer reductions belong to the two-phase backward, which rejects extra_attrs (sfgs_rasterize_backward)
-  const auto kernel = a->ED > 0 ? render_bwd_warp_kernel<false, true>
-                      : peer    ? render_bwd_warp_kernel<true, false>
-                                : render_bwd_warp_kernel<false, false>;
+  // peer reductions belong to the two-phase backward, which rejects extra_attrs (sfgs_rasterize_backward); the
+  // ordered path (part != nullptr) rejects both (sfgs_rasterize_backward_deterministic)
+  const auto kernel = part != nullptr ? render_bwd_warp_kernel<false, false, true>
+                      : a->ED > 0     ? render_bwd_warp_kernel<false, true>
+                      : peer          ? render_bwd_warp_kernel<true, false>
+                                      : render_bwd_warp_kernel<false, false>;
   SFGS_COUNT_LAUNCH();
   kernel<<<grid, BWD_THREADS, smem, st>>>(im.ranges, (const char*)b.point_list, im.hdr, a->width, a->height, band0,
                                           a->background, g.rec, a->accum_alphas, im.n_contrib, a->dL_dpix,
                                           a->dL_dpix_depth, a->dL_dpix_norm, a->dL_dpix_alpha, a->norm_raw, acc, pt,
-                                          a->extra_attrs, a->dL_dpix_extra, a->dL_dextra, a->ED);
+                                          a->extra_attrs, a->dL_dpix_extra, a->dL_dextra, a->ED, part, written);
 }

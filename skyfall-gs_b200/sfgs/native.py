@@ -86,7 +86,7 @@ class BinningView(C.Structure):
 ABI_VERSION = 4   # SFGS_VERSION of include/sfgs.h these struct mirrors were written for
 
 EXPORTS = [
-    "sfgs_rasterize_forward", "sfgs_rasterize_backward", "sfgs_mark_visible",
+    "sfgs_rasterize_forward", "sfgs_rasterize_backward", "sfgs_rasterize_backward_deterministic", "sfgs_mark_visible",
     "sfgs_geom_bytes", "sfgs_image_bytes", "sfgs_binning_bytes",
     "sfgs_geom_layout", "sfgs_image_layout", "sfgs_binning_layout", "sfgs_last_capacity",
     "sfgs_fusedssim_forward", "sfgs_fusedssim_backward", "sfgs_dist2_knn3",
@@ -96,7 +96,7 @@ EXPORTS = [
     "sfgs_densification_stats", "sfgs_densify_plan_blocks", "sfgs_densify_plan", "sfgs_densify_apply",
 ]
 STAGE_NAMES = ["fwd_zero", "preprocess", "tile_scan", "emit_keys", "tile_sort", "render_fwd", "bwd_zero", "render_bwd",
-               "gauss_bwd"]
+               "gauss_bwd", "bwd_order"]
 
 _lib = None
 
@@ -115,6 +115,8 @@ def lib() -> C.CDLL:
     L.sfgs_rasterize_forward.restype = C.c_int
     L.sfgs_rasterize_backward.argtypes = [C.POINTER(BackwardArgs)]
     L.sfgs_rasterize_backward.restype = C.c_int
+    L.sfgs_rasterize_backward_deterministic.argtypes = [C.POINTER(BackwardArgs)]
+    L.sfgs_rasterize_backward_deterministic.restype = C.c_int
     L.sfgs_mark_visible.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.sfgs_mark_visible.restype = C.c_int
     L.sfgs_geom_bytes.argtypes = [C.c_int]; L.sfgs_geom_bytes.restype = C.c_size_t

@@ -12,7 +12,9 @@ iteration), and the scratch byte tensors have this library's layout.
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
+import warnings
 
 import torch
 
@@ -145,6 +147,36 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
     return ret + (norm_raw,) if fuse_normalize else ret
 
 
+def _use_deterministic(has_extra, has_peers):
+    """torch.are_deterministic_algorithms_enabled(), checked against the options the deterministic backward lacks:
+    those raise as torch's own ops do, or warn under warn_only=True (and the default backward runs)."""
+    if not torch.are_deterministic_algorithms_enabled():
+        return False
+    what = ["extra_attrs"] * has_extra + ["acc_peers"] * has_peers
+    if not what:
+        return True
+    msg = (f"rasterize_gaussians_backward with {' and '.join(what)} does not have a deterministic implementation, but "
+           "you set 'torch.use_deterministic_algorithms(True)'. You can turn off determinism just for this operation, "
+           "or you can use the 'warn_only=True' option, if that's acceptable for your application.")
+    if torch.is_deterministic_algorithms_warn_only_enabled():
+        warnings.warn(msg)
+        return False
+    raise RuntimeError(msg)
+
+
+@contextlib.contextmanager
+def _no_fill(on):
+    """Deterministic mode makes torch.empty fill new memory (torch.utils.deterministic.fill_uninitialized_memory).
+    Every buffer the backward allocates is written by its kernels before it is read, so with `on` that fill of the
+    outputs and the scratch (about 1.2 GB for a 1080p frame of 1M Gaussians) is skipped."""
+    fill = torch.utils.deterministic.fill_uninitialized_memory
+    torch.utils.deterministic.fill_uninitialized_memory = fill and not on
+    try:
+        yield
+    finally:
+        torch.utils.deterministic.fill_uninitialized_memory = fill
+
+
 def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rotations, extra_attrs, scale_modifier,
                                  cov3Ds_precomp, norm3Ds_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
                                  kernel_size, dL_dout_color, dL_dout_depth, dL_dout_norm, dL_dout_alpha,
@@ -158,11 +190,17 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     Two-phase form for the tile-row sharded multi-GPU mode (include/sfgs.h): `phase=1` runs only the blend adjoint
     of this rank's band and returns the [P,16] sums (`acc`, allocated here unless given); `phase=2` runs only the
     per-Gaussian adjoint for `gauss_range=(begin, end)` from `acc`, whose row 0 is Gaussian `begin` (e.g. a
-    reduce-scatter result), and returns the usual tuple with rows [begin, end) valid."""
+    reduce-scatter result), and returns the usual tuple with rows [begin, end) valid.
+
+    Under `torch.use_deterministic_algorithms(True)` the call runs the deterministic backward
+    (sfgs_rasterize_backward_deterministic): the same outputs up to the order of the sums, bit-identical from run to
+    run.  `extra_attrs` and `acc_peers` have no deterministic implementation: they raise, or with `warn_only=True`
+    warn and run the default backward."""
+    F = int(extra_attrs.shape[1]) if (extra_attrs is not None and extra_attrs.numel() != 0) else 0
+    deterministic = _use_deterministic(F > 0, acc_peers is not None)
     L = N.lib()
     P = int(means3D.shape[0])
     H, W = int(dL_dout_color.shape[1]), int(dL_dout_color.shape[2])
-    F = int(extra_attrs.shape[1]) if (extra_attrs is not None and extra_attrs.numel() != 0) else 0
     M = int(sh.shape[1]) if (sh is not None and sh.numel() != 0) else 0
     dev = means3D.device
     fopt = dict(dtype=torch.float32, device=dev)
@@ -172,7 +210,7 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
         return (z(P, 3), z(P, 3), z(P, 1), z(P, 3), z(P, 6), z(P, 3), z(P, M, 3), z(P, 3), z(P, 4),
                 z(P, F) if F > 0 else torch.empty(0, **fopt))
 
-    with torch.cuda.device(dev):
+    with torch.cuda.device(dev), _no_fill(deterministic):
         # one allocation for all fixed-width per-Gaussian gradients (every element is written by the kernel)
         widths = dict(means3D=3, means2D=3, colors=3, depths=1, conic=4, opacity=1, cov3D=6, norm3D=3, scales=3, rot=4)
         pad = lambda n: (n + 3) & ~3                       # keep every sub-array 16-byte aligned  # noqa: E731
@@ -245,7 +283,14 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
         a.stream = torch.cuda.current_stream(dev).cuda_stream
         if tile_rows is not None:
             a.tile_row_begin, a.tile_row_end = _band(tile_rows)
-        N.check(L.sfgs_rasterize_backward(C.byref(a)), "sfgs_rasterize_backward")
+        if deterministic:
+            N.check(L.sfgs_rasterize_backward_deterministic(C.byref(a)), "sfgs_rasterize_backward_deterministic")
+        else:
+            N.check(L.sfgs_rasterize_backward(C.byref(a)), "sfgs_rasterize_backward")
+        # the arena and its callback form a reference cycle: drop the scratch now (stream-ordered, like any freed
+        # tensor) instead of whenever the garbage collector runs — the deterministic path's scratch is ~0.5 KB per
+        # tile instance
+        scratch.tensor = None
     if phase == 1:
         return acc      # None when the sums went straight to the peers' slices
     return (outs["means2D"], outs["colors"], outs["opacity"], outs["means3D"], outs["cov3D"], outs["norm3D"],
