@@ -3,13 +3,9 @@
 // Replaces BACKWARD::render / renderCUDA (RAST/cuda_rasterizer/backward.cu:509-754), which issues >= 14
 // global float atomicAdd per (pixel, Gaussian) pair.
 //
-// Each warp owns an 8x4 pixel block and runs its own pipeline; nothing in the kernel is block-wide:
+// The tile / block / pixel mapping, the reach-list walk (back to front, from the block's last contributor) and the
+// double-buffered chunk loop are those of sfgs_blend_walk.cuh.  Per 16-record chunk:
 //
-//   scan     the warp walks the tile's sorted list back to front 32 positions at a time (one coalesced read of the
-//            reach masks, see sfgs_common.cuh), keeps the positions whose mask has ITS block's bit (ballot + prefix
-//            popcount into a small ring), and as soon as 16 are collected gathers exactly those 16 records (two lanes
-//            per 64-byte record, cp.async) into its private double-buffered chunk slot — while the previous chunk is
-//            being processed;
 //   phase 1  pixel-parallel (lane = pixel): the per-pixel recursion over the chunk's records in slot order.  The
 //            reference's eight per-channel accumulators collapse into the scalar form
 //                dL/dalpha_j = T_j (g_j - A_j),  g_j = <dL/dpix, attr_j>,  A_j = a_{j+1} g_{j+1} + (1 - a_{j+1}) A_{j+1}
@@ -31,8 +27,8 @@
 //            plain 16-byte stores to its own row of a partial table instead, row (sorted instance) * 8 + block, and
 //            sets that row's written flag; a later pass adds the rows of each Gaussian in a fixed order.
 //
-// Chunks are always full except the last one of a warp.  A record that none of the warp's 32 pixels blends (0.6 % on
-// the benchmark frame: the reach mask is conservative) occupies a slot with zeros.
+// A record that none of the warp's 32 pixels blends (0.6 % on the benchmark frame: the reach mask is conservative)
+// occupies a slot with zeros.
 // (T is recovered back to front as T_j = T_{j+1} * rcp.approx(1 - alpha_{j+1}).  Refining the reciprocal with a Newton step
 // costs time and does NOT change the error statistics against the float64 adjudicator — the worst elements are
 // summation-order noise of ill-conditioned sums, which vary by 5x between runs of either implementation, not T drift.)
@@ -42,12 +38,10 @@
 // the expansion's error was several times the direct sum's for the many small records centred inside the block, and
 // the float64-adjudicated conic gradients (cov3D, scales, rotations) exceeded the reference build's error.  Centred
 // offsets (+-3.5 .. +-0.5, rows +-0.5) bring it back within the reference's error.)
-#include "sfgs_common.cuh"
+#include "sfgs_blend_walk.cuh"
 
 namespace {
 
-constexpr int BWD_THREADS = 256;
-constexpr int BWD_WARPS = BWD_THREADS / 32;
 constexpr int PIXF = 8;           // floats per pixel-table row: dLc[3], dLd, dLn[3], half centre (see below)
 
 // PEER: the target may be another GPU's memory reached over NVLink and every GPU of the node adds into it, so the
@@ -69,14 +63,10 @@ struct PeerTable {
   int per;      // Gaussians per slice
 };
 
-constexpr int W4_CH = 16;
-struct alignas(16) WarpSmem {
-  float4 rec[2][W4_CH][4];      // 2 KB   the chunk's blend records, double buffered; the free word [1].w of a staged
-                                //        record carries its list position (bits of a uint32)
-  uint32_t gid[2][W4_CH];       // Gaussian id of each slot
-  float2 wh[32][W4_CH + 1];     // 4.25 KB phase-1 -> phase-2 hand-over, [pixel][slot], padded
+struct WarpSmem {
+  BlendStage<true> st;          // 2.4 KB the walk's records, ring and gid words
+  float2 wh[32][BLEND_CH + 1];  // 4.25 KB phase-1 -> phase-2 hand-over, [pixel][slot], padded
   float pix[32][PIXF];          // 1 KB    per-pixel cotangents
-  uint32_t list[64];            // ring of collected list positions
 };
 
 // HAS_EXTRA: also the adjoint of the ED channels of `extras` [P,ED] (extra_attrs; Skyfall-GS never passes them):
@@ -86,7 +76,7 @@ struct alignas(16) WarpSmem {
 // of `part` [R*8,16] and written[row] is set; exactly one warp owns each row.  `acc` is not touched.  The slot's gid
 // word carries the sorted instance range.x + list position instead of the Gaussian id (nothing else reads it here).
 template <bool PEER, bool HAS_EXTRA, bool ORDERED = false>
-__global__ void __launch_bounds__(BWD_THREADS, 3)
+__global__ void __launch_bounds__(BLEND_THREADS, 3)
 render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict__ binning_base,
                        const uint32_t* __restrict__ hdr, int W, int H, int band0,
                        const float* __restrict__ bg_color, const float* __restrict__ rec,
@@ -107,24 +97,20 @@ render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict_
   const uint32_t* __restrict__ point_list = bl.point_list;
   const unsigned char* __restrict__ inst_mask = bl.inst_mask;
 
-  const int tiles_x = (W + SFGS_TILE - 1) / SFGS_TILE;
-  const int tile_y = blockIdx.y + band0;
-  const int tile = tile_y * tiles_x + blockIdx.x;
-  const int px = blockIdx.x * SFGS_TILE + (wid & 1) * 8 + (lane & 7);
-  const int py = tile_y * SFGS_TILE + (wid >> 1) * 4 + (lane >> 3);
-  const bool inside = px < W && py < H;
-  const uint32_t pix_id = (uint32_t)W * py + px;
-  const float pixfx = (float)px, pixfy = (float)py;
+  const BlendPixel px(band0, W, H, wid, lane);
+  const bool inside = px.inside;
+  const uint32_t pix_id = px.id;
+  const float pixfx = px.x, pixfy = px.y;
   const size_t HW = (size_t)H * W;
 
-  const uint2 range = ranges[tile];
+  const uint2 range = ranges[px.tile];
   const int total = (int)(range.y - range.x);
   if (total == 0) return;
 
   const float T_final = inside ? (1 - accum_alphas[pix_id]) : 0;
   float T = T_final;
   const uint32_t last_contributor = inside ? n_contrib[pix_id] : 0;
-  // records at list position >= max(last_contributor) over the warp's block are never used by it
+  // records at 1-based list position > max(last_contributor) over the warp's block are never used by it
   uint32_t wmax = last_contributor;
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) wmax = max(wmax, __shfl_xor_sync(0xffffffffu, wmax, o));
@@ -180,61 +166,22 @@ render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict_
   // extras' recursion only
   float C = 0.f, last_alpha = 0.f;
   const SfgsExpConsts ek = sfgs_exp_consts(hdr[HDR_ZERO]);
-  const unsigned lt_mask = (1u << lane) - 1u;
-
-  // ---- scan + gather of the next chunk into buffer `buf`; returns the number of records in it (0 = list exhausted)
-  int p = used;                    // positions [0, p) are still unscanned; the next window is p-1 ... p-32
-  int head = 0, have = 0;          // ring of collected positions: [head, head + have)
-  auto scan_gather = [&](int buf) -> int {
-    while (have < W4_CH && p > 0) {
-      const int pos = p - 1 - lane;
-      unsigned m = 0;
-      if (pos >= 0) m = inst_mask[range.x + pos];
-      const bool bit = (m >> wid) & 1u;
-      const unsigned b = __ballot_sync(0xffffffffu, bit);
-      if (bit) S.list[(head + have + __popc(b & lt_mask)) & 63] = (uint32_t)pos;   // lane 0 = highest position first
-      have += __popc(b);
-      p -= 32;
-    }
-    __syncwarp();
-    const int n = min(have, W4_CH);
-    if (lane < 2 * n) {              // two lanes per 64-byte record
-      const int r = lane >> 1, hf = lane & 1;
-      const uint32_t pos = S.list[(head + r) & 63];
-      const uint32_t id = point_list[range.x + pos];
-      const float* src = rec + (size_t)id * REC_FLOATS;
-      // the record's second quad is (con.z, opacity, depth, free): it is copied as 8 + 4 bytes and the free word takes
-      // the list position, so phase 1 finds every per-record value it needs at an immediate offset of one base
-      if (hf == 0) {
-        cp_async16(&S.rec[buf][r][0], src);
-        cp_async16(&S.rec[buf][r][2], src + 8);
-        S.gid[buf][r] = ORDERED ? range.x + pos : id;     // ORDERED: the sorted instance, which names the row
-      } else {
-        cp_async16(&S.rec[buf][r][3], src + 12);
-        cp_async8(&S.rec[buf][r][1], src + 4);
-        cp_async4(&S.rec[buf][r][1].z, src + 6);
-        S.rec[buf][r][1].w = __uint_as_float(pos);
-      }
-    }
-    cp_async_commit();
-    head = (head + n) & 63;
-    have -= n;
-    return n;
-  };
+  BlendWalk<true, ORDERED ? GID_INSTANCE : GID_GAUSSIAN> walk(S.st, inst_mask, point_list, rec, range, used, wid,
+                                                               lane);
 
   // ---- phase 2: lane (k = lane & 15, half = lane >> 4) sums slot k of the chunk over pixels half*16 .. +15.  The
   // half is 8 x 2 pixels; in coordinates centred on it, its pixel i sits at the compile-time offset
   // (x, y) = ((i & 7) - 3.5, (i >> 3) - 0.5).  The loop sums h against those constants, and the moments about the
   // record's centre (dx = DX - x, dy = DY - y, where (DX, DY) = record centre - half centre) follow once per chunk
   // (see the numerics note at the top).
-  const int ck = lane & (W4_CH - 1), chalf = lane >> 4;
-  auto phase2 = [&](int n, int buf) {
+  const int ck = lane & (BLEND_CH - 1), chalf = lane >> 4;
+  auto phase2 = [&](int buf, int n) {
     __syncwarp();
     const bool have_rec = ck < n;
     const int slot = have_rec ? ck : 0;          // idle lanes shadow slot 0 (always valid, n >= 1)
-    const float4 ra = S.rec[buf][slot][0];      // mx, my, con.x, con.y
-    const float4 rb = S.rec[buf][slot][1];      // con.z, opac, depth
-    const uint32_t gid = S.gid[buf][slot];
+    const float4 ra = S.st.rec[buf][slot][0];   // mx, my, con.x, con.y
+    const float4 rb = S.st.rec[buf][slot][1];   // con.z, opac, depth
+    const uint32_t gid = S.st.gid[buf][slot];
     const float2* whp = &S.wh[chalf * 16][ck];
     const float4* pix = reinterpret_cast<const float4*>(&S.pix[chalf * 16][0]);
     const float DX = ra.x - pix[1].w, DY = ra.y - pix[3].w;
@@ -251,7 +198,7 @@ render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict_
     for (int i = 0; i < 16; i++) {
       const float x = (float)(i & 7) - 3.5f;
       const int r = i >> 3;
-      const float2 wh = whp[i * (W4_CH + 1)];
+      const float2 wh = whp[i * (BLEND_CH + 1)];
       const float4 p0 = pix[2 * i], p1 = pix[2 * i + 1];
       s0 = fmaf(wh.x, p0.x, s0); s1 = fmaf(wh.x, p0.y, s1); s2 = fmaf(wh.x, p0.z, s2); s3 = fmaf(wh.x, p0.w, s3);
       s4 = fmaf(wh.x, p1.x, s4); s5 = fmaf(wh.x, p1.y, s5); s6 = fmaf(wh.x, p1.z, s6);
@@ -276,7 +223,7 @@ render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict_
 #undef XH
     if (ORDERED && have_rec) {
       const float o = rb.y;
-      const size_t row = (size_t)gid * BWD_WARPS + wid;
+      const size_t row = (size_t)gid * BLEND_WARPS + wid;
       float4* dst = reinterpret_cast<float4*>(part + row * 16);
       if (lane < 16) {
         dst[0] = make_float4(s0, s1, s2, s3);
@@ -307,91 +254,79 @@ render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict_
     __syncwarp();
   };
 
-  int buf = 0;
-  int n_cur = scan_gather(0);
-  while (n_cur > 0) {
-    cp_async_wait_all();
-    __syncwarp();                                   // chunk `buf` has landed and is visible to the whole warp
-    const int n_next = scan_gather(buf ^ 1);        // the next chunk's gather overlaps the math below
-    // ---- phase 1: pixel-parallel recursion over the chunk's records, slot order = back to front.  Branch-free: a
-    // chunk is one basic block, so the scheduler can overlap slot k+1's load -> exp chain with slot k's recursion (a
-    // (block, record) pair that no pixel blends is 0.6 % of the pairs: the work a branch would skip is negligible, the
-    // selects cost what the branch bookkeeping did)
-    auto slot_body = [&](const int k, const float4 ra, const float4 rb) {
-      const float dx = ra.x - pixfx, dy = ra.y - pixfy;
-      const float power = -0.5f * (ra.z * dx * dx + rb.x * dy * dy) - ra.w * dx * dy;
-      const float G = sfgs_expf(power, ek);
-      const float alpha = min(0.99f, rb.y * G);
-      const bool active = (__float_as_uint(rb.w) < last_contributor) && !(power > 0.0f) && !(alpha < 1.0f / 255.0f);
-      const float4 rc = S.rec[buf][k][2];       // r, g, b, nx
-      const float4 rd = S.rec[buf][k][3];       // ny, nz
-      // 1 - alpha is in [0.01, 1]: the approximate reciprocal (1 ulp, one MUFU) needs no range fix-up; it is shared
-      // by the T recovery and the background term
-      const float one_m_alpha = 1.f - alpha;
-      float inv_1ma;
-      asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(inv_1ma) : "f"(one_m_alpha));
-      const float Tn = T * inv_1ma;
-      // two independent chains: halves the dependent-FMA latency of the dot product
-      float g = rc.x * dLc0, g2 = rc.w * dLn0;
-      g += rc.y * dLc1; g2 += rd.x * dLn1;
-      g += rc.z * dLc2; g2 += rd.y * dLn2;
-      g += rb.z * dLd;  g2 += dLa;
-      g += g2;
-      float dL_dalpha_T = g - C;                  // dL/dalpha / T
-      if constexpr (HAS_EXTRA) {
-        const uint32_t gid = S.gid[buf][k];
-        for (int ch = 0; ch < ED; ch++) {
-          const float ex = extras[(size_t)gid * ED + ch];
-          const float ree = last_alpha * last_extra[ch] + (1.f - last_alpha) * accum_ree[ch];
-          dL_dalpha_T += (ex - ree) * dL_dpixel_extra[ch];
-          accum_ree[ch] = active ? ree : accum_ree[ch];
-          last_extra[ch] = active ? ex : last_extra[ch];
-          if (active) atomicAdd(&dL_dextras[(size_t)gid * ED + ch], alpha * Tn * dL_dpixel_extra[ch]);
-        }
-        last_alpha = active ? alpha : last_alpha;
+  // ---- phase 1: pixel-parallel recursion over the chunk's records, slot order = back to front.  Branch-free: a
+  // chunk is one basic block, so the scheduler can overlap slot k+1's load -> exp chain with slot k's recursion (a
+  // (block, record) pair that no pixel blends is 0.6 % of the pairs: the work a branch would skip is negligible, the
+  // selects cost what the branch bookkeeping did)
+  auto slot = [&](const int buf, const int k, const float4 ra /* mx, my, con.x, con.y */,
+                  const float4 rb /* con.z, opac, depth, 1-based list position */) {
+    const float dx = ra.x - pixfx, dy = ra.y - pixfy;
+    const float power = -0.5f * (ra.z * dx * dx + rb.x * dy * dy) - ra.w * dx * dy;
+    const float G = sfgs_expf(power, ek);
+    const float alpha = min(0.99f, rb.y * G);
+    const bool active = (__float_as_uint(rb.w) <= last_contributor) && !(power > 0.0f) && !(alpha < 1.0f / 255.0f);
+    const float4 rc = S.st.rec[buf][k][2];    // r, g, b, nx
+    const float4 rd = S.st.rec[buf][k][3];    // ny, nz
+    // 1 - alpha is in [0.01, 1]: the approximate reciprocal (1 ulp, one MUFU) needs no range fix-up; it is shared
+    // by the T recovery and the background term
+    const float one_m_alpha = 1.f - alpha;
+    float inv_1ma;
+    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(inv_1ma) : "f"(one_m_alpha));
+    const float Tn = T * inv_1ma;
+    // two independent chains: halves the dependent-FMA latency of the dot product
+    float g = rc.x * dLc0, g2 = rc.w * dLn0;
+    g += rc.y * dLc1; g2 += rd.x * dLn1;
+    g += rc.z * dLc2; g2 += rd.y * dLn2;
+    g += rb.z * dLd;  g2 += dLa;
+    g += g2;
+    float dL_dalpha_T = g - C;                  // dL/dalpha / T
+    if constexpr (HAS_EXTRA) {
+      const uint32_t gid = S.st.gid[buf][k];
+      for (int ch = 0; ch < ED; ch++) {
+        const float ex = extras[(size_t)gid * ED + ch];
+        const float ree = last_alpha * last_extra[ch] + (1.f - last_alpha) * accum_ree[ch];
+        dL_dalpha_T += (ex - ree) * dL_dpixel_extra[ch];
+        accum_ree[ch] = active ? ree : accum_ree[ch];
+        last_extra[ch] = active ? ex : last_extra[ch];
+        if (active) atomicAdd(&dL_dextras[(size_t)gid * ED + ch], alpha * Tn * dL_dpixel_extra[ch]);
       }
-      const float dL_dalpha = fmaf(tb, inv_1ma, Tn * dL_dalpha_T);
-      const float w_out = active ? alpha * Tn : 0.f;
-      const float h_out = active ? G * dL_dalpha : 0.f;
-      T = active ? Tn : T;
-      // the roundings of forming A from (A, g_last, last_alpha) at the next record: (1 - alpha) * C, then one FMA
-      C = active ? fmaf(alpha, g, __fmul_rn(one_m_alpha, C)) : C;
-      S.wh[lane][k] = make_float2(w_out, h_out);
-    };
-    auto slot = [&](const int k) {
-      slot_body(k, S.rec[buf][k][0] /* mx, my, con.x, con.y */, S.rec[buf][k][1] /* con.z, opac, depth, list position */);
-    };
-    if (n_cur == W4_CH) {                           // every chunk of a warp but its last: no per-slot bound test
+      last_alpha = active ? alpha : last_alpha;
+    }
+    const float dL_dalpha = fmaf(tb, inv_1ma, Tn * dL_dalpha_T);
+    const float w_out = active ? alpha * Tn : 0.f;
+    const float h_out = active ? G * dL_dalpha : 0.f;
+    T = active ? Tn : T;
+    // the roundings of forming A from (A, g_last, last_alpha) at the next record: (1 - alpha) * C, then one FMA
+    C = active ? fmaf(alpha, g, __fmul_rn(one_m_alpha, C)) : C;
+    S.wh[lane][k] = make_float2(w_out, h_out);
+  };
+  blend_chunks<ORDERED>(walk, [] { return false; }, [&](const int buf, const int n) {
+    if (n == BLEND_CH) {                            // every chunk of a warp but its last: no per-slot bound test
       // slot k+1's parameters are read before slot k's hand-over store (the compiler cannot move a shared-memory
       // load above that store on its own), so their latency overlaps slot k's arithmetic
-      float4 ra_n = S.rec[buf][0][0], rb_n = S.rec[buf][0][1];
+      float4 ra_n = S.st.rec[buf][0][0], rb_n = S.st.rec[buf][0][1];
 #pragma unroll
-      for (int k = 0; k < W4_CH; k++) {
+      for (int k = 0; k < BLEND_CH; k++) {
         const float4 ra = ra_n, rb = rb_n;
-        if (k + 1 < W4_CH) { ra_n = S.rec[buf][k + 1][0]; rb_n = S.rec[buf][k + 1][1]; }
-        slot_body(k, ra, rb);
+        if (k + 1 < BLEND_CH) { ra_n = S.st.rec[buf][k + 1][0]; rb_n = S.st.rec[buf][k + 1][1]; }
+        slot(buf, k, ra, rb);
       }
     } else {
 #pragma unroll 1
-      for (int k = 0; k < n_cur; k++) slot(k);
+      for (int k = 0; k < n; k++) slot(buf, k, S.st.rec[buf][k][0], S.st.rec[buf][k][1]);
     }
-    phase2(n_cur, buf);
-    // (as buf ^= 1, ptxas spills in two of the three default instantiations; as 1 - buf, it spills one word in the
-    // ORDERED one)
-    buf = ORDERED ? buf ^ 1 : 1 - buf;
-    n_cur = n_next;
-  }
+    phase2(buf, n);
+  });
 }
 
 }  // namespace
 
 void sfgs_launch_render_bwd(const sfgs_backward_args* a, const GeomLayout& g, const ImageLayout& im,
                             const BinningLayout& b, float* acc, float* part, unsigned char* written, cudaStream_t st) {
-  const SfgsBand band = sfgs_band(a->tile_row_begin, a->tile_row_end, im.tiles_y);
-  const int band0 = band.b0, band1 = band.b1;
-  if (band1 <= band0) return;
-  dim3 grid(im.tiles_x, band1 - band0, 1);
-  const size_t smem = sizeof(WarpSmem) * BWD_WARPS;
+  dim3 grid;
+  int band0;
+  if (!blend_grid(a->tile_row_begin, a->tile_row_end, im, grid, band0)) return;
+  const size_t smem = sizeof(WarpSmem) * BLEND_WARPS;
   static SfgsPerDeviceOnce attr_once;   // function attributes are per device
   if (attr_once.first_use()) {
     cudaFuncSetAttribute(render_bwd_warp_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -412,7 +347,7 @@ void sfgs_launch_render_bwd(const sfgs_backward_args* a, const GeomLayout& g, co
                       : peer          ? render_bwd_warp_kernel<true, false>
                                       : render_bwd_warp_kernel<false, false>;
   SFGS_COUNT_LAUNCH();
-  kernel<<<grid, BWD_THREADS, smem, st>>>(im.ranges, (const char*)b.point_list, im.hdr, a->width, a->height, band0,
+  kernel<<<grid, BLEND_THREADS, smem, st>>>(im.ranges, (const char*)b.point_list, im.hdr, a->width, a->height, band0,
                                           a->background, g.rec, a->accum_alphas, im.n_contrib, a->dL_dpix,
                                           a->dL_dpix_depth, a->dL_dpix_norm, a->dL_dpix_alpha, a->norm_raw, acc, pt,
                                           a->extra_attrs, a->dL_dpix_extra, a->dL_dextra, a->ED, part, written);
