@@ -202,6 +202,21 @@ int sfgs_rasterize_backward(const sfgs_backward_args* a);
  * The outputs equal sfgs_rasterize_backward's up to the rounding of the sums' order. */
 int sfgs_rasterize_backward_deterministic(const sfgs_backward_args* a);
 
+/* ---- subpixel offsets (Mip-Splatting's ray jitter: GaussianRasterizationSettings.subpixel_offset) -------------
+ * The three calls above with per-pixel sample positions: pixel (x, y) (centres at integer coordinates) blends the
+ * splats of its own tile's list at (x + off[y][x][0], y + off[y][x][1]).  subpixel_offset is a DEVICE [H,W,2] float
+ * array indexed by the full-frame pixel (also under a tile-row band); NULL means exactly the call without the suffix.
+ *   - Tile lists are not changed: radii, tiles_touched, keys, point_list and ranges are those of the call without
+ *     offsets.  Every per-pixel rule (power > 0 and alpha < 1/255 skips, the T < 1e-4 stop, n_contrib, background)
+ *     is unchanged; only the sample position moves.
+ *   - Any finite offset is allowed; a NaN or Inf offset makes the forward return SFGS_E_BADARG.
+ *   - No gradient is formed with respect to the offsets.
+ *   - The backward must get the same buffer, with the same contents, as the forward (like norm_raw).
+ *   - ED > 0 (extra_attrs), out_peers and acc_peers return SFGS_E_UNSUPPORTED before any CUDA work. */
+int sfgs_rasterize_forward_subpixel(const sfgs_forward_args* a, const float* subpixel_offset);
+int sfgs_rasterize_backward_subpixel(const sfgs_backward_args* a, const float* subpixel_offset);
+int sfgs_rasterize_backward_deterministic_subpixel(const sfgs_backward_args* a, const float* subpixel_offset);
+
 /* ---- markVisible --------------------------------------------------------- */
 int sfgs_mark_visible(int P, const float* means3D, const float* viewmatrix,
                       const float* projmatrix, unsigned char* present, void* stream);

@@ -30,12 +30,15 @@ void sfgs_launch_mark_visible(int P, const float* means3D, const float* viewmatr
                               cudaStream_t st);
 void sfgs_launch_tile_scan(const ImageLayout& im, unsigned long long capacity, cudaStream_t st);
 void sfgs_launch_scatter(const GeomLayout& g, const ImageLayout& im, const BinningLayout& b, int P,
-                         unsigned long long capacity, cudaStream_t st);
-void sfgs_launch_tile_sort(const GeomLayout& g, const ImageLayout& im, const BinningLayout& b, int P, cudaStream_t st);
+                         unsigned long long capacity, bool dilate, cudaStream_t st);
+void sfgs_launch_tile_sort(const GeomLayout& g, const ImageLayout& im, const BinningLayout& b, int P, bool dilate,
+                           cudaStream_t st);
+void sfgs_launch_offset_bound(const ImageLayout& im, int W, int H, const float* off, cudaStream_t st);
 void sfgs_launch_render_fwd(const sfgs_forward_args* a, const GeomLayout& g, const ImageLayout& im,
-                            const BinningLayout& b, cudaStream_t st);
+                            const BinningLayout& b, const float* off, cudaStream_t st);
 void sfgs_launch_render_bwd(const sfgs_backward_args* a, const GeomLayout& g, const ImageLayout& im,
-                            const BinningLayout& b, float* acc, float* part, unsigned char* written, cudaStream_t st);
+                            const BinningLayout& b, float* acc, float* part, unsigned char* written, const float* off,
+                            cudaStream_t st);
 size_t sfgs_order_scratch_bytes(int P, long long R);
 SfgsOrderScratch sfgs_order_scratch(char* base, int P, long long R);
 void sfgs_launch_order_prepare(int P, const GeomLayout& g, const ImageLayout& im, const BinningLayout& b,
@@ -188,7 +191,20 @@ struct PinnedHdr {
 constexpr int MAX_DEVICES = 64;
 thread_local PinnedHdr t_hdr_dev[MAX_DEVICES];
 
-int rasterize_backward(const sfgs_backward_args* a, bool deterministic);
+int rasterize_forward(const sfgs_forward_args* a, const float* off);
+int rasterize_backward(const sfgs_backward_args* a, bool deterministic, const float* off);
+
+// the combinations the subpixel-offset entry points have no kernels for (checked before any CUDA work)
+int subpixel_unsupported_fwd(const sfgs_forward_args* a) {
+  if (a->ED > 0) return fail(SFGS_E_UNSUPPORTED, "forward_subpixel: extra_attrs are not supported with subpixel offsets");
+  if (a->out_peers != nullptr) return fail(SFGS_E_UNSUPPORTED, "forward_subpixel: out_peers are not supported with subpixel offsets");
+  return SFGS_OK;
+}
+int subpixel_unsupported_bwd(const sfgs_backward_args* a) {
+  if (a->ED > 0) return fail(SFGS_E_UNSUPPORTED, "backward_subpixel: extra_attrs are not supported with subpixel offsets");
+  if (a->acc_peers != nullptr) return fail(SFGS_E_UNSUPPORTED, "backward_subpixel: acc_peers are not supported with subpixel offsets");
+  return SFGS_OK;
+}
 
 }  // namespace
 
@@ -226,7 +242,31 @@ int sfgs_binning_layout(char* base, long long capacity, sfgs_binning_view* out) 
   return SFGS_OK;
 }
 
-int sfgs_rasterize_forward(const sfgs_forward_args* a) {
+int sfgs_rasterize_forward(const sfgs_forward_args* a) { return rasterize_forward(a, nullptr); }
+int sfgs_rasterize_backward(const sfgs_backward_args* a) { return rasterize_backward(a, false, nullptr); }
+int sfgs_rasterize_backward_deterministic(const sfgs_backward_args* a) { return rasterize_backward(a, true, nullptr); }
+
+int sfgs_rasterize_forward_subpixel(const sfgs_forward_args* a, const float* subpixel_offset) {
+  if (!a) return fail(SFGS_E_BADARG, "forward: null args");
+  if (subpixel_offset != nullptr && subpixel_unsupported_fwd(a)) return SFGS_E_UNSUPPORTED;
+  return rasterize_forward(a, subpixel_offset);
+}
+int sfgs_rasterize_backward_subpixel(const sfgs_backward_args* a, const float* subpixel_offset) {
+  if (!a) return fail(SFGS_E_BADARG, "backward: null args");
+  if (subpixel_offset != nullptr && subpixel_unsupported_bwd(a)) return SFGS_E_UNSUPPORTED;
+  return rasterize_backward(a, false, subpixel_offset);
+}
+int sfgs_rasterize_backward_deterministic_subpixel(const sfgs_backward_args* a, const float* subpixel_offset) {
+  if (!a) return fail(SFGS_E_BADARG, "backward: null args");
+  if (subpixel_offset != nullptr && subpixel_unsupported_bwd(a)) return SFGS_E_UNSUPPORTED;
+  return rasterize_backward(a, true, subpixel_offset);
+}
+
+}  // extern "C"
+
+namespace {
+
+int rasterize_forward(const sfgs_forward_args* a, const float* off) {
   if (!a) return fail(SFGS_E_BADARG, "forward: null args");
   if (a->P < 0 || a->width <= 0 || a->height <= 0) return fail(SFGS_E_BADARG, "forward: bad sizes");
   if (a->ED < 0 || a->ED > SFGS_MAX_EXTRA) return fail(SFGS_E_BADARG, "forward: ED out of range");
@@ -287,6 +327,7 @@ int sfgs_rasterize_forward(const sfgs_forward_args* a) {
     // tile histogram + header start at zero
     PROF_BEGIN(ST_FWD_ZERO);
     CU(cudaMemsetAsync(im.hdr, 0, im.zero_bytes, st));   // header + tile histogram are adjacent
+    if (off) sfgs_launch_offset_bound(im, a->width, a->height, off, st);   // the masks' dilation, before the key scatter
     PROF_END();
 
     if (P > 0) {
@@ -301,20 +342,20 @@ int sfgs_rasterize_forward(const sfgs_forward_args* a) {
     STAGE_CHECK("tile_scan");
     // num_rendered and the overflow flag are final after the scan: start their copy now and let the host wait
     // on this event only, so it returns (and the caller can queue the backward) while sort + blend still run
-    CU(cudaMemcpyAsync(hhdr, im.hdr, 8 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(hhdr, im.hdr, HDR_COPY_WORDS * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
     CU(cudaEventRecord(t_hdr.ev, st));
     if (P > 0) {
       PROF_BEGIN(ST_EMIT);
-      sfgs_launch_scatter(g, im, b, a->P, (unsigned long long)capacity, st);
+      sfgs_launch_scatter(g, im, b, a->P, (unsigned long long)capacity, off != nullptr, st);
       PROF_END();
       STAGE_CHECK("scatter_keys");
       PROF_BEGIN(ST_SORT);
-      sfgs_launch_tile_sort(g, im, b, a->P, st);
+      sfgs_launch_tile_sort(g, im, b, a->P, off != nullptr, st);
       PROF_END();
       STAGE_CHECK("tile_sort");
     }
     PROF_BEGIN(ST_RENDER_FWD);
-    sfgs_launch_render_fwd(a, g, im, b, st);
+    sfgs_launch_render_fwd(a, g, im, b, off, st);
     PROF_END();
     STAGE_CHECK("render_fwd");
 
@@ -324,6 +365,7 @@ int sfgs_rasterize_forward(const sfgs_forward_args* a) {
     // the reference's checkFrustum traps the kernel when `prefiltered` is set and a point fails the test
     // (RAST/cuda_rasterizer/auxiliary.h:157-161); here the frame is reported as an argument error instead
     if (hhdr[HDR_PREFILTER]) return fail(SFGS_E_BADARG, "forward: prefiltered was set but a Gaussian failed the frustum test");
+    if (hhdr[HDR_OFF_BAD]) return fail(SFGS_E_BADARG, "forward_subpixel: a subpixel offset is NaN or Inf");
     if (!hhdr[HDR_OVERFLOW]) break;
     if (attempt == 2) return fail(SFGS_E_CUDA, "forward: binning capacity overflow persisted");
     capacity = R + R / 16 + 4096;   // the exact count is now known; run the pipeline again with room for it
@@ -334,14 +376,7 @@ int sfgs_rasterize_forward(const sfgs_forward_args* a) {
   return (int)R;
 }
 
-int sfgs_rasterize_backward(const sfgs_backward_args* a) { return rasterize_backward(a, false); }
-int sfgs_rasterize_backward_deterministic(const sfgs_backward_args* a) { return rasterize_backward(a, true); }
-
-}  // extern "C"
-
-namespace {
-
-int rasterize_backward(const sfgs_backward_args* a, bool deterministic) {
+int rasterize_backward(const sfgs_backward_args* a, bool deterministic, const float* off) {
   if (!a) return fail(SFGS_E_BADARG, "backward: null args");
   if (a->P < 0 || a->width <= 0 || a->height <= 0) return fail(SFGS_E_BADARG, "backward: bad sizes");
   if (deterministic && a->acc_peers != nullptr)
@@ -416,7 +451,7 @@ int rasterize_backward(const sfgs_backward_args* a, bool deterministic) {
     PROF_END();
     if (R > 0) {
       PROF_BEGIN(ST_RENDER_BWD);
-      sfgs_launch_render_bwd(a, g, im, b, acc, order.part, order.written, st);
+      sfgs_launch_render_bwd(a, g, im, b, acc, order.part, order.written, off, st);
       PROF_END();
       STAGE_CHECK("render_bwd");
     }
@@ -439,7 +474,7 @@ int rasterize_backward(const sfgs_backward_args* a, bool deterministic) {
     PROF_END();
     if (a->R > 0) {
       PROF_BEGIN(ST_RENDER_BWD);
-      sfgs_launch_render_bwd(a, g, im, b, acc, nullptr, nullptr, st);
+      sfgs_launch_render_bwd(a, g, im, b, acc, nullptr, nullptr, off, st);
       PROF_END();
       STAGE_CHECK("render_bwd");
     }

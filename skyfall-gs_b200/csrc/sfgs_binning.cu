@@ -109,10 +109,11 @@ tile_scan_kernel(int tiles, const uint32_t* __restrict__ tile_count, uint2* __re
 // With P >= 2^24 the key stays depth_bits << 32 | id and the sort kernels compute the masks as before.
 // ITEMS: instances per thread (independent loads in flight).  With the mask the kernel needs ~36 live floats per
 // instance in flight, so the packed path runs two per thread; the unpacked path forms no mask and runs four.
-template <bool PACK, int ITEMS>
-__global__ void __launch_bounds__(256)
-scatter_keys_kernel(const uint4* __restrict__ tmp, const uint2* __restrict__ ranges, uint32_t* __restrict__ tile_count,
-                    const uint32_t* __restrict__ hdr, const float* __restrict__ rec, int gx, uint64_t* __restrict__ keys) {
+// DILATE: the reach masks of a forward with subpixel offsets (reach_mask_t, sfgs_common.cuh).
+template <bool PACK, int ITEMS, bool DILATE>
+__device__ __forceinline__ void scatter_keys(const uint4* __restrict__ tmp, const uint2* __restrict__ ranges,
+                                             uint32_t* __restrict__ tile_count, const uint32_t* __restrict__ hdr,
+                                             const float* __restrict__ rec, int gx, uint64_t* __restrict__ keys) {
   if (hdr[HDR_OVERFLOW]) return;
   const uint32_t R = hdr[HDR_R];
   const uint32_t i0 = blockIdx.x * (256u * ITEMS) + threadIdx.x;
@@ -141,10 +142,25 @@ scatter_keys_kernel(const uint4* __restrict__ tmp, const uint2* __restrict__ ran
       uint32_t lo = t[u].x;
       if (PACK) {
         const int tile_px = (int)(t[u].z % (uint32_t)gx) * SFGS_TILE, tile_py = (int)(t[u].z / (uint32_t)gx) * SFGS_TILE;
-        lo = (t[u].x << 8) | reach_mask(r0[u].x, r0[u].y, r0[u].z, r0[u].w, r1[u].x, r1[u].y, tile_px, tile_py);
+        const float2 e = DILATE ? sfgs_offset_bound(hdr) : make_float2(0.f, 0.f);
+        lo = (t[u].x << 8) |
+             reach_mask_t<DILATE>(r0[u].x, r0[u].y, r0[u].z, r0[u].w, r1[u].x, r1[u].y, tile_px, tile_py, e.x, e.y);
       }
       keys[start[u] + slot[u]] = ((uint64_t)t[u].y << 32) | lo;
     }
+}
+template <bool PACK, int ITEMS>
+__global__ void __launch_bounds__(256)
+scatter_keys_kernel(const uint4* __restrict__ tmp, const uint2* __restrict__ ranges, uint32_t* __restrict__ tile_count,
+                    const uint32_t* __restrict__ hdr, const float* __restrict__ rec, int gx, uint64_t* __restrict__ keys) {
+  scatter_keys<PACK, ITEMS, false>(tmp, ranges, tile_count, hdr, rec, gx, keys);
+}
+// the packed path with subpixel offsets (the unpacked scatter forms no masks: it serves both)
+__global__ void __launch_bounds__(256)
+scatter_keys_dilated_kernel(const uint4* __restrict__ tmp, const uint2* __restrict__ ranges,
+                            uint32_t* __restrict__ tile_count, const uint32_t* __restrict__ hdr,
+                            const float* __restrict__ rec, int gx, uint64_t* __restrict__ keys) {
+  scatter_keys<true, 2, true>(tmp, ranges, tile_count, hdr, rec, gx, keys);
 }
 
 // ---- per-tile sort -------------------------------------------------------------
@@ -297,10 +313,13 @@ __device__ __forceinline__ uint64_t key_unpack(uint64_t k) { return (k & 0xfffff
 
 // Output of one sorted tile list: Gaussian ids, reach masks, and the sorted keys in canonical form.
 // PADDED: `sorted` is a shared-memory sort buffer (PADIDX layout); otherwise plain memory.
-template <bool PACK, int STRIDE, bool PADDED>
+// DILATE (unpacked path only): the reach masks of a forward with subpixel offsets, dilated by the bound in the image
+// header.
+template <bool PACK, int STRIDE, bool PADDED, bool DILATE = false>
 __device__ __forceinline__ void emit_sorted(const uint64_t* sorted, uint64_t* bucket, int n, int first, uint32_t base,
                                             uint32_t* __restrict__ point_list, unsigned char* __restrict__ inst_mask,
-                                            const float* __restrict__ rec, int tile, int gx) {
+                                            const float* __restrict__ rec, int tile, int gx,
+                                            const uint32_t* __restrict__ hdr = nullptr) {
   const int tile_px = (tile % gx) * SFGS_TILE, tile_py = (tile / gx) * SFGS_TILE;
   for (int i = first; i < n; i += STRIDE) {
     const uint64_t k = sorted[PADDED ? PADIDX(i) : i];
@@ -314,7 +333,9 @@ __device__ __forceinline__ void emit_sorted(const uint64_t* sorted, uint64_t* bu
       point_list[base + i] = id;
       const float4 r0 = *reinterpret_cast<const float4*>(rec + (size_t)id * REC_FLOATS);
       const float2 r1 = *reinterpret_cast<const float2*>(rec + (size_t)id * REC_FLOATS + 4);
-      inst_mask[base + i] = (unsigned char)reach_mask(r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, tile_px, tile_py);
+      const float2 e = DILATE ? sfgs_offset_bound(hdr) : make_float2(0.f, 0.f);
+      inst_mask[base + i] =
+          (unsigned char)reach_mask_t<DILATE>(r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, tile_px, tile_py, e.x, e.y);
     }
   }
 }
@@ -410,11 +431,11 @@ __device__ __forceinline__ void warp_merge_sort(uint64_t* buf, const uint64_t* _
   }
 }
 
-template <bool PACK>
-__global__ void __launch_bounds__(WS_WARPS * 32)
-tile_sort_warp_kernel(int tiles, const uint2* __restrict__ ranges, const uint32_t* __restrict__ hdr, uint64_t* __restrict__ keys,
-                      uint32_t* __restrict__ point_list, const float* __restrict__ rec, int gx,
-                      unsigned char* __restrict__ inst_mask) {
+template <bool PACK, bool DILATE>
+__device__ __forceinline__ void tile_sort_warp(int tiles, const uint2* __restrict__ ranges, const uint32_t* __restrict__ hdr,
+                                               uint64_t* __restrict__ keys, uint32_t* __restrict__ point_list,
+                                               const float* __restrict__ rec, int gx,
+                                               unsigned char* __restrict__ inst_mask) {
   if (hdr[HDR_OVERFLOW]) return;
   __shared__ __align__(16) uint64_t s_keys[WS_WARPS][WS_MAX + WS_MAX / 16];      // 17 KB
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -428,7 +449,21 @@ tile_sort_warp_kernel(int tiles, const uint2* __restrict__ ranges, const uint32_
   if (n <= 32 * 4) warp_merge_sort<4>(buf, bucket, n, lane);
   else if (n <= 32 * 8) warp_merge_sort<8>(buf, bucket, n, lane);
   else warp_merge_sort<16>(buf, bucket, n, lane);
-  emit_sorted<PACK, 32, true>(buf, bucket, n, lane, rg.x, point_list, inst_mask, rec, tile, gx);
+  emit_sorted<PACK, 32, true, DILATE>(buf, bucket, n, lane, rg.x, point_list, inst_mask, rec, tile, gx, hdr);
+}
+template <bool PACK>
+__global__ void __launch_bounds__(WS_WARPS * 32)
+tile_sort_warp_kernel(int tiles, const uint2* __restrict__ ranges, const uint32_t* __restrict__ hdr, uint64_t* __restrict__ keys,
+                      uint32_t* __restrict__ point_list, const float* __restrict__ rec, int gx,
+                      unsigned char* __restrict__ inst_mask) {
+  tile_sort_warp<PACK, false>(tiles, ranges, hdr, keys, point_list, rec, gx, inst_mask);
+}
+// the unpacked path with subpixel offsets (the packed path's masks come from the dilated key scatter)
+__global__ void __launch_bounds__(WS_WARPS * 32)
+tile_sort_warp_dilated_kernel(int tiles, const uint2* __restrict__ ranges, const uint32_t* __restrict__ hdr,
+                              uint64_t* __restrict__ keys, uint32_t* __restrict__ point_list,
+                              const float* __restrict__ rec, int gx, unsigned char* __restrict__ inst_mask) {
+  tile_sort_warp<false, true>(tiles, ranges, hdr, keys, point_list, rec, gx, inst_mask);
 }
 
 // ---- longer lists: one CTA of 256 threads per tile, a small persistent grid strides over the tiles ----------------------
@@ -437,11 +472,11 @@ tile_sort_warp_kernel(int tiles, const uint2* __restrict__ ranges, const uint32_
 // are sorted with 4 keys per thread, 1025..4096 with 16, longer ones by the global radix fallback.
 constexpr int CS_THREADS = 256;
 constexpr int CS_WINDOW = 4096;
-template <bool PACK>
-__global__ void __launch_bounds__(CS_THREADS, 3)
-tile_sort_kernel(int tiles, const uint2* __restrict__ ranges, const uint32_t* __restrict__ hdr, uint64_t* __restrict__ keys,
-                 uint64_t* __restrict__ keys_tmp, uint32_t* __restrict__ point_list,
-                 const float* __restrict__ rec, int gx, unsigned char* __restrict__ inst_mask) {
+template <bool PACK, bool DILATE>
+__device__ __forceinline__ void tile_sort_cta(int tiles, const uint2* __restrict__ ranges, const uint32_t* __restrict__ hdr,
+                                              uint64_t* __restrict__ keys, uint64_t* __restrict__ keys_tmp,
+                                              uint32_t* __restrict__ point_list, const float* __restrict__ rec, int gx,
+                                              unsigned char* __restrict__ inst_mask) {
   if (hdr[HDR_OVERFLOW] || hdr[HDR_MAXTILE] <= (uint32_t)WS_MAX) return;   // every list is in the warp class
   extern __shared__ __align__(16) unsigned char sort_smem[];
   // [PADIDX(CS_WINDOW)] keys + [CS_THREADS + 1] splits; the oversized-tile radix path reuses the space as 2560 scratch words
@@ -455,13 +490,28 @@ tile_sort_kernel(int tiles, const uint2* __restrict__ ranges, const uint32_t* __
     if (n <= CS_WINDOW) {
       if (n <= CS_THREADS * 4) merge_sort_smem<CS_THREADS, 4>(s, s_lo, bucket, n);
       else merge_sort_smem<CS_THREADS, 16>(s, s_lo, bucket, n);
-      emit_sorted<PACK, CS_THREADS, true>(s, bucket, n, threadIdx.x, rg.x, point_list, inst_mask, rec, tile, gx);
+      emit_sorted<PACK, CS_THREADS, true, DILATE>(s, bucket, n, threadIdx.x, rg.x, point_list, inst_mask, rec, tile, gx, hdr);
     } else {
       radix_global(bucket, keys_tmp + rg.x, n, reinterpret_cast<uint32_t*>(s));
-      emit_sorted<PACK, CS_THREADS, false>(bucket, bucket, n, threadIdx.x, rg.x, point_list, inst_mask, rec, tile, gx);
+      emit_sorted<PACK, CS_THREADS, false, DILATE>(bucket, bucket, n, threadIdx.x, rg.x, point_list, inst_mask, rec, tile,
+                                                   gx, hdr);
     }
     __syncthreads();     // the shared buffer is reused by the next tile
   }
+}
+template <bool PACK>
+__global__ void __launch_bounds__(CS_THREADS, 3)
+tile_sort_kernel(int tiles, const uint2* __restrict__ ranges, const uint32_t* __restrict__ hdr, uint64_t* __restrict__ keys,
+                 uint64_t* __restrict__ keys_tmp, uint32_t* __restrict__ point_list,
+                 const float* __restrict__ rec, int gx, unsigned char* __restrict__ inst_mask) {
+  tile_sort_cta<PACK, false>(tiles, ranges, hdr, keys, keys_tmp, point_list, rec, gx, inst_mask);
+}
+// two resident CTAs per SM, not three: the dilated masks need more than the 80 registers of three
+__global__ void __launch_bounds__(CS_THREADS, 2)
+tile_sort_dilated_kernel(int tiles, const uint2* __restrict__ ranges, const uint32_t* __restrict__ hdr,
+                         uint64_t* __restrict__ keys, uint64_t* __restrict__ keys_tmp, uint32_t* __restrict__ point_list,
+                         const float* __restrict__ rec, int gx, unsigned char* __restrict__ inst_mask) {
+  tile_sort_cta<false, true>(tiles, ranges, hdr, keys, keys_tmp, point_list, rec, gx, inst_mask);
 }
 
 }  // namespace
@@ -479,23 +529,28 @@ static inline bool sfgs_keys_packed(int P) {
 }
 
 void sfgs_launch_scatter(const GeomLayout& g, const ImageLayout& im, const BinningLayout& b, int P,
-                         unsigned long long capacity, cudaStream_t st) {
+                         unsigned long long capacity, bool dilate, cudaStream_t st) {
   SFGS_COUNT_LAUNCH();
   if (capacity == 0) return;
   auto blocks_for = [&](int it) { return (unsigned)((capacity + 256ull * it - 1) / (256ull * it)); };
-  if (sfgs_keys_packed(P)) scatter_keys_kernel<true, 2><<<blocks_for(2), 256, 0, st>>>(b.tmp, im.ranges, im.tile_count, im.hdr, g.rec, im.tiles_x, b.keys);
+  if (sfgs_keys_packed(P) && dilate) scatter_keys_dilated_kernel<<<blocks_for(2), 256, 0, st>>>(b.tmp, im.ranges, im.tile_count, im.hdr, g.rec, im.tiles_x, b.keys);
+  else if (sfgs_keys_packed(P)) scatter_keys_kernel<true, 2><<<blocks_for(2), 256, 0, st>>>(b.tmp, im.ranges, im.tile_count, im.hdr, g.rec, im.tiles_x, b.keys);
   else scatter_keys_kernel<false, 4><<<blocks_for(4), 256, 0, st>>>(b.tmp, im.ranges, im.tile_count, im.hdr, g.rec, im.tiles_x, b.keys);
 }
 
-template <bool PACK>
+// The two sort kernels of one key layout: the packed ones, the unpacked ones, or (DILATE) the unpacked ones that form
+// the dilated masks of a forward with subpixel offsets.
+template <bool PACK, bool DILATE = false>
 static void launch_tile_sorts(const GeomLayout& g, const ImageLayout& im, const BinningLayout& b, cudaStream_t st) {
   constexpr size_t smem_cta = (CS_WINDOW + CS_WINDOW / 16) * sizeof(uint64_t) + (CS_THREADS + 1) * sizeof(int);
+  const auto warp_kernel = DILATE ? tile_sort_warp_dilated_kernel : tile_sort_warp_kernel<PACK>;
+  const auto cta_kernel = DILATE ? tile_sort_dilated_kernel : tile_sort_kernel<PACK>;
   static SfgsPerDeviceOnce attr_once;   // function attributes are per device
   if (attr_once.first_use()) {
-    cudaFuncSetAttribute(tile_sort_kernel<PACK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_cta);
+    cudaFuncSetAttribute(cta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_cta);
   }
   SFGS_COUNT_LAUNCH();
-  tile_sort_warp_kernel<PACK><<<(im.tiles + WS_WARPS - 1) / WS_WARPS, WS_WARPS * 32, 0, st>>>(
+  warp_kernel<<<(im.tiles + WS_WARPS - 1) / WS_WARPS, WS_WARPS * 32, 0, st>>>(
       im.tiles, im.ranges, im.hdr, b.keys, b.point_list, g.rec, im.tiles_x, b.inst_mask);
   // lists beyond the warp class: a persistent grid (three resident CTAs per SM) that returns at once when the frame's
   // longest list (header word written by the scan) is inside the warp class
@@ -504,11 +559,13 @@ static void launch_tile_sorts(const GeomLayout& g, const ImageLayout& im, const 
   { int v = 0; if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && v > 0) sms = v; }
   const int grid_cta = im.tiles < 3 * sms ? im.tiles : 3 * sms;
   SFGS_COUNT_LAUNCH();
-  tile_sort_kernel<PACK><<<grid_cta, CS_THREADS, smem_cta, st>>>(im.tiles, im.ranges, im.hdr, b.keys, b.keys_tmp, b.point_list,
-                                                                  g.rec, im.tiles_x, b.inst_mask);
+  cta_kernel<<<grid_cta, CS_THREADS, smem_cta, st>>>(im.tiles, im.ranges, im.hdr, b.keys, b.keys_tmp, b.point_list, g.rec,
+                                                     im.tiles_x, b.inst_mask);
 }
 
-void sfgs_launch_tile_sort(const GeomLayout& g, const ImageLayout& im, const BinningLayout& b, int P, cudaStream_t st) {
-  if (sfgs_keys_packed(P)) launch_tile_sorts<true>(g, im, b, st);
+void sfgs_launch_tile_sort(const GeomLayout& g, const ImageLayout& im, const BinningLayout& b, int P, bool dilate,
+                           cudaStream_t st) {
+  if (sfgs_keys_packed(P)) launch_tile_sorts<true>(g, im, b, st);   // with offsets, the key scatter dilated the masks
+  else if (dilate) launch_tile_sorts<false, true>(g, im, b, st);
   else launch_tile_sorts<false>(g, im, b, st);
 }

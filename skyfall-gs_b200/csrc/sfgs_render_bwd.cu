@@ -39,6 +39,7 @@
 // the float64-adjudicated conic gradients (cov3D, scales, rotations) exceeded the reference build's error.  Centred
 // offsets (+-3.5 .. +-0.5, rows +-0.5) bring it back within the reference's error.)
 #include "sfgs_blend_walk.cuh"
+#include <type_traits>
 
 namespace {
 
@@ -68,6 +69,9 @@ struct WarpSmem {
   float2 wh[32][BLEND_CH + 1];  // 4.25 KB phase-1 -> phase-2 hand-over, [pixel][slot], padded
   float pix[32][PIXF];          // 1 KB    per-pixel cotangents
 };
+struct WarpSmemJitter : WarpSmem {
+  float2 pos[32];               // 256 B   per-pixel sample positions (JITTER)
+};
 
 // HAS_EXTRA: also the adjoint of the ED channels of `extras` [P,ED] (extra_attrs; Skyfall-GS never passes them):
 // phase 1 keeps the reference's per-pixel recursion of the extras and adds one global atomicAdd per (pixel, Gaussian,
@@ -75,21 +79,25 @@ struct WarpSmem {
 // ORDERED: no reduction at all.  The 16 words of a (block, record) pair go to row (range.x + list position) * 8 + wid
 // of `part` [R*8,16] and written[row] is set; exactly one warp owns each row.  `acc` is not touched.  The slot's gid
 // word carries the sorted instance range.x + list position instead of the Gaussian id (nothing else reads it here).
-template <bool PEER, bool HAS_EXTRA, bool ORDERED = false>
-__global__ void __launch_bounds__(BLEND_THREADS, 3)
-render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict__ binning_base,
-                       const uint32_t* __restrict__ hdr, int W, int H, int band0,
-                       const float* __restrict__ bg_color, const float* __restrict__ rec,
-                       const float* __restrict__ accum_alphas, const uint32_t* __restrict__ n_contrib,
-                       const float* __restrict__ dL_dpixels, const float* __restrict__ dL_dpixel_depths,
-                       const float* __restrict__ dL_dpixel_norms, const float* __restrict__ dL_dpixel_alphas,
-                       const float* __restrict__ norm_raw, float* __restrict__ acc /* [P,16] zero-initialised */,
-                       const PeerTable peers, const float* __restrict__ extras,
-                       const float* __restrict__ dL_dpixel_extras, float* __restrict__ dL_dextras, int ED,
-                       float* __restrict__ part, unsigned char* __restrict__ written) {
+// JITTER: subpixel offsets — pixel (x, y) samples the splats at (x, y) + off[W y + x] ([H,W,2] floats, the buffer the
+// forward used).  Phase 1 only moves the pixel; phase 2 sums h against each pixel's sample position about the half's
+// centre (read from the warp's table `pos`), with the same centred origin.
+template <bool PEER, bool HAS_EXTRA, bool ORDERED, bool JITTER>
+__device__ __forceinline__ void
+render_bwd_warp(const uint2* __restrict__ ranges, const char* __restrict__ binning_base,
+                const uint32_t* __restrict__ hdr, int W, int H, int band0,
+                const float* __restrict__ bg_color, const float* __restrict__ rec,
+                const float* __restrict__ accum_alphas, const uint32_t* __restrict__ n_contrib,
+                const float* __restrict__ dL_dpixels, const float* __restrict__ dL_dpixel_depths,
+                const float* __restrict__ dL_dpixel_norms, const float* __restrict__ dL_dpixel_alphas,
+                const float* __restrict__ norm_raw, float* __restrict__ acc /* [P,16] zero-initialised */,
+                const PeerTable peers, const float* __restrict__ extras,
+                const float* __restrict__ dL_dpixel_extras, float* __restrict__ dL_dextras, int ED,
+                float* __restrict__ part, unsigned char* __restrict__ written, const float2* __restrict__ off) {
+  using Smem = std::conditional_t<JITTER, WarpSmemJitter, WarpSmem>;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  WarpSmem& S = reinterpret_cast<WarpSmem*>(smem_raw)[wid];
+  Smem& S = reinterpret_cast<Smem*>(smem_raw)[wid];
 
   // the binning buffer layout depends on the capacity the forward used; it is recorded in the image header
   const unsigned long long cap = ((unsigned long long)hdr[HDR_CAP_HI] << 32) | hdr[HDR_CAP_LO];
@@ -100,7 +108,7 @@ render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict_
   const BlendPixel px(band0, W, H, wid, lane);
   const bool inside = px.inside;
   const uint32_t pix_id = px.id;
-  const float pixfx = px.x, pixfy = px.y;
+  float pixfx = px.x, pixfy = px.y;          // the sample position (the pixel centre without offsets)
   const size_t HW = (size_t)H * W;
 
   const uint2 range = ranges[px.tile];
@@ -148,6 +156,12 @@ render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict_
     pt[1] = make_float4(dLn0, dLn1, dLn2, (lane & 1) ? pixfy - (float)((lane >> 3) & 1) + 0.5f
                                                      : pixfx - (float)(lane & 7) + 3.5f);
   }
+  if constexpr (JITTER) {
+    // the sample position goes to the warp's table: phase 2 reads every pixel's, phase 1 its own at each chunk (so it
+    // is not held in registers across phase 2)
+    const float2 o = inside ? off[pix_id] : make_float2(0.f, 0.f);
+    S.pos[lane] = make_float2(px.x + o.x, px.y + o.y);
+  }
   __syncwarp();
 
   // extras: the pixel's cotangents and the reference's recursion state (accum_ree = the extras' A, last_extra = g_last)
@@ -192,31 +206,61 @@ render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict_
     const float u0 = fmaf(au, DX, bu * DY), v0 = fmaf(av, DX, bv * DY);
     const float urow[2] = {fmaf(bu, 0.5f, u0), fmaf(bu, -0.5f, u0)}, vrow[2] = {fmaf(bv, 0.5f, v0), fmaf(bv, -0.5f, v0)};
     float s0 = 0, s1 = 0, s2 = 0, s3 = 0, s4 = 0, s5 = 0, s6 = 0;      // sum w * dL/dpix_c
-    float h1[2] = {0, 0}, hx[2] = {0, 0}, sxx = 0;                    // per row: sum h * {1, x}; sum h x^2
     float sab = 0;
+    float sh, shx, shy, shxx, shxy, shyy;     // sums of h * {1, dx, dy, dx^2, dx dy, dy^2} over the half
+    if constexpr (JITTER) {
+      // pixel i samples at (x, y) = its sample position - the half's centre (exact: the two are close), i.e. its
+      // compile-time offset plus its own subpixel offset: the sums of h * {1, x, y, x^2, x y, y^2} run over those, the
+      // moments about the record's centre follow by the same expansion, and |u| + |v| is evaluated per pixel
+      const float2* posp = &S.pos[chalf * 16];
+      const float hcx = pix[1].w, hcy = pix[3].w;
+      float sx = 0, sy = 0, sxx = 0, sxy = 0, syy = 0;
+      sh = 0;
+#pragma unroll 4                            // fully unrolled, the ORDERED instantiation spills
+      for (int i = 0; i < 16; i++) {
+        const float2 q = posp[i];
+        const float x = q.x - hcx, y = q.y - hcy;
+        const float2 wh = whp[i * (BLEND_CH + 1)];
+        const float4 p0 = pix[2 * i], p1 = pix[2 * i + 1];
+        s0 = fmaf(wh.x, p0.x, s0); s1 = fmaf(wh.x, p0.y, s1); s2 = fmaf(wh.x, p0.z, s2); s3 = fmaf(wh.x, p0.w, s3);
+        s4 = fmaf(wh.x, p1.x, s4); s5 = fmaf(wh.x, p1.y, s5); s6 = fmaf(wh.x, p1.z, s6);
+        const float hx = wh.y * x, hy = wh.y * y;
+        sh += wh.y;
+        sx += hx; sy += hy;
+        sxx = fmaf(hx, x, sxx); sxy = fmaf(hx, y, sxy); syy = fmaf(hy, y, syy);
+        const float u = fmaf(-au, x, fmaf(-bu, y, u0)), v = fmaf(-av, x, fmaf(-bv, y, v0));
+        sab = fmaf(fabsf(wh.y), fabsf(u) + fabsf(v), sab);
+      }
+      shx = fmaf(DX, sh, -sx); shy = fmaf(DY, sh, -sy);
+      shxx = fmaf(DX, shx, -fmaf(DX, sx, -sxx));
+      shxy = fmaf(DX, shy, -fmaf(DY, sx, -sxy));
+      shyy = fmaf(DY, shy, -fmaf(DY, sy, -syy));
+    } else {
+      float h1[2] = {0, 0}, hx[2] = {0, 0}, sxx = 0;                  // per row: sum h * {1, x}; sum h x^2
 #pragma unroll
-    for (int i = 0; i < 16; i++) {
-      const float x = (float)(i & 7) - 3.5f;
-      const int r = i >> 3;
-      const float2 wh = whp[i * (BLEND_CH + 1)];
-      const float4 p0 = pix[2 * i], p1 = pix[2 * i + 1];
-      s0 = fmaf(wh.x, p0.x, s0); s1 = fmaf(wh.x, p0.y, s1); s2 = fmaf(wh.x, p0.z, s2); s3 = fmaf(wh.x, p0.w, s3);
-      s4 = fmaf(wh.x, p1.x, s4); s5 = fmaf(wh.x, p1.y, s5); s6 = fmaf(wh.x, p1.z, s6);
-      h1[r] += wh.y;
-      hx[r] = fmaf(wh.y, x, hx[r]);
-      sxx = fmaf(wh.y, x * x, sxx);
-      const float u = fmaf(-au, x, urow[r]), v = fmaf(-av, x, vrow[r]);
-      sab = fmaf(fabsf(wh.y), fabsf(u) + fabsf(v), sab);
+      for (int i = 0; i < 16; i++) {
+        const float x = (float)(i & 7) - 3.5f;
+        const int r = i >> 3;
+        const float2 wh = whp[i * (BLEND_CH + 1)];
+        const float4 p0 = pix[2 * i], p1 = pix[2 * i + 1];
+        s0 = fmaf(wh.x, p0.x, s0); s1 = fmaf(wh.x, p0.y, s1); s2 = fmaf(wh.x, p0.z, s2); s3 = fmaf(wh.x, p0.w, s3);
+        s4 = fmaf(wh.x, p1.x, s4); s5 = fmaf(wh.x, p1.y, s5); s6 = fmaf(wh.x, p1.z, s6);
+        h1[r] += wh.y;
+        hx[r] = fmaf(wh.y, x, hx[r]);
+        sxx = fmaf(wh.y, x * x, sxx);
+        const float u = fmaf(-au, x, urow[r]), v = fmaf(-av, x, vrow[r]);
+        sab = fmaf(fabsf(wh.y), fabsf(u) + fabsf(v), sab);
+      }
+      // sums of h * {1, x, y, x^2, x y, y^2} over the half (y = -0.5 in row 0, +0.5 in row 1) ...
+      sh = h1[0] + h1[1];
+      const float sx = hx[0] + hx[1], sy = 0.5f * (h1[1] - h1[0]);
+      const float sxy = 0.5f * (hx[1] - hx[0]), syy = 0.25f * sh;
+      // ... and about the centre: sum h dx = DX sum h - sum h x, sum h dx^2 = DX sum h dx - (DX sum h x - sum h x^2), ...
+      shx = fmaf(DX, sh, -sx); shy = fmaf(DY, sh, -sy);
+      shxx = fmaf(DX, shx, -fmaf(DX, sx, -sxx));
+      shxy = fmaf(DX, shy, -fmaf(DY, sx, -sxy));
+      shyy = fmaf(DY, shy, -fmaf(DY, sy, -syy));
     }
-    // sums of h * {1, x, y, x^2, x y, y^2} over the half (y = -0.5 in row 0, +0.5 in row 1) ...
-    float sh = h1[0] + h1[1];
-    const float sx = hx[0] + hx[1], sy = 0.5f * (h1[1] - h1[0]);
-    const float sxy = 0.5f * (hx[1] - hx[0]), syy = 0.25f * sh;
-    // ... and about the centre: sum h dx = DX sum h - sum h x, sum h dx^2 = DX sum h dx - (DX sum h x - sum h x^2), ...
-    float shx = fmaf(DX, sh, -sx), shy = fmaf(DY, sh, -sy);
-    float shxx = fmaf(DX, shx, -fmaf(DX, sx, -sxx));
-    float shxy = fmaf(DX, shy, -fmaf(DY, sx, -sxy));
-    float shyy = fmaf(DY, shy, -fmaf(DY, sy, -syy));
 #define XH(v) v += __shfl_xor_sync(0xffffffffu, v, 16)
     XH(s0); XH(s1); XH(s2); XH(s3); XH(s4); XH(s5); XH(s6);
     XH(sh); XH(shx); XH(shy); XH(shxx); XH(shxy); XH(shyy); XH(sab);
@@ -301,6 +345,11 @@ render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict_
     S.wh[lane][k] = make_float2(w_out, h_out);
   };
   blend_chunks<ORDERED>(walk, [] { return false; }, [&](const int buf, const int n) {
+    if constexpr (JITTER) {
+      const float2 q = S.pos[lane];
+      pixfx = q.x;
+      pixfy = q.y;
+    }
     if (n == BLEND_CH) {                            // every chunk of a warp but its last: no per-slot bound test
       // slot k+1's parameters are read before slot k's hand-over store (the compiler cannot move a shared-memory
       // load above that store on its own), so their latency overlaps slot k's arithmetic
@@ -319,13 +368,65 @@ render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict_
   });
 }
 
+template <bool PEER, bool HAS_EXTRA, bool ORDERED = false>
+__global__ void __launch_bounds__(BLEND_THREADS, 3)
+render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict__ binning_base,
+                       const uint32_t* __restrict__ hdr, int W, int H, int band0,
+                       const float* __restrict__ bg_color, const float* __restrict__ rec,
+                       const float* __restrict__ accum_alphas, const uint32_t* __restrict__ n_contrib,
+                       const float* __restrict__ dL_dpixels, const float* __restrict__ dL_dpixel_depths,
+                       const float* __restrict__ dL_dpixel_norms, const float* __restrict__ dL_dpixel_alphas,
+                       const float* __restrict__ norm_raw, float* __restrict__ acc /* [P,16] zero-initialised */,
+                       const PeerTable peers, const float* __restrict__ extras,
+                       const float* __restrict__ dL_dpixel_extras, float* __restrict__ dL_dextras, int ED,
+                       float* __restrict__ part, unsigned char* __restrict__ written) {
+  render_bwd_warp<PEER, HAS_EXTRA, ORDERED, false>(ranges, binning_base, hdr, W, H, band0, bg_color, rec, accum_alphas,
+                                                   n_contrib, dL_dpixels, dL_dpixel_depths, dL_dpixel_norms,
+                                                   dL_dpixel_alphas, norm_raw, acc, peers, extras, dL_dpixel_extras,
+                                                   dL_dextras, ED, part, written, nullptr);
+}
+
+// subpixel offsets: device-scope reductions (ORDERED = false) or the deterministic partial rows; no extra_attrs, no
+// peers (the _subpixel entry points reject both)
+template <bool ORDERED>
+__global__ void __launch_bounds__(BLEND_THREADS, 3)
+render_bwd_jitter_kernel(const uint2* __restrict__ ranges, const char* __restrict__ binning_base,
+                         const uint32_t* __restrict__ hdr, int W, int H, int band0,
+                         const float* __restrict__ bg_color, const float* __restrict__ rec,
+                         const float* __restrict__ accum_alphas, const uint32_t* __restrict__ n_contrib,
+                         const float* __restrict__ dL_dpixels, const float* __restrict__ dL_dpixel_depths,
+                         const float* __restrict__ dL_dpixel_norms, const float* __restrict__ dL_dpixel_alphas,
+                         const float* __restrict__ norm_raw, float* __restrict__ acc, float* __restrict__ part,
+                         unsigned char* __restrict__ written, const float2* __restrict__ off) {
+  render_bwd_warp<false, false, ORDERED, true>(ranges, binning_base, hdr, W, H, band0, bg_color, rec, accum_alphas,
+                                               n_contrib, dL_dpixels, dL_dpixel_depths, dL_dpixel_norms,
+                                               dL_dpixel_alphas, norm_raw, acc, PeerTable{}, nullptr, nullptr, nullptr,
+                                               0, part, written, off);
+}
+
 }  // namespace
 
 void sfgs_launch_render_bwd(const sfgs_backward_args* a, const GeomLayout& g, const ImageLayout& im,
-                            const BinningLayout& b, float* acc, float* part, unsigned char* written, cudaStream_t st) {
+                            const BinningLayout& b, float* acc, float* part, unsigned char* written, const float* off,
+                            cudaStream_t st) {
   dim3 grid;
   int band0;
   if (!blend_grid(a->tile_row_begin, a->tile_row_end, im, grid, band0)) return;
+  if (off != nullptr) {
+    const size_t smem_j = sizeof(WarpSmemJitter) * BLEND_WARPS;
+    static SfgsPerDeviceOnce attr_once_j;
+    if (attr_once_j.first_use()) {
+      cudaFuncSetAttribute(render_bwd_jitter_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_j);
+      cudaFuncSetAttribute(render_bwd_jitter_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_j);
+    }
+    const auto kernel = part != nullptr ? render_bwd_jitter_kernel<true> : render_bwd_jitter_kernel<false>;
+    SFGS_COUNT_LAUNCH();
+    kernel<<<grid, BLEND_THREADS, smem_j, st>>>(im.ranges, (const char*)b.point_list, im.hdr, a->width, a->height, band0,
+                                                a->background, g.rec, a->accum_alphas, im.n_contrib, a->dL_dpix,
+                                                a->dL_dpix_depth, a->dL_dpix_norm, a->dL_dpix_alpha, a->norm_raw, acc,
+                                                part, written, reinterpret_cast<const float2*>(off));
+    return;
+  }
   const size_t smem = sizeof(WarpSmem) * BLEND_WARPS;
   static SfgsPerDeviceOnce attr_once;   // function attributes are per device
   if (attr_once.first_use()) {

@@ -12,6 +12,8 @@
 // (the reference gathers colour/depth/normal from global memory per pixel), and a warp whose 32 pixels are saturated
 // stops on its own.
 #include "sfgs_blend_walk.cuh"
+#include <algorithm>
+#include <type_traits>
 
 namespace {
 
@@ -23,14 +25,22 @@ struct OutPeers {
 
 // HAS_EXTRA: also blend the ED channels of `extras` [P,ED] into out_extra [ED,H,W] (extra_attrs; Skyfall-GS never
 // passes them).  The channels are read from global memory per applied pair, so this instantiation is a slow path.
+// How the body takes the peer table: the form that leaves the code generated for the two default kernels what it was
+// before the body moved out of them (by value with extra_attrs, by reference otherwise; the semantics are the same).
 template <bool HAS_EXTRA>
-__global__ void __launch_bounds__(BLEND_THREADS)
-render_fwd_warp_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list,
-                       const unsigned char* __restrict__ inst_mask, const uint32_t* __restrict__ hdr, int W, int H,
-                       int band0, const float* __restrict__ rec, const float* __restrict__ bg_color,
-                       float* __restrict__ out_color, float* __restrict__ out_depth, float* __restrict__ out_norm,
-                       float* __restrict__ out_norm_raw, float* __restrict__ out_alpha, uint32_t* __restrict__ n_contrib,
-                       const OutPeers peers, const float* __restrict__ extras, int ED, float* __restrict__ out_extra) {
+using PeersArg = std::conditional_t<HAS_EXTRA, const OutPeers, const OutPeers&>;
+
+// JITTER: subpixel offsets — pixel (x, y) samples the splats at (x, y) + off[W y + x] ([H,W,2] floats); the tile's
+// list, the walk and the slot body are unchanged (the reach masks were dilated by the offsets' bound).
+template <bool HAS_EXTRA, bool JITTER>
+__device__ __forceinline__ void
+render_fwd_warp(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list,
+                const unsigned char* __restrict__ inst_mask, const uint32_t* __restrict__ hdr, int W, int H,
+                int band0, const float* __restrict__ rec, const float* __restrict__ bg_color,
+                float* __restrict__ out_color, float* __restrict__ out_depth, float* __restrict__ out_norm,
+                float* __restrict__ out_norm_raw, float* __restrict__ out_alpha, uint32_t* __restrict__ n_contrib,
+                PeersArg<HAS_EXTRA> peers, const float* __restrict__ extras, int ED, float* __restrict__ out_extra,
+                const float2* __restrict__ off) {
   if (hdr[HDR_OVERFLOW]) return;
   __shared__ BlendStage<HAS_EXTRA> s_warp[BLEND_WARPS];   // extra_attrs: the slot's gid word is the Gaussian id
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
@@ -38,7 +48,8 @@ render_fwd_warp_kernel(const uint2* __restrict__ ranges, const uint32_t* __restr
   const BlendPixel pix(band0, W, H, wid, lane);
   const bool inside = pix.inside;
   const uint32_t pix_id = pix.id;
-  const float pixfx = pix.x, pixfy = pix.y;
+  const float2 o = JITTER && inside ? off[pix_id] : make_float2(0.f, 0.f);
+  const float pixfx = JITTER ? pix.x + o.x : pix.x, pixfy = JITTER ? pix.y + o.y : pix.y;
 
   const uint2 range = ranges[pix.tile];
   const int total = (int)(range.y - range.x);
@@ -135,13 +146,78 @@ render_fwd_warp_kernel(const uint2* __restrict__ ranges, const uint32_t* __restr
   }
 }
 
+template <bool HAS_EXTRA>
+__global__ void __launch_bounds__(BLEND_THREADS)
+render_fwd_warp_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list,
+                       const unsigned char* __restrict__ inst_mask, const uint32_t* __restrict__ hdr, int W, int H,
+                       int band0, const float* __restrict__ rec, const float* __restrict__ bg_color,
+                       float* __restrict__ out_color, float* __restrict__ out_depth, float* __restrict__ out_norm,
+                       float* __restrict__ out_norm_raw, float* __restrict__ out_alpha, uint32_t* __restrict__ n_contrib,
+                       const OutPeers peers, const float* __restrict__ extras, int ED, float* __restrict__ out_extra) {
+  render_fwd_warp<HAS_EXTRA, false>(ranges, point_list, inst_mask, hdr, W, H, band0, rec, bg_color, out_color, out_depth,
+                                    out_norm, out_norm_raw, out_alpha, n_contrib, peers, extras, ED, out_extra, nullptr);
+}
+
+// subpixel offsets: local outputs only, no extra_attrs (sfgs_rasterize_forward_subpixel rejects both)
+__global__ void __launch_bounds__(BLEND_THREADS)
+render_fwd_jitter_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list,
+                         const unsigned char* __restrict__ inst_mask, const uint32_t* __restrict__ hdr, int W, int H,
+                         int band0, const float* __restrict__ rec, const float* __restrict__ bg_color,
+                         float* __restrict__ out_color, float* __restrict__ out_depth, float* __restrict__ out_norm,
+                         float* __restrict__ out_norm_raw, float* __restrict__ out_alpha,
+                         uint32_t* __restrict__ n_contrib, const float2* __restrict__ off) {
+  render_fwd_warp<false, true>(ranges, point_list, inst_mask, hdr, W, H, band0, rec, bg_color, out_color, out_depth,
+                               out_norm, out_norm_raw, out_alpha, n_contrib, OutPeers{}, nullptr, 0, nullptr, off);
+}
+
+// max |off_x|, max |off_y| over the frame into HDR_OFF_EX / HDR_OFF_EY (non-negative floats order as their bits), and
+// HDR_OFF_BAD if any offset is NaN or Inf (those are left out of the bound; the forward then fails)
+__global__ void __launch_bounds__(256)
+offset_bound_kernel(size_t n, const float2* __restrict__ off, uint32_t* __restrict__ hdr) {
+  float ex = 0.f, ey = 0.f;
+  bool bad = false;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const float2 o = off[i];
+    const bool fx = isfinite(o.x), fy = isfinite(o.y);
+    bad |= !fx || !fy;
+    ex = fmaxf(ex, fx ? fabsf(o.x) : 0.f);
+    ey = fmaxf(ey, fy ? fabsf(o.y) : 0.f);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    ex = fmaxf(ex, __shfl_xor_sync(0xffffffffu, ex, o));
+    ey = fmaxf(ey, __shfl_xor_sync(0xffffffffu, ey, o));
+  }
+  bad = __any_sync(0xffffffffu, bad);
+  if ((threadIdx.x & 31) == 0) {
+    atomicMax(&hdr[HDR_OFF_EX], __float_as_uint(ex));
+    atomicMax(&hdr[HDR_OFF_EY], __float_as_uint(ey));
+    if (bad) hdr[HDR_OFF_BAD] = 1u;
+  }
+}
+
 }  // namespace
 
+void sfgs_launch_offset_bound(const ImageLayout& im, int W, int H, const float* off, cudaStream_t st) {
+  const size_t n = (size_t)W * H;
+  const unsigned blocks = (unsigned)std::min<size_t>((n + 255) / 256, 132 * 8);
+  SFGS_COUNT_LAUNCH();
+  offset_bound_kernel<<<blocks, 256, 0, st>>>(n, reinterpret_cast<const float2*>(off), im.hdr);
+}
+
 void sfgs_launch_render_fwd(const sfgs_forward_args* a, const GeomLayout& g, const ImageLayout& im,
-                            const BinningLayout& b, cudaStream_t st) {
+                            const BinningLayout& b, const float* off, cudaStream_t st) {
   dim3 grid;
   int band0;
   if (!blend_grid(a->tile_row_begin, a->tile_row_end, im, grid, band0)) return;
+  if (off != nullptr) {
+    SFGS_COUNT_LAUNCH();
+    render_fwd_jitter_kernel<<<grid, BLEND_THREADS, 0, st>>>(im.ranges, b.point_list, b.inst_mask, im.hdr, a->width,
+                                                             a->height, band0, g.rec, a->background, a->out_color,
+                                                             a->out_depth, a->out_norm, a->out_norm_raw, a->out_alpha,
+                                                             im.n_contrib, reinterpret_cast<const float2*>(off));
+    return;
+  }
   OutPeers op = {};
   if (a->out_peers != nullptr && a->n_out_peers > 0)
     for (op.n = 0; op.n < a->n_out_peers && op.n < 8; op.n++) op.p[op.n] = a->out_peers[op.n];

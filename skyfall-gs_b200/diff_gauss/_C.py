@@ -7,14 +7,14 @@ from sfgs.rasterizer import mark_visible, rasterize_gaussians, rasterize_gaussia
 from sfgs.native import lib as _lib
 
 
-def rasterize_gaussians_fused(*args):
+def rasterize_gaussians_fused(*args, **kw):
     """`rasterize_gaussians` with the F.normalize post-op fused into the blend kernel; returns the reference's
     10-tuple (normal map already unit length) + the un-normalised blend needed by the backward."""
-    return rasterize_gaussians(*args, fuse_normalize=True)
+    return rasterize_gaussians(*args, fuse_normalize=True, **kw)
 
 
-def rasterize_gaussians_backward_fused(*args, norm_raw):
-    return rasterize_gaussians_backward(*args, norm_raw=norm_raw)
+def rasterize_gaussians_backward_fused(*args, norm_raw, **kw):
+    return rasterize_gaussians_backward(*args, norm_raw=norm_raw, **kw)
 
 
 _lib()  # fail at import time if the CUDA library has not been built

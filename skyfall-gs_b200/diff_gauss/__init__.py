@@ -35,6 +35,13 @@ MAX_EXTRA_DIMS = 34  # RAST/cuda_rasterizer/auxiliary.h:20
 # it loads each pixel's cotangent (SURVEY.md 8f rank 1).  Set SFGS_FUSE_NORMALIZE=0 to get the torch post-op back.
 FUSE_NORMALIZE = os.environ.get("SFGS_FUSE_NORMALIZE", "1") != "0"
 
+# GaussianRasterizationSettings.subpixel_offset (Mip-Splatting's ray jitter: Skyfall-GS's train.py --ray_jitter draws
+# U(-0.5, 0.5) per pixel, and --resample_gt_image resamples the target at the same positions).  The reference's
+# rasterizer drops it; with SFGS_SUBPIXEL_OFFSET=1 a [H,W,2] tensor is honoured: pixel (x, y) samples the splats at
+# (x + off[y,x,0], y + off[y,x,1]).  Placeholders with numel() <= 1 are ignored.  Off by default, so the default
+# keeps the reference's semantics exactly.
+SUBPIXEL_OFFSET = os.environ.get("SFGS_SUBPIXEL_OFFSET", "0") == "1"
+
 
 class GaussianRasterizationSettings(NamedTuple):
     image_height: int
@@ -42,7 +49,7 @@ class GaussianRasterizationSettings(NamedTuple):
     tanfovx: float
     tanfovy: float
     kernel_size: float
-    subpixel_offset: torch.Tensor  # accepted for API compatibility; the reference never forwards it either
+    subpixel_offset: torch.Tensor  # ignored (as by the reference) unless SUBPIXEL_OFFSET is on
     bg: torch.Tensor
     scale_modifier: float
     viewmatrix: torch.Tensor
@@ -71,6 +78,22 @@ def _guarded(fn, args, debug, dump_name, label):
         raise
 
 
+def _subpixel_offset(rs):
+    """The offsets to honour: None unless SUBPIXEL_OFFSET is on and the settings carry a [H,W,2] tensor."""
+    off = rs.subpixel_offset
+    if not SUBPIXEL_OFFSET or not isinstance(off, torch.Tensor) or off.numel() <= 1:
+        return None
+    if tuple(off.shape) != (int(rs.image_height), int(rs.image_width), 2):
+        raise ValueError(f"subpixel_offset must have shape ({int(rs.image_height)}, {int(rs.image_width)}, 2), "
+                         f"got {tuple(off.shape)}")
+    return off.detach()
+
+
+def _with_offset(fn):
+    """fn with the subpixel offsets taken from its last positional argument."""
+    return lambda *a, **kw: fn(*a[:-1], subpixel_offset=a[-1], **kw)
+
+
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
@@ -83,14 +106,19 @@ class _RasterizeGaussians(torch.autograd.Function):
                        rs.tanfovx, rs.tanfovy, rs.kernel_size, rs.image_height, rs.image_width, sh, rs.sh_degree,
                        rs.campos, rs.prefiltered, rs.debug)
         ctx.fused = bool(fuse_normalize)
+        off = _subpixel_offset(rs)
+        fwd = _C.rasterize_gaussians_fused if ctx.fused else _C.rasterize_gaussians
+        if off is not None:
+            # the offsets travel as the last argument, so that the debug snapshot holds them too
+            fwd, native_args = _with_offset(fwd), native_args + (off,)
         if ctx.fused:
             (num_rendered, color, depth, norm, alpha, radii, extra, geom_buf, binning_buf, img_buf,
-             norm_raw) = _guarded(_C.rasterize_gaussians_fused, native_args, rs.debug, "snapshot_fw.dump", "forward")
+             norm_raw) = _guarded(fwd, native_args, rs.debug, "snapshot_fw.dump", "forward")
         else:
             (num_rendered, color, depth, norm, alpha, radii, extra,
-             geom_buf, binning_buf, img_buf) = _guarded(_C.rasterize_gaussians, native_args, rs.debug,
-                                                        "snapshot_fw.dump", "forward")
+             geom_buf, binning_buf, img_buf) = _guarded(fwd, native_args, rs.debug, "snapshot_fw.dump", "forward")
             norm_raw = torch.empty(0, device=means3D.device)
+        ctx.subpixel_offset = off
         ctx.raster_settings = rs
         ctx.num_rendered = num_rendered
         ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, norm3Ds_precomp, radii,
@@ -109,7 +137,9 @@ class _RasterizeGaussians(torch.autograd.Function):
                        geom_buf, ctx.num_rendered, binning_buf, img_buf, alpha, rs.debug)
         bwd = _C.rasterize_gaussians_backward
         if ctx.fused:
-            bwd = lambda *a: _C.rasterize_gaussians_backward_fused(*a, norm_raw=norm_raw)  # noqa: E731
+            bwd = lambda *a, **kw: _C.rasterize_gaussians_backward_fused(*a, norm_raw=norm_raw, **kw)  # noqa: E731
+        if ctx.subpixel_offset is not None:
+            bwd, native_args = _with_offset(bwd), native_args + (ctx.subpixel_offset,)
         (g_means2D, g_colors, g_opac, g_means3D, g_cov3D, g_norm3D, g_sh, g_scales, g_rot,
          g_extra_attrs) = _guarded(bwd, native_args, rs.debug, "snapshot_bw.dump", "backward")
         # order of forward's inputs; the settings tuple and the fusion flag get no gradient

@@ -64,19 +64,33 @@ class _Arena:
             return None
 
 
+def check_subpixel_offset(subpixel_offset, H, W):
+    """Validate a per-pixel offset tensor: CUDA float32 of shape (H, W, 2).  Raises ValueError otherwise."""
+    t = subpixel_offset
+    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float32 or tuple(t.shape) != (H, W, 2):
+        what = (f"{t.dtype} {tuple(t.shape)} on {t.device}" if isinstance(t, torch.Tensor) else type(t).__name__)
+        raise ValueError(f"subpixel_offset must be a CUDA float32 tensor of shape ({H}, {W}, 2), got {what}")
+
+
 def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations, scale_modifier,
                         cov3Ds_precomp, norm3Ds_precomp, extra_attrs, attr_degree, viewmatrix, projmatrix,
                         tan_fovx, tan_fovy, kernel_size, image_height, image_width, sh, degree, campos,
                         prefiltered, debug, capacity_hint=0, tile_rows=None, fuse_normalize=False, out_planes=None,
-                        out_peers=None):
+                        out_peers=None, subpixel_offset=None):
     """Same positional signature and return tuple as the reference's `_C.rasterize_gaussians`.  With
     `fuse_normalize=True` the returned normal map is already F.normalize(., dim=0) (the reference's torch post-op,
-    diff_gauss/__init__.py:48) and the un-normalised blend is appended to the tuple for the backward."""
+    diff_gauss/__init__.py:48) and the un-normalised blend is appended to the tuple for the backward.
+
+    `subpixel_offset` ([H,W,2] CUDA float32, or None): pixel (x, y) samples the splats at (x + off[y,x,0],
+    y + off[y,x,1]) (sfgs_rasterize_forward_subpixel); the backward must be given the same tensor.  Offsets must be
+    finite; a NaN or Inf raises."""
     if means3D.ndim != 2 or means3D.shape[1] != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")
+    H, W, F = int(image_height), int(image_width), int(attr_degree)
+    if subpixel_offset is not None:
+        check_subpixel_offset(subpixel_offset, H, W)
     L = N.lib()
     P = int(means3D.shape[0])
-    H, W, F = int(image_height), int(image_width), int(attr_degree)
     dev = means3D.device
     fopt = dict(dtype=torch.float32, device=dev)
 
@@ -141,7 +155,11 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
         a.capacity_hint = int(capacity_hint)
         if tile_rows is not None:
             a.tile_row_begin, a.tile_row_end = _band(tile_rows)
-        rendered = N.check(L.sfgs_rasterize_forward(C.byref(a)), "sfgs_rasterize_forward")
+        if subpixel_offset is not None:
+            rendered = N.check(L.sfgs_rasterize_forward_subpixel(C.byref(a), _ptr(subpixel_offset, keep)),
+                               "sfgs_rasterize_forward_subpixel")
+        else:
+            rendered = N.check(L.sfgs_rasterize_forward(C.byref(a)), "sfgs_rasterize_forward")
     ret = (rendered, out_color, out_depth, out_norm, out_alpha, radii, out_extra,
            geom.tensor, binning.tensor, img.tensor)
     return ret + (norm_raw,) if fuse_normalize else ret
@@ -182,7 +200,7 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
                                  kernel_size, dL_dout_color, dL_dout_depth, dL_dout_norm, dL_dout_alpha,
                                  dL_dout_extra, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer,
                                  out_alpha, debug, tile_rows=None, norm_raw=None, phase=0, acc=None,
-                                 gauss_range=None, acc_peers=None, peer_slice=0):
+                                 gauss_range=None, acc_peers=None, peer_slice=0, subpixel_offset=None):
     """Same positional signature and return tuple as the reference's `_C.rasterize_gaussians_backward`.  With
     `norm_raw` (the extra tensor a `fuse_normalize=True` forward returned) `dL_dout_norm` is taken w.r.t. the unit
     normal map and the adjoint of F.normalize is applied inside the blend-adjoint kernel.
@@ -195,7 +213,12 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     Under `torch.use_deterministic_algorithms(True)` the call runs the deterministic backward
     (sfgs_rasterize_backward_deterministic): the same outputs up to the order of the sums, bit-identical from run to
     run.  `extra_attrs` and `acc_peers` have no deterministic implementation: they raise, or with `warn_only=True`
-    warn and run the default backward."""
+    warn and run the default backward.
+
+    `subpixel_offset`: the tensor the forward was given (sfgs_rasterize_backward_subpixel and its deterministic form);
+    no gradient is formed with respect to it."""
+    if subpixel_offset is not None:
+        check_subpixel_offset(subpixel_offset, int(dL_dout_color.shape[1]), int(dL_dout_color.shape[2]))
     F = int(extra_attrs.shape[1]) if (extra_attrs is not None and extra_attrs.numel() != 0) else 0
     deterministic = _use_deterministic(F > 0, acc_peers is not None)
     L = N.lib()
@@ -283,7 +306,14 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
         a.stream = torch.cuda.current_stream(dev).cuda_stream
         if tile_rows is not None:
             a.tile_row_begin, a.tile_row_end = _band(tile_rows)
-        if deterministic:
+        if subpixel_offset is not None:
+            off = _ptr(subpixel_offset, keep)
+            if deterministic:
+                N.check(L.sfgs_rasterize_backward_deterministic_subpixel(C.byref(a), off),
+                        "sfgs_rasterize_backward_deterministic_subpixel")
+            else:
+                N.check(L.sfgs_rasterize_backward_subpixel(C.byref(a), off), "sfgs_rasterize_backward_subpixel")
+        elif deterministic:
             N.check(L.sfgs_rasterize_backward_deterministic(C.byref(a)), "sfgs_rasterize_backward_deterministic")
         else:
             N.check(L.sfgs_rasterize_backward(C.byref(a)), "sfgs_rasterize_backward")
