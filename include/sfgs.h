@@ -197,6 +197,7 @@ int sfgs_rasterize_backward(const sfgs_backward_args* a);
  *   phase 0 and phase 1 (the blend adjoint) need `radii` and `scratch_alloc`: the extra scratch is
  *     4 P + 524 R bytes (+ alignment; R = instances of the forward), on top of the P*16 floats of `acc` when that is
  *     not given;
+ *   (sfgs_rasterize_backward_camera adds 35 * 8 * ceil(P / 96) bytes for the camera partials);
  *   phase 2 runs the per-Gaussian adjoint, which has no reduction, exactly as sfgs_rasterize_backward does;
  *   acc_peers (system-scope reductions) and ED > 0 (extra_attrs) return SFGS_E_UNSUPPORTED before any CUDA work.
  * The outputs equal sfgs_rasterize_backward's up to the rounding of the sums' order. */
@@ -216,6 +217,28 @@ int sfgs_rasterize_backward_deterministic(const sfgs_backward_args* a);
 int sfgs_rasterize_forward_subpixel(const sfgs_forward_args* a, const float* subpixel_offset);
 int sfgs_rasterize_backward_subpixel(const sfgs_backward_args* a, const float* subpixel_offset);
 int sfgs_rasterize_backward_deterministic_subpixel(const sfgs_backward_args* a, const float* subpixel_offset);
+
+/* ---- camera gradients (pose refinement: Camera(..., optimizing=True) of scene/cameras.py) -------------------------
+ * The backward above that also writes dL_dcamera, a DEVICE [35] float array: dL/dviewmatrix[16], dL/dprojmatrix[16],
+ * dL/dcampos[3], each in its input's element order [4*c + r].  subpixel_offset == NULL and deterministic == 0 give the
+ * default backward; a non-NULL offset follows sfgs_rasterize_backward_subpixel and deterministic != 0
+ * sfgs_rasterize_backward_deterministic, with their validation (e.g. ED > 0 with either returns SFGS_E_UNSUPPORTED).
+ *   - The gradients are the adjoint of the chain dL_dmean3D differentiates: the projected centre through projmatrix
+ *     (with its 1/(w + 1e-7) divide), the view-space point through viewmatrix (the depth, and J(t)·W of the EWA
+ *     covariance with the Mip coefficient, the same limx/limy clamps), and the SH view direction
+ *     normalize(mean - campos).  Discrete decisions (culling, tile lists, clamp sets, alpha and T thresholds, the normal's
+ *     sign flip) and the abs-gradient channel contribute nothing; entries the forward never reads (viewmatrix[3], [7],
+ *     [11], [15], projmatrix[2], [6], [10], [14]) are exactly 0; with colors_precomp dL/dcampos is exactly 0.
+ *   - The sum over Gaussians runs in float64, in an order fixed by P alone, and is rounded to float once: the camera
+ *     gradients are bit-reproducible whenever the blend-adjoint sums are (deterministic != 0).
+ *   - Every other output is bit-identical to the same backward without camera gradients.
+ *   - scratch_alloc is required; the extra scratch is 35 * 8 * ceil(P / 96) bytes (+ alignment) on top of what the
+ *     backward it follows needs.
+ *   - Phase 0 only: phases 1 and 2 and acc_peers return SFGS_E_UNSUPPORTED, a NULL dL_dcamera SFGS_E_BADARG, before
+ *     any CUDA work.
+ * No gradient is formed for tan_fovx / tan_fovy (the intrinsics) or the subpixel offsets. */
+int sfgs_rasterize_backward_camera(const sfgs_backward_args* a, const float* subpixel_offset, int deterministic,
+                                   float* dL_dcamera);
 
 /* ---- markVisible --------------------------------------------------------- */
 int sfgs_mark_visible(int P, const float* means3D, const float* viewmatrix,

@@ -38,6 +38,9 @@ constexpr int O_MEAN2D = 0, O_CONIC = 3, O_OPAC = 7, O_COLOR = 8, O_DEPTH = 11, 
 constexpr int GB_FIXED = 31;       // fixed-width gradient floats per Gaussian
 constexpr int GB_SH_ROW = 19;      // staged dL_dsh factors per Gaussian (odd: rows start in different banks)
 constexpr int GB_NFIXED = 10;     // fixed-width output arrays
+// camera terms of one Gaussian (the camera adjoint): dL/dviewmatrix[16], dL/dprojmatrix[16], dL/dcampos[3], each in its
+// input's element order [4*c + r]
+constexpr int C_VIEW = 0, C_PROJ = 16, C_CAMPOS = 32, GB_CAM = 35;
 
 // Shared-memory image of one stage's inputs, indexed by slot (position in the stage's list of visible Gaussians).
 // Field-major, so the adjoint's threads (consecutive slots) read consecutive words.
@@ -92,13 +95,21 @@ __device__ __forceinline__ float3 dnormvdv3(float3 v, float3 dv) {
 
 // The adjoint chain of one rasterized Gaussian from its blend-adjoint sums A0..A3 and forward record rec1..rec3.
 // The expressions and their float/double promotions are the reference's; do not reassociate them.
-template <class SH>
+// CAM: also the Gaussian's camera terms (cam), the adjoint of the same chain with respect to the camera: the view-space
+// point t (dL/dt, with the depth) and W of J(t)·W (dL/dT), the projected centre (the 1/(w + 1e-7) multipliers) and the
+// SH view direction (minus the dnormvdv3 result).  Entries the forward does not read (viewmatrix[3,7,11,15],
+// projmatrix[2,6,10,14]) stay 0.
+template <bool CAM, class SH>
 __device__ __forceinline__ void gauss_adjoint(
     int D, float mx, float my, float mz, bool has_scales, float4 q_in, float scx, float scy, float scz,
     float scale_modifier, bool has_sh, unsigned cm, SH sh, const float* cov3D, bool norm_precomp, float4 A0,
     float4 A1, float4 A2, float4 A3, float4 rec1, float4 rec2, float4 rec3, const float* __restrict__ view,
     const float* __restrict__ proj, float h_x, float h_y, float tan_fovx, float tan_fovy, float kernel_size,
-    const float* __restrict__ campos, float (&out)[GB_ROW]) {
+    const float* __restrict__ campos, float (&out)[GB_ROW], float (&cam)[GB_CAM]) {
+  if constexpr (CAM) {
+#pragma unroll
+    for (int j = 0; j < GB_CAM; j++) cam[j] = 0.f;
+  }
   float o_mean2D[3] = {0, 0, 0}, o_conic[4] = {0, 0, 0, 0}, o_opac = 0, o_color[3] = {0, 0, 0}, o_depth = 0;
   float o_mean[3] = {0, 0, 0}, o_cov[6] = {0, 0, 0, 0, 0, 0}, o_norm[3] = {0, 0, 0};
   float o_scale[3] = {0, 0, 0}, o_rot[4] = {0, 0, 0, 0};
@@ -208,6 +219,25 @@ __device__ __forceinline__ void gauss_adjoint(
     o_mean[0] = view[0] * dL_dtx + view[1] * dL_dty + view[2] * dL_dtz;
     o_mean[1] = view[4] * dL_dtx + view[5] * dL_dty + view[6] * dL_dtz;
     o_mean[2] = view[8] * dL_dtx + view[9] * dL_dty + view[10] * dL_dtz;
+    if constexpr (CAM) {
+      // t = [m, 1]·view (columns 0..2): dL/dview[4k + r] = m_k dL/dt_r, dL/dview[12 + r] = dL/dt_r.  T = J·W with
+      // W[k][r] = view[4r + k] and J = [[a0, 0, a2], [0, b1, b2]]: dL/dW[k][r] = sum_i J[i][k] dL/dT[i][r].
+      const float m3[3] = {mx, my, mz};
+      const float dt[3] = {dL_dtx, dL_dty, dL_dtz};
+      const float dT0[3] = {dL_dT00, dL_dT01, dL_dT02}, dT1[3] = {dL_dT10, dL_dT11, dL_dT12};
+#pragma unroll
+      for (int r = 0; r < 3; r++) {
+#pragma unroll
+        for (int k = 0; k < 3; k++) cam[C_VIEW + 4 * k + r] = m3[k] * dt[r];
+        cam[C_VIEW + 12 + r] = dt[r];
+      }
+#pragma unroll
+      for (int r = 0; r < 3; r++) {
+        cam[C_VIEW + 4 * r + 0] += a0 * dT0[r];
+        cam[C_VIEW + 4 * r + 1] += b1 * dT1[r];
+        cam[C_VIEW + 4 * r + 2] += a2 * dT0[r] + b2 * dT1[r];
+      }
+    }
   }
 
   // ---------------- projected centre and depth -> mean (preprocessCUDA bwd) ----------------
@@ -226,6 +256,23 @@ __device__ __forceinline__ void gauss_adjoint(
     const float e1 = (view[6] - view[7] * mul3) * o_depth;
     const float e2 = (view[10] - view[11] * mul3) * o_depth;
     o_mean[0] += e0; o_mean[1] += e1; o_mean[2] += e2;
+    if constexpr (CAM) {
+      // the homogeneous centre [m, 1]·proj and its divide: dL/dhom = (gx w, gy w, ., -(gx mul1 + gy mul2)), w = m_w;
+      // the depth is t_z: dL/dview[4k + 2] = m_k dL/ddepth, dL/dview[14] = dL/ddepth
+      const float m3[3] = {mx, my, mz};
+      const float dhx = gx * m_w, dhy = gy * m_w, dhw = -(gx * mul1 + gy * mul2);
+#pragma unroll
+      for (int k = 0; k < 3; k++) {
+        cam[C_PROJ + 4 * k + 0] = m3[k] * dhx;
+        cam[C_PROJ + 4 * k + 1] = m3[k] * dhy;
+        cam[C_PROJ + 4 * k + 3] = m3[k] * dhw;
+        cam[C_VIEW + 4 * k + 2] += m3[k] * o_depth;
+      }
+      cam[C_PROJ + 12] = dhx;
+      cam[C_PROJ + 13] = dhy;
+      cam[C_PROJ + 15] = dhw;
+      cam[C_VIEW + 14] += o_depth;
+    }
   }
 
   // ---------------- RGB -> SH and view direction -> mean ----------------
@@ -290,6 +337,15 @@ __device__ __forceinline__ void gauss_adjoint(
       dL_ddir.z = dRGBdz[0] * dL_dRGB[0] + dRGBdz[1] * dL_dRGB[1] + dRGBdz[2] * dL_dRGB[2];
       const float3 dm = dnormvdv3(make_float3(ox, oy, oz), dL_ddir);
       o_mean[0] += dm.x; o_mean[1] += dm.y; o_mean[2] += dm.z;
+      if constexpr (CAM) {
+        // -dnormvdv3(v, dL_ddir), evaluated again in double: reading dm here would give its final products a second
+        // use, and the compiler would then no longer fuse them into the o_mean sums, changing dL_dmean3D's rounding
+        const double vx = ox, vy = oy, vz = oz, gx = dL_ddir.x, gy = dL_ddir.y, gz = dL_ddir.z;
+        const double s2 = vx * vx + vy * vy + vz * vz, inv = 1.0 / (s2 * sqrt(s2));
+        cam[C_CAMPOS + 0] = (float)(-((s2 - vx * vx) * gx - vy * vx * gy - vz * vx * gz) * inv);
+        cam[C_CAMPOS + 1] = (float)(-(-vx * vy * gx + (s2 - vy * vy) * gy - vz * vy * gz) * inv);
+        cam[C_CAMPOS + 2] = (float)(-(-vx * vz * gx - vy * vz * gy + (s2 - vz * vz) * gz) * inv);
+      }
     };
     sh_adjoint(sh);
   }
@@ -421,18 +477,27 @@ __device__ __forceinline__ void copy_range(float* __restrict__ dst, const float*
   }
 }
 
-__global__ void __launch_bounds__(GB_THREADS, GB_CTAS_PER_SM)
-gauss_bwd_kernel(int g_begin, int g_end, int spans_per_cta, int acc_row0, int D, int M,
-                 const float* __restrict__ means3D, const int* __restrict__ radii, const float* __restrict__ shs,
-                 const unsigned char* __restrict__ clamped, const float* __restrict__ scales,
-                 const float* __restrict__ rotations, float scale_modifier, const float* __restrict__ cov3Ds,
-                 const float* __restrict__ rec, const float* __restrict__ norm3D_precomp,
-                 const float* __restrict__ view, const float* __restrict__ proj, float h_x, float h_y,
-                 float tan_fovx, float tan_fovy, float kernel_size, const float* __restrict__ campos,
-                 const float* __restrict__ acc, float* __restrict__ dL_dmean2D, float* __restrict__ dL_dconic,
-                 float* __restrict__ dL_dopacity, float* __restrict__ dL_dcolor, float* __restrict__ dL_ddepth,
-                 float* __restrict__ dL_dmean3D, float* __restrict__ dL_dcov3D, float* __restrict__ dL_dnorm3D,
-                 float* __restrict__ dL_dsh, float* __restrict__ dL_dscale, float* __restrict__ dL_drot) {
+// The camera terms of a stage's slots are staged, field-major, after the span's staged outputs in the consumed inputs.
+constexpr int GB_CAM_STAGE = (GB_SPAN * (GB_SH_ROW + GB_FIXED) + 4 * GB_NFIXED + 3) & ~3;
+static_assert(sizeof(float) * (GB_CAM_STAGE + GB_CAM * GB_SLOTS) <= sizeof(GbInputs),
+              "a stage's camera terms fit beside a span's staged outputs");
+
+// The per-Gaussian adjoint over spans [g_begin, g_end).  CAM: also the camera adjoint; span s (counted from g_begin)
+// writes cam_part[j * nspans + s], the float64 sum of its rasterized Gaussians' camera term j in index order.
+template <bool CAM>
+__device__ __forceinline__ void
+gauss_bwd_body(int g_begin, int g_end, int spans_per_cta, int acc_row0, int D, int M,
+               const float* __restrict__ means3D, const int* __restrict__ radii, const float* __restrict__ shs,
+               const unsigned char* __restrict__ clamped, const float* __restrict__ scales,
+               const float* __restrict__ rotations, float scale_modifier, const float* __restrict__ cov3Ds,
+               const float* __restrict__ rec, const float* __restrict__ norm3D_precomp,
+               const float* __restrict__ view, const float* __restrict__ proj, float h_x, float h_y,
+               float tan_fovx, float tan_fovy, float kernel_size, const float* __restrict__ campos,
+               const float* __restrict__ acc, float* __restrict__ dL_dmean2D, float* __restrict__ dL_dconic,
+               float* __restrict__ dL_dopacity, float* __restrict__ dL_dcolor, float* __restrict__ dL_ddepth,
+               float* __restrict__ dL_dmean3D, float* __restrict__ dL_dcov3D, float* __restrict__ dL_dnorm3D,
+               float* __restrict__ dL_dsh, float* __restrict__ dL_dscale, float* __restrict__ dL_drot,
+               double* __restrict__ cam_part) {
   extern __shared__ __align__(16) unsigned char gb_smem[];
   GbShared& S = *reinterpret_cast<GbShared*>(gb_smem);
   const int t = threadIdx.x, lane = t & 31, wid = t >> 5;
@@ -541,20 +606,21 @@ gauss_bwd_kernel(int g_begin, int g_end, int spans_per_cta, int acc_row0, int D,
     // ---------------- adjoint: thread k takes slot k ----------------
     GbInputs& in = S.buf[b];
     float o[GB_ROW];
+    float cam[GB_CAM];
     const bool active = t < nslots_cur;
     if (active) {
       const int k = t;
       const float* shk = reinterpret_cast<const float*>(&in.sh[0][k]);   // float j at word (j >> 2) * 4 * SLOTS + (j & 3)
       const float cov3D[6] = {in.cov[0][k], in.cov[1][k], in.cov[2][k], in.cov[3][k], in.cov[4][k], in.cov[5][k]};
       const unsigned cm = has_sh ? (in.clamped[k] >> (8 * (S.gidx[b][k] & 3))) & 0xffu : 0u;
-      gauss_adjoint(D, in.mean[0][k], in.mean[1][k], in.mean[2][k], has_scales,
+      gauss_adjoint<CAM>(D, in.mean[0][k], in.mean[1][k], in.mean[2][k], has_scales,
                     has_scales ? in.rot[k] : make_float4(0.f, 0.f, 0.f, 0.f),
                     has_scales ? in.scale[0][k] : 0.f, has_scales ? in.scale[1][k] : 0.f,
                     has_scales ? in.scale[2][k] : 0.f, scale_modifier, has_sh, cm,
                     [&](int j) { return shk[(j >> 2) * (4 * GB_SLOTS) + (j & 3)]; }, cov3D,
                     norm3D_precomp != nullptr, in.acc[0][k], in.acc[1][k], in.acc[2][k], in.acc[3][k],
                     in.rec[0][k], in.rec[1][k], in.rec[2][k], view, proj, h_x, h_y, tan_fovx, tan_fovy,
-                    kernel_size, campos, o);
+                    kernel_size, campos, o, cam);
     }
     // ---------------- epilogue, span by span: stage the span's outputs, then write each output's range once ----------
     // Staged over the consumed inputs: the dL_dsh factor rows, then one image per fixed-width array laid out as its
@@ -562,6 +628,7 @@ gauss_bwd_kernel(int g_begin, int g_end, int spans_per_cta, int acc_row0, int D,
     // The fixed-width arrays are then plain copies; dL_dsh is formed while it is written, for any M.
     float* const sh_rows = reinterpret_cast<float*>(&S.buf[b]);
     float* const images = sh_rows + GB_SPAN * GB_SH_ROW;
+    float* const cam_stage = sh_rows + GB_CAM_STAGE;
     const int rel = active ? S.gidx[b][t] - (g_begin + first_cur * GB_SPAN) : -1;   // span * GB_SPAN + position
     for (int sp = 0; sp < nsp_cur; sp++) {
       const int base = g_begin + (first_cur + sp) * GB_SPAN, n = min(GB_SPAN, g_end - base);
@@ -584,7 +651,24 @@ gauss_bwd_kernel(int g_begin, int g_end, int spans_per_cta, int acc_row0, int D,
       };
       if (active && rel / GB_SPAN == sp) stage(rel % GB_SPAN, false);
       if (t < n && S.slot[b][sp][t] < 0) stage(t, true);
+      if constexpr (CAM) {
+        if (sp == 0 && active) {
+#pragma unroll
+          for (int j = 0; j < GB_CAM; j++) cam_stage[j * GB_SLOTS + t] = cam[j];
+        }
+      }
       __syncthreads();
+      if constexpr (CAM) {
+        // thread j sums term j over the span's Gaussians in index order
+        if (t < GB_CAM) {
+          double s = 0.0;
+          for (int p = 0; p < n; p++) {
+            const int k = S.slot[b][sp][p];
+            if (k >= 0) s += (double)cam_stage[t * GB_SLOTS + k];
+          }
+          cam_part[(size_t)t * nspans + first_cur + sp] = s;
+        }
+      }
 #pragma unroll
       for (int x = 0; x < GB_NFIXED; x++)
         copy_range(fixed_out[x] + (size_t)base * kFixedW[x], images + kImageOff[x] + pre[x], n * kFixedW[x]);
@@ -603,6 +687,54 @@ gauss_bwd_kernel(int g_begin, int g_end, int spans_per_cta, int acc_row0, int D,
     nsp_cur = nsp_next;
     nslots_cur = nslots_next;
   }
+}
+
+#define GB_PARAMS                                                                                                    \
+  int g_begin, int g_end, int spans_per_cta, int acc_row0, int D, int M, const float* __restrict__ means3D,         \
+      const int* __restrict__ radii, const float* __restrict__ shs, const unsigned char* __restrict__ clamped,      \
+      const float* __restrict__ scales, const float* __restrict__ rotations, float scale_modifier,                  \
+      const float* __restrict__ cov3Ds, const float* __restrict__ rec, const float* __restrict__ norm3D_precomp,    \
+      const float* __restrict__ view, const float* __restrict__ proj, float h_x, float h_y, float tan_fovx,         \
+      float tan_fovy, float kernel_size, const float* __restrict__ campos, const float* __restrict__ acc,           \
+      float* __restrict__ dL_dmean2D, float* __restrict__ dL_dconic, float* __restrict__ dL_dopacity,               \
+      float* __restrict__ dL_dcolor, float* __restrict__ dL_ddepth, float* __restrict__ dL_dmean3D,                 \
+      float* __restrict__ dL_dcov3D, float* __restrict__ dL_dnorm3D, float* __restrict__ dL_dsh,                    \
+      float* __restrict__ dL_dscale, float* __restrict__ dL_drot
+#define GB_ARGS                                                                                                      \
+  g_begin, g_end, spans_per_cta, acc_row0, D, M, means3D, radii, shs, clamped, scales, rotations, scale_modifier,   \
+      cov3Ds, rec, norm3D_precomp, view, proj, h_x, h_y, tan_fovx, tan_fovy, kernel_size, campos, acc, dL_dmean2D,  \
+      dL_dconic, dL_dopacity, dL_dcolor, dL_ddepth, dL_dmean3D, dL_dcov3D, dL_dnorm3D, dL_dsh, dL_dscale, dL_drot
+
+__global__ void __launch_bounds__(GB_THREADS, GB_CTAS_PER_SM) gauss_bwd_kernel(GB_PARAMS) {
+  gauss_bwd_body<false>(GB_ARGS, nullptr);
+}
+
+__global__ void __launch_bounds__(GB_THREADS, GB_CTAS_PER_SM)
+gauss_bwd_camera_kernel(GB_PARAMS, double* __restrict__ cam_part) {
+  gauss_bwd_body<true>(GB_ARGS, cam_part);
+}
+
+#undef GB_PARAMS
+#undef GB_ARGS
+
+// dL_dcamera[j] = the sum of the spans' partials of term j, rounded to float once.  The order depends on nspans only:
+// thread i adds spans i, i + CR_THREADS, ... in turn, then a fixed tree adds the threads' sums.
+constexpr int CR_THREADS = 256;
+__global__ void __launch_bounds__(CR_THREADS)
+camera_reduce_kernel(int nspans, const double* __restrict__ cam_part, float* __restrict__ dL_dcamera) {
+  __shared__ double s[CR_THREADS];
+  const int j = blockIdx.x, t = threadIdx.x;
+  const double* p = cam_part + (size_t)j * nspans;
+  double v = 0.0;
+  for (int i = t; i < nspans; i += CR_THREADS) v += p[i];
+  s[t] = v;
+  __syncthreads();
+#pragma unroll
+  for (int w = CR_THREADS / 2; w > 0; w >>= 1) {
+    if (t < w) s[t] += s[t + w];
+    __syncthreads();
+  }
+  if (t == 0) dL_dcamera[j] = (float)s[0];
 }
 
 }  // namespace
@@ -625,12 +757,22 @@ void sfgs_launch_acc_clear_visible(int P, const int* radii, float* acc, cudaStre
   acc_clear_visible_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, radii, acc);
 }
 
+size_t sfgs_camera_scratch_bytes(int P) { return sfgs_align_up((size_t)GB_CAM * ((P + GB_SPAN - 1) / GB_SPAN) * sizeof(double)); }
+
+void sfgs_launch_camera_reduce(int P, const double* cam_part, float* dL_dcamera, cudaStream_t st) {
+  SFGS_COUNT_LAUNCH();
+  camera_reduce_kernel<<<GB_CAM, CR_THREADS, 0, st>>>((P + GB_SPAN - 1) / GB_SPAN, cam_part, dL_dcamera);
+}
+
+// cam_part: NULL for the adjoint alone; else [35][spans] doubles (sfgs_camera_scratch_bytes) that receive every span's
+// camera partials
 void sfgs_launch_gauss_bwd(const sfgs_backward_args* a, const GeomLayout& g, float focal_x, float focal_y,
-                           const float* acc, int g_begin, int g_end, int acc_row0, cudaStream_t st) {
+                           const float* acc, int g_begin, int g_end, int acc_row0, double* cam_part, cudaStream_t st) {
   if (g_end <= g_begin) return;
   static SfgsPerDeviceOnce attr_once;
   if (attr_once.first_use()) {
     cudaFuncSetAttribute(gauss_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GbShared));
+    cudaFuncSetAttribute(gauss_bwd_camera_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GbShared));
   }
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
@@ -643,9 +785,15 @@ void sfgs_launch_gauss_bwd(const sfgs_backward_args* a, const GeomLayout& g, flo
   const float* cov3D_ptr = a->cov3D_precomp != nullptr ? a->cov3D_precomp : g.cov3D;
   float* dL_dsh = a->M > 0 ? a->dL_dsh : nullptr;
   SFGS_COUNT_LAUNCH();
-  gauss_bwd_kernel<<<blocks, GB_THREADS, sizeof(GbShared), st>>>(
-      g_begin, g_end, spans_per_cta, acc_row0, a->D, a->M, a->means3D, a->radii, a->shs, g.clamped, a->scales, a->rotations,
-      a->scale_modifier, cov3D_ptr, g.rec, a->norm3D_precomp, a->viewmatrix, a->projmatrix, focal_x, focal_y,
-      a->tan_fovx, a->tan_fovy, a->kernel_size, a->cam_pos, acc, a->dL_dmean2D, a->dL_dconic, a->dL_dopacity,
-      a->dL_dcolor, a->dL_ddepth, a->dL_dmean3D, a->dL_dcov3D, a->dL_dnorm3D, dL_dsh, a->dL_dscale, a->dL_drot);
+#define GB_LAUNCH_ARGS                                                                                               \
+  g_begin, g_end, spans_per_cta, acc_row0, a->D, a->M, a->means3D, a->radii, a->shs, g.clamped, a->scales,          \
+      a->rotations, a->scale_modifier, cov3D_ptr, g.rec, a->norm3D_precomp, a->viewmatrix, a->projmatrix, focal_x,  \
+      focal_y, a->tan_fovx, a->tan_fovy, a->kernel_size, a->cam_pos, acc, a->dL_dmean2D, a->dL_dconic,              \
+      a->dL_dopacity, a->dL_dcolor, a->dL_ddepth, a->dL_dmean3D, a->dL_dcov3D, a->dL_dnorm3D, dL_dsh, a->dL_dscale, \
+      a->dL_drot
+  if (cam_part != nullptr)
+    gauss_bwd_camera_kernel<<<blocks, GB_THREADS, sizeof(GbShared), st>>>(GB_LAUNCH_ARGS, cam_part);
+  else
+    gauss_bwd_kernel<<<blocks, GB_THREADS, sizeof(GbShared), st>>>(GB_LAUNCH_ARGS);
+#undef GB_LAUNCH_ARGS
 }

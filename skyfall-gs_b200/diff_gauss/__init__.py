@@ -14,6 +14,7 @@ statistics consumed by scene/gaussian_model.py:744-749.
 """
 from __future__ import annotations
 
+import functools
 import os
 import sys
 from typing import NamedTuple
@@ -95,16 +96,24 @@ def _with_offset(fn):
 
 
 class _RasterizeGaussians(torch.autograd.Function):
+    # viewmatrix, projmatrix and campos are inputs of their own (the settings tuple is not tracked by autograd), so a
+    # camera built from parameters that require grad (scene/cameras.py: Camera(..., optimizing=True)) gets gradients.
+    CAMERA_INPUTS = slice(12, 15)
+
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                norm3Ds_precomp, extra_attrs, raster_settings, fuse_normalize=False):
+                norm3Ds_precomp, extra_attrs, raster_settings, fuse_normalize=False, viewmatrix=None, projmatrix=None,
+                campos=None):
         rs = raster_settings
+        viewmatrix = rs.viewmatrix if viewmatrix is None else viewmatrix
+        projmatrix = rs.projmatrix if projmatrix is None else projmatrix
+        campos = rs.campos if campos is None else campos
         n_extra = extra_attrs.shape[1] if extra_attrs.shape[0] != 0 else 0
         assert n_extra <= MAX_EXTRA_DIMS
         native_args = (rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier,
-                       cov3Ds_precomp, norm3Ds_precomp, extra_attrs, n_extra, rs.viewmatrix, rs.projmatrix,
+                       cov3Ds_precomp, norm3Ds_precomp, extra_attrs, n_extra, viewmatrix, projmatrix,
                        rs.tanfovx, rs.tanfovy, rs.kernel_size, rs.image_height, rs.image_width, sh, rs.sh_degree,
-                       rs.campos, rs.prefiltered, rs.debug)
+                       campos, rs.prefiltered, rs.debug)
         ctx.fused = bool(fuse_normalize)
         off = _subpixel_offset(rs)
         fwd = _C.rasterize_gaussians_fused if ctx.fused else _C.rasterize_gaussians
@@ -120,6 +129,7 @@ class _RasterizeGaussians(torch.autograd.Function):
             norm_raw = torch.empty(0, device=means3D.device)
         ctx.subpixel_offset = off
         ctx.raster_settings = rs
+        ctx.camera = (viewmatrix, projmatrix, campos)
         ctx.num_rendered = num_rendered
         ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, norm3Ds_precomp, radii,
                               extra_attrs, sh, geom_buf, binning_buf, img_buf, alpha, norm_raw)
@@ -131,27 +141,37 @@ class _RasterizeGaussians(torch.autograd.Function):
         rs = ctx.raster_settings
         (colors_precomp, means3D, scales, rotations, cov3Ds_precomp, norm3Ds_precomp, radii, extra_attrs, sh,
          geom_buf, binning_buf, img_buf, alpha, norm_raw) = ctx.saved_tensors
+        viewmatrix, projmatrix, campos = ctx.camera
         native_args = (rs.bg, means3D, radii, colors_precomp, scales, rotations, extra_attrs, rs.scale_modifier,
-                       cov3Ds_precomp, norm3Ds_precomp, rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy,
-                       rs.kernel_size, g_color, g_depth, g_norm, g_alpha, g_extra, sh, rs.sh_degree, rs.campos,
+                       cov3Ds_precomp, norm3Ds_precomp, viewmatrix, projmatrix, rs.tanfovx, rs.tanfovy,
+                       rs.kernel_size, g_color, g_depth, g_norm, g_alpha, g_extra, sh, rs.sh_degree, campos,
                        geom_buf, ctx.num_rendered, binning_buf, img_buf, alpha, rs.debug)
         bwd = _C.rasterize_gaussians_backward
         if ctx.fused:
             bwd = lambda *a, **kw: _C.rasterize_gaussians_backward_fused(*a, norm_raw=norm_raw, **kw)  # noqa: E731
+        camera_grad = any(ctx.needs_input_grad[_RasterizeGaussians.CAMERA_INPUTS])
+        if camera_grad:
+            # only when asked for: a camera without requires_grad keeps the default native call
+            bwd = functools.partial(bwd, camera_grad=True)
         if ctx.subpixel_offset is not None:
             bwd, native_args = _with_offset(bwd), native_args + (ctx.subpixel_offset,)
-        (g_means2D, g_colors, g_opac, g_means3D, g_cov3D, g_norm3D, g_sh, g_scales, g_rot,
-         g_extra_attrs) = _guarded(bwd, native_args, rs.debug, "snapshot_bw.dump", "backward")
+        grads = _guarded(bwd, native_args, rs.debug, "snapshot_bw.dump", "backward")
+        (g_means2D, g_colors, g_opac, g_means3D, g_cov3D, g_norm3D, g_sh, g_scales, g_rot, g_extra_attrs) = grads[:10]
+        g_camera = (None, None, None)
+        if camera_grad:
+            g_camera = tuple(g.to(dtype=t.dtype, device=t.device) if need else None for g, t, need in
+                             zip(grads[10:], ctx.camera, ctx.needs_input_grad[_RasterizeGaussians.CAMERA_INPUTS]))
         # order of forward's inputs; the settings tuple and the fusion flag get no gradient
         return (g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rot, g_cov3D, g_norm3D, g_extra_attrs,
-                None, None)
+                None, None) + g_camera
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                         norm3Ds_precomp, extra_attrs, raster_settings):
+    rs = raster_settings
     color, depth, norm, alpha, radii, extra = _RasterizeGaussians.apply(
         means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, norm3Ds_precomp,
-        extra_attrs, raster_settings, FUSE_NORMALIZE)
+        extra_attrs, raster_settings, FUSE_NORMALIZE, rs.viewmatrix, rs.projmatrix, rs.campos)
     if not FUSE_NORMALIZE:
         # the reference normalises the blended normal map in torch, inside the autograd graph (diff_gauss/__init__.py:48)
         norm = torch.nn.functional.normalize(norm, p=2, dim=0)

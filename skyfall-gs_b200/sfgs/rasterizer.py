@@ -200,7 +200,8 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
                                  kernel_size, dL_dout_color, dL_dout_depth, dL_dout_norm, dL_dout_alpha,
                                  dL_dout_extra, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer,
                                  out_alpha, debug, tile_rows=None, norm_raw=None, phase=0, acc=None,
-                                 gauss_range=None, acc_peers=None, peer_slice=0, subpixel_offset=None):
+                                 gauss_range=None, acc_peers=None, peer_slice=0, subpixel_offset=None,
+                                 camera_grad=False):
     """Same positional signature and return tuple as the reference's `_C.rasterize_gaussians_backward`.  With
     `norm_raw` (the extra tensor a `fuse_normalize=True` forward returned) `dL_dout_norm` is taken w.r.t. the unit
     normal map and the adjoint of F.normalize is applied inside the blend-adjoint kernel.
@@ -216,7 +217,11 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     warn and run the default backward.
 
     `subpixel_offset`: the tensor the forward was given (sfgs_rasterize_backward_subpixel and its deterministic form);
-    no gradient is formed with respect to it."""
+    no gradient is formed with respect to it.
+
+    `camera_grad=True` (one-call backward only): the same call through sfgs_rasterize_backward_camera, which also forms
+    the camera gradients; the tuple then ends with (dL_dviewmatrix [4,4], dL_dprojmatrix [4,4], dL_dcampos [3]), in the
+    layout of the inputs.  Every other output is bit-identical to the call without it."""
     if subpixel_offset is not None:
         check_subpixel_offset(subpixel_offset, int(dL_dout_color.shape[1]), int(dL_dout_color.shape[2]))
     F = int(extra_attrs.shape[1]) if (extra_attrs is not None and extra_attrs.numel() != 0) else 0
@@ -230,8 +235,9 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
 
     if P == 0:
         z = lambda *s: torch.zeros(s, **fopt)  # noqa: E731
-        return (z(P, 3), z(P, 3), z(P, 1), z(P, 3), z(P, 6), z(P, 3), z(P, M, 3), z(P, 3), z(P, 4),
-                z(P, F) if F > 0 else torch.empty(0, **fopt))
+        ret = (z(P, 3), z(P, 3), z(P, 1), z(P, 3), z(P, 6), z(P, 3), z(P, M, 3), z(P, 3), z(P, 4),
+               z(P, F) if F > 0 else torch.empty(0, **fopt))
+        return ret + (z(4, 4), z(4, 4), z(3)) if camera_grad else ret
 
     with torch.cuda.device(dev), _no_fill(deterministic):
         # one allocation for all fixed-width per-Gaussian gradients (every element is written by the kernel)
@@ -306,7 +312,12 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
         a.stream = torch.cuda.current_stream(dev).cuda_stream
         if tile_rows is not None:
             a.tile_row_begin, a.tile_row_end = _band(tile_rows)
-        if subpixel_offset is not None:
+        if camera_grad:
+            dL_dcamera = torch.empty((35,), **fopt)
+            off = _ptr(subpixel_offset, keep) if subpixel_offset is not None else None
+            N.check(L.sfgs_rasterize_backward_camera(C.byref(a), off, int(deterministic), dL_dcamera.data_ptr()),
+                    "sfgs_rasterize_backward_camera")
+        elif subpixel_offset is not None:
             off = _ptr(subpixel_offset, keep)
             if deterministic:
                 N.check(L.sfgs_rasterize_backward_deterministic_subpixel(C.byref(a), off),
@@ -323,8 +334,11 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
         scratch.tensor = None
     if phase == 1:
         return acc      # None when the sums went straight to the peers' slices
-    return (outs["means2D"], outs["colors"], outs["opacity"], outs["means3D"], outs["cov3D"], outs["norm3D"],
-            dL_dsh, outs["scales"], outs["rot"], dL_dextra)
+    ret = (outs["means2D"], outs["colors"], outs["opacity"], outs["means3D"], outs["cov3D"], outs["norm3D"],
+           dL_dsh, outs["scales"], outs["rot"], dL_dextra)
+    if camera_grad:
+        ret += (dL_dcamera[0:16].view(4, 4), dL_dcamera[16:32].view(4, 4), dL_dcamera[32:35])
+    return ret
 
 
 def mark_visible(means3D, viewmatrix, projmatrix):
