@@ -197,7 +197,8 @@ int sfgs_rasterize_backward(const sfgs_backward_args* a);
  *   phase 0 and phase 1 (the blend adjoint) need `radii` and `scratch_alloc`: the extra scratch is
  *     4 P + 524 R bytes (+ alignment; R = instances of the forward), on top of the P*16 floats of `acc` when that is
  *     not given;
- *   (sfgs_rasterize_backward_camera adds 35 * 8 * ceil(P / 96) bytes for the camera partials);
+ *   (sfgs_rasterize_backward_camera adds 35 * 8 * ceil(P / 96) bytes for the camera partials,
+ *   sfgs_rasterize_backward_camera_intrinsics 37 * 8 * ceil(P / 96));
  *   phase 2 runs the per-Gaussian adjoint, which has no reduction, exactly as sfgs_rasterize_backward does;
  *   acc_peers (system-scope reductions) and ED > 0 (extra_attrs) return SFGS_E_UNSUPPORTED before any CUDA work.
  * The outputs equal sfgs_rasterize_backward's up to the rounding of the sums' order. */
@@ -236,9 +237,23 @@ int sfgs_rasterize_backward_deterministic_subpixel(const sfgs_backward_args* a, 
  *     backward it follows needs.
  *   - Phase 0 only: phases 1 and 2 and acc_peers return SFGS_E_UNSUPPORTED, a NULL dL_dcamera SFGS_E_BADARG, before
  *     any CUDA work.
- * No gradient is formed for tan_fovx / tan_fovy (the intrinsics) or the subpixel offsets. */
+ * No gradient is formed for tan_fovx / tan_fovy (see sfgs_rasterize_backward_camera_intrinsics) or the subpixel
+ * offsets. */
 int sfgs_rasterize_backward_camera(const sfgs_backward_args* a, const float* subpixel_offset, int deterministic,
                                    float* dL_dcamera);
+
+/* ---- camera and focal-length gradients (focal refinement) ----------------------------------------------------------
+ * sfgs_rasterize_backward_camera with dL_dcamera a DEVICE [37] float array: the 35 camera gradients in the layout
+ * above, then dL/dtan_fovx and dL/dtan_fovy.  The focal lengths W / (2 tan_fovx) and H / (2 tan_fovy) enter the EWA
+ * Jacobian J (and through it the 2D covariance, the Mip coefficient and the conic); the frustum clamp bounds
+ * ±1.3 tan_fov move with them, so a clamped t_x / t_y contributes through the bound.  The principal point and the
+ * projection entries of the field of view enter through projmatrix and are in dL/dprojmatrix.  The cull, the radius
+ * and the tile lists are discrete and contribute nothing.
+ *   - The first 35 entries and every other output are bit-identical to sfgs_rasterize_backward_camera's.
+ *   - Summation, reproducibility, arguments and rejections as for sfgs_rasterize_backward_camera; the extra scratch is
+ *     37 * 8 * ceil(P / 96) bytes (+ alignment). */
+int sfgs_rasterize_backward_camera_intrinsics(const sfgs_backward_args* a, const float* subpixel_offset,
+                                              int deterministic, float* dL_dcamera);
 
 /* ---- markVisible --------------------------------------------------------- */
 int sfgs_mark_visible(int P, const float* means3D, const float* viewmatrix,

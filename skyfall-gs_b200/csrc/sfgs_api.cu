@@ -53,9 +53,10 @@ int sfgs_launch_activations_bwd(int P, const float* opacity_raw, const float* sc
                                 const float* g_rotations, float* g_opacity_raw, float* g_scaling_raw,
                                 float* g_rotation_raw, cudaStream_t st);
 void sfgs_launch_gauss_bwd(const sfgs_backward_args* a, const GeomLayout& g, float focal_x, float focal_y,
-                           const float* acc, int g_begin, int g_end, int acc_row0, double* cam_part, cudaStream_t st);
-size_t sfgs_camera_scratch_bytes(int P);
-void sfgs_launch_camera_reduce(int P, const double* cam_part, float* dL_dcamera, cudaStream_t st);
+                           const float* acc, int g_begin, int g_end, int acc_row0, double* cam_part, int ncam,
+                           cudaStream_t st);
+size_t sfgs_camera_scratch_bytes(int P, int ncam);
+void sfgs_launch_camera_reduce(int P, int ncam, const double* cam_part, float* dL_dcamera, cudaStream_t st);
 void sfgs_launch_acc_clear_visible(int P, const int* radii, float* acc, cudaStream_t st);
 
 namespace {
@@ -194,7 +195,8 @@ constexpr int MAX_DEVICES = 64;
 thread_local PinnedHdr t_hdr_dev[MAX_DEVICES];
 
 int rasterize_forward(const sfgs_forward_args* a, const float* off);
-int rasterize_backward(const sfgs_backward_args* a, bool deterministic, const float* off, float* dL_dcamera);
+int rasterize_backward(const sfgs_backward_args* a, bool deterministic, const float* off, float* dL_dcamera,
+                       int ncam);
 
 // the combinations the subpixel-offset entry points have no kernels for (checked before any CUDA work)
 int subpixel_unsupported_fwd(const sfgs_forward_args* a) {
@@ -206,6 +208,25 @@ int subpixel_unsupported_bwd(const sfgs_backward_args* a) {
   if (a->ED > 0) return fail(SFGS_E_UNSUPPORTED, "backward_subpixel: extra_attrs are not supported with subpixel offsets");
   if (a->acc_peers != nullptr) return fail(SFGS_E_UNSUPPORTED, "backward_subpixel: acc_peers are not supported with subpixel offsets");
   return SFGS_OK;
+}
+
+// the camera entries: ncam = 35 (pose terms) or 37 (pose and focal terms); the checks come before any CUDA work
+int backward_camera(const char* name, const sfgs_backward_args* a, const float* off, int deterministic,
+                    float* dL_dcamera, int ncam) {
+  auto reject = [name](int code, const char* what) {
+    char m[160];
+    snprintf(m, sizeof(m), "%s: %s", name, what);
+    return fail(code, m);
+  };
+  if (!a) return reject(SFGS_E_BADARG, "null args");
+  if (!dL_dcamera) return reject(SFGS_E_BADARG, "null dL_dcamera");
+  if (a->phase != 0)
+    return reject(SFGS_E_UNSUPPORTED, "camera gradients are formed by the one-call backward (phase 0) only");
+  if (a->acc_peers != nullptr)
+    return reject(SFGS_E_UNSUPPORTED, "acc_peers (the multi-GPU backward) have no camera gradients");
+  if (!a->scratch_alloc) return reject(SFGS_E_BADARG, "null scratch allocator");
+  if (off != nullptr && subpixel_unsupported_bwd(a)) return SFGS_E_UNSUPPORTED;
+  return rasterize_backward(a, deterministic != 0, off, dL_dcamera, ncam);
 }
 
 }  // namespace
@@ -245,8 +266,8 @@ int sfgs_binning_layout(char* base, long long capacity, sfgs_binning_view* out) 
 }
 
 int sfgs_rasterize_forward(const sfgs_forward_args* a) { return rasterize_forward(a, nullptr); }
-int sfgs_rasterize_backward(const sfgs_backward_args* a) { return rasterize_backward(a, false, nullptr, nullptr); }
-int sfgs_rasterize_backward_deterministic(const sfgs_backward_args* a) { return rasterize_backward(a, true, nullptr, nullptr); }
+int sfgs_rasterize_backward(const sfgs_backward_args* a) { return rasterize_backward(a, false, nullptr, nullptr, 0); }
+int sfgs_rasterize_backward_deterministic(const sfgs_backward_args* a) { return rasterize_backward(a, true, nullptr, nullptr, 0); }
 
 int sfgs_rasterize_forward_subpixel(const sfgs_forward_args* a, const float* subpixel_offset) {
   if (!a) return fail(SFGS_E_BADARG, "forward: null args");
@@ -256,25 +277,22 @@ int sfgs_rasterize_forward_subpixel(const sfgs_forward_args* a, const float* sub
 int sfgs_rasterize_backward_subpixel(const sfgs_backward_args* a, const float* subpixel_offset) {
   if (!a) return fail(SFGS_E_BADARG, "backward: null args");
   if (subpixel_offset != nullptr && subpixel_unsupported_bwd(a)) return SFGS_E_UNSUPPORTED;
-  return rasterize_backward(a, false, subpixel_offset, nullptr);
+  return rasterize_backward(a, false, subpixel_offset, nullptr, 0);
 }
 int sfgs_rasterize_backward_deterministic_subpixel(const sfgs_backward_args* a, const float* subpixel_offset) {
   if (!a) return fail(SFGS_E_BADARG, "backward: null args");
   if (subpixel_offset != nullptr && subpixel_unsupported_bwd(a)) return SFGS_E_UNSUPPORTED;
-  return rasterize_backward(a, true, subpixel_offset, nullptr);
+  return rasterize_backward(a, true, subpixel_offset, nullptr, 0);
 }
 
 int sfgs_rasterize_backward_camera(const sfgs_backward_args* a, const float* subpixel_offset, int deterministic,
                                    float* dL_dcamera) {
-  if (!a) return fail(SFGS_E_BADARG, "backward_camera: null args");
-  if (!dL_dcamera) return fail(SFGS_E_BADARG, "backward_camera: null dL_dcamera");
-  if (a->phase != 0)
-    return fail(SFGS_E_UNSUPPORTED, "backward_camera: camera gradients are formed by the one-call backward (phase 0) only");
-  if (a->acc_peers != nullptr)
-    return fail(SFGS_E_UNSUPPORTED, "backward_camera: acc_peers (the multi-GPU backward) have no camera gradients");
-  if (!a->scratch_alloc) return fail(SFGS_E_BADARG, "backward_camera: null scratch allocator");
-  if (subpixel_offset != nullptr && subpixel_unsupported_bwd(a)) return SFGS_E_UNSUPPORTED;
-  return rasterize_backward(a, deterministic != 0, subpixel_offset, dL_dcamera);
+  return backward_camera("backward_camera", a, subpixel_offset, deterministic, dL_dcamera, 35);
+}
+
+int sfgs_rasterize_backward_camera_intrinsics(const sfgs_backward_args* a, const float* subpixel_offset,
+                                              int deterministic, float* dL_dcamera) {
+  return backward_camera("backward_camera_intrinsics", a, subpixel_offset, deterministic, dL_dcamera, 37);
 }
 
 }  // extern "C"
@@ -391,8 +409,10 @@ int rasterize_forward(const sfgs_forward_args* a, const float* off) {
   return (int)R;
 }
 
-// dL_dcamera: NULL, or (phase 0 only, checked by the caller) the DEVICE [35] camera gradients to form as well
-int rasterize_backward(const sfgs_backward_args* a, bool deterministic, const float* off, float* dL_dcamera) {
+// dL_dcamera: NULL, or (phase 0 only, checked by the caller) the DEVICE [ncam] camera gradients to form as well:
+// ncam = 35 (pose terms) or 37 (pose and focal terms)
+int rasterize_backward(const sfgs_backward_args* a, bool deterministic, const float* off, float* dL_dcamera,
+                       int ncam) {
   if (!a) return fail(SFGS_E_BADARG, "backward: null args");
   if (a->P < 0 || a->width <= 0 || a->height <= 0) return fail(SFGS_E_BADARG, "backward: bad sizes");
   if (deterministic && a->acc_peers != nullptr)
@@ -401,7 +421,7 @@ int rasterize_backward(const sfgs_backward_args* a, bool deterministic, const fl
     return fail(SFGS_E_UNSUPPORTED, "backward_deterministic: extra_attrs have no deterministic implementation");
   const bool cam = dL_dcamera != nullptr;
   if (a->P == 0) {
-    if (cam) CU(cudaMemsetAsync(dL_dcamera, 0, 35 * sizeof(float), (cudaStream_t)a->stream));
+    if (cam) CU(cudaMemsetAsync(dL_dcamera, 0, (size_t)ncam * sizeof(float), (cudaStream_t)a->stream));
     return SFGS_OK;
   }
   const int phase = a->phase;
@@ -458,7 +478,7 @@ int rasterize_backward(const sfgs_backward_args* a, bool deterministic, const fl
   if ((!acc && !peer) || ordered || cam) {
     const size_t acc_bytes = !acc ? sfgs_align_up((size_t)P * 16 * sizeof(float)) : 0;
     const size_t order_bytes = ordered ? sfgs_order_scratch_bytes(P, R) : 0;
-    const size_t abytes = acc_bytes + order_bytes + (cam ? sfgs_camera_scratch_bytes(P) : 0) + SFGS_ALIGN;
+    const size_t abytes = acc_bytes + order_bytes + (cam ? sfgs_camera_scratch_bytes(P, ncam) : 0) + SFGS_ALIGN;
     char* aptr = a->scratch_alloc(a->scratch_user, abytes);
     if (!aptr) return fail(SFGS_E_ALLOC, "backward: scratch allocator returned NULL");
     char* base = sfgs_align_ptr(aptr);
@@ -504,8 +524,8 @@ int rasterize_backward(const sfgs_backward_args* a, bool deterministic, const fl
   }
   if (do_gauss) {
     PROF_BEGIN(ST_GAUSS_BWD);
-    sfgs_launch_gauss_bwd(a, g, focal_x, focal_y, acc, g_begin, g_end, phase == 2 ? g_begin : 0, cam_part, st);
-    if (cam) sfgs_launch_camera_reduce(P, cam_part, dL_dcamera, st);
+    sfgs_launch_gauss_bwd(a, g, focal_x, focal_y, acc, g_begin, g_end, phase == 2 ? g_begin : 0, cam_part, ncam, st);
+    if (cam) sfgs_launch_camera_reduce(P, ncam, cam_part, dL_dcamera, st);
     PROF_END();
     STAGE_CHECK("gauss_bwd");
   }

@@ -39,8 +39,8 @@ constexpr int GB_FIXED = 31;       // fixed-width gradient floats per Gaussian
 constexpr int GB_SH_ROW = 19;      // staged dL_dsh factors per Gaussian (odd: rows start in different banks)
 constexpr int GB_NFIXED = 10;     // fixed-width output arrays
 // camera terms of one Gaussian (the camera adjoint): dL/dviewmatrix[16], dL/dprojmatrix[16], dL/dcampos[3], each in its
-// input's element order [4*c + r]
-constexpr int C_VIEW = 0, C_PROJ = 16, C_CAMPOS = 32, GB_CAM = 35;
+// input's element order [4*c + r] (the GB_CAM_POSE pose terms), then dL/dtan_fovx and dL/dtan_fovy (the focal terms)
+constexpr int C_VIEW = 0, C_PROJ = 16, C_CAMPOS = 32, GB_CAM_POSE = 35, C_TANX = 35, C_TANY = 36, GB_CAM = 37;
 
 // Shared-memory image of one stage's inputs, indexed by slot (position in the stage's list of visible Gaussians).
 // Field-major, so the adjoint's threads (consecutive slots) read consecutive words.
@@ -95,20 +95,21 @@ __device__ __forceinline__ float3 dnormvdv3(float3 v, float3 dv) {
 
 // The adjoint chain of one rasterized Gaussian from its blend-adjoint sums A0..A3 and forward record rec1..rec3.
 // The expressions and their float/double promotions are the reference's; do not reassociate them.
-// CAM: also the Gaussian's camera terms (cam), the adjoint of the same chain with respect to the camera: the view-space
+// NCAM > 0: also the Gaussian's camera terms (cam), the adjoint of the same chain with respect to the camera: the view-space
 // point t (dL/dt, with the depth) and W of J(t)·W (dL/dT), the projected centre (the 1/(w + 1e-7) multipliers) and the
 // SH view direction (minus the dnormvdv3 result).  Entries the forward does not read (viewmatrix[3,7,11,15],
-// projmatrix[2,6,10,14]) stay 0.
-template <bool CAM, class SH>
+// projmatrix[2,6,10,14]) stay 0.  NCAM: the number of camera terms formed, 0 (none), GB_CAM_POSE or GB_CAM (the pose
+// terms and the focal terms).
+template <int NCAM, class SH>
 __device__ __forceinline__ void gauss_adjoint(
     int D, float mx, float my, float mz, bool has_scales, float4 q_in, float scx, float scy, float scz,
     float scale_modifier, bool has_sh, unsigned cm, SH sh, const float* cov3D, bool norm_precomp, float4 A0,
     float4 A1, float4 A2, float4 A3, float4 rec1, float4 rec2, float4 rec3, const float* __restrict__ view,
     const float* __restrict__ proj, float h_x, float h_y, float tan_fovx, float tan_fovy, float kernel_size,
     const float* __restrict__ campos, float (&out)[GB_ROW], float (&cam)[GB_CAM]) {
-  if constexpr (CAM) {
+  if constexpr (NCAM > 0) {
 #pragma unroll
-    for (int j = 0; j < GB_CAM; j++) cam[j] = 0.f;
+    for (int j = 0; j < NCAM; j++) cam[j] = 0.f;
   }
   float o_mean2D[3] = {0, 0, 0}, o_conic[4] = {0, 0, 0, 0}, o_opac = 0, o_color[3] = {0, 0, 0}, o_depth = 0;
   float o_mean[3] = {0, 0, 0}, o_cov[6] = {0, 0, 0, 0, 0, 0}, o_norm[3] = {0, 0, 0};
@@ -219,7 +220,7 @@ __device__ __forceinline__ void gauss_adjoint(
     o_mean[0] = view[0] * dL_dtx + view[1] * dL_dty + view[2] * dL_dtz;
     o_mean[1] = view[4] * dL_dtx + view[5] * dL_dty + view[6] * dL_dtz;
     o_mean[2] = view[8] * dL_dtx + view[9] * dL_dty + view[10] * dL_dtz;
-    if constexpr (CAM) {
+    if constexpr (NCAM > 0) {
       // t = [m, 1]·view (columns 0..2): dL/dview[4k + r] = m_k dL/dt_r, dL/dview[12 + r] = dL/dt_r.  T = J·W with
       // W[k][r] = view[4r + k] and J = [[a0, 0, a2], [0, b1, b2]]: dL/dW[k][r] = sum_i J[i][k] dL/dT[i][r].
       const float m3[3] = {mx, my, mz};
@@ -237,6 +238,21 @@ __device__ __forceinline__ void gauss_adjoint(
         cam[C_VIEW + 4 * r + 1] += b1 * dT1[r];
         cam[C_VIEW + 4 * r + 2] += a2 * dT0[r] + b2 * dT1[r];
       }
+    }
+    if constexpr (NCAM > C_TANY) {
+      // The focal terms.  h = W / (2 tan) enters J00 = h_x / tz and J02 = -h_x tx / tz^2 (tx the clamped t_x), so
+      // dL/dh_x = dL/dJ00 / tz - dL/dJ02 tx / tz^2 and dh_x/dtan_fovx = -h_x / tan_fovx.  A clamped t_x is
+      // ±1.3 tan_fovx · tz: J02 then also moves with the bound, by ∓1.3 h_x / tz.  Likewise y with h_y, J11, J12.
+      // In double, from the float values the chain already holds: new uses of its float products could change the
+      // compiler's fusion of them into the gradient sums.
+      const double z = tz, zi = 1.0 / z, hx = h_x, hy = h_y;
+      const double dJ02 = dL_dJ02, dJ12 = dL_dJ12;
+      double gtx = -(hx / (double)tan_fovx) * (((double)dL_dJ00 - dJ02 * (double)tx * zi) * zi);
+      double gty = -(hy / (double)tan_fovy) * (((double)dL_dJ11 - dJ12 * (double)ty * zi) * zi);
+      if (txtz < -limx || txtz > limx) gtx += dJ02 * ((txtz > 0.f ? -1.3 : 1.3) * hx * zi);
+      if (tytz < -limy || tytz > limy) gty += dJ12 * ((tytz > 0.f ? -1.3 : 1.3) * hy * zi);
+      cam[C_TANX] = (float)gtx;
+      cam[C_TANY] = (float)gty;
     }
   }
 
@@ -256,7 +272,7 @@ __device__ __forceinline__ void gauss_adjoint(
     const float e1 = (view[6] - view[7] * mul3) * o_depth;
     const float e2 = (view[10] - view[11] * mul3) * o_depth;
     o_mean[0] += e0; o_mean[1] += e1; o_mean[2] += e2;
-    if constexpr (CAM) {
+    if constexpr (NCAM > 0) {
       // the homogeneous centre [m, 1]·proj and its divide: dL/dhom = (gx w, gy w, ., -(gx mul1 + gy mul2)), w = m_w;
       // the depth is t_z: dL/dview[4k + 2] = m_k dL/ddepth, dL/dview[14] = dL/ddepth
       const float m3[3] = {mx, my, mz};
@@ -337,7 +353,7 @@ __device__ __forceinline__ void gauss_adjoint(
       dL_ddir.z = dRGBdz[0] * dL_dRGB[0] + dRGBdz[1] * dL_dRGB[1] + dRGBdz[2] * dL_dRGB[2];
       const float3 dm = dnormvdv3(make_float3(ox, oy, oz), dL_ddir);
       o_mean[0] += dm.x; o_mean[1] += dm.y; o_mean[2] += dm.z;
-      if constexpr (CAM) {
+      if constexpr (NCAM > 0) {
         // -dnormvdv3(v, dL_ddir), evaluated again in double: reading dm here would give its final products a second
         // use, and the compiler would then no longer fuse them into the o_mean sums, changing dL_dmean3D's rounding
         const double vx = ox, vy = oy, vz = oz, gx = dL_ddir.x, gy = dL_ddir.y, gz = dL_ddir.z;
@@ -482,9 +498,10 @@ constexpr int GB_CAM_STAGE = (GB_SPAN * (GB_SH_ROW + GB_FIXED) + 4 * GB_NFIXED +
 static_assert(sizeof(float) * (GB_CAM_STAGE + GB_CAM * GB_SLOTS) <= sizeof(GbInputs),
               "a stage's camera terms fit beside a span's staged outputs");
 
-// The per-Gaussian adjoint over spans [g_begin, g_end).  CAM: also the camera adjoint; span s (counted from g_begin)
-// writes cam_part[j * nspans + s], the float64 sum of its rasterized Gaussians' camera term j in index order.
-template <bool CAM>
+// The per-Gaussian adjoint over spans [g_begin, g_end).  NCAM > 0: also the first NCAM camera terms; span s (counted
+// from g_begin) writes cam_part[j * nspans + s], the float64 sum of its rasterized Gaussians' camera term j in index
+// order.
+template <int NCAM>
 __device__ __forceinline__ void
 gauss_bwd_body(int g_begin, int g_end, int spans_per_cta, int acc_row0, int D, int M,
                const float* __restrict__ means3D, const int* __restrict__ radii, const float* __restrict__ shs,
@@ -613,7 +630,7 @@ gauss_bwd_body(int g_begin, int g_end, int spans_per_cta, int acc_row0, int D, i
       const float* shk = reinterpret_cast<const float*>(&in.sh[0][k]);   // float j at word (j >> 2) * 4 * SLOTS + (j & 3)
       const float cov3D[6] = {in.cov[0][k], in.cov[1][k], in.cov[2][k], in.cov[3][k], in.cov[4][k], in.cov[5][k]};
       const unsigned cm = has_sh ? (in.clamped[k] >> (8 * (S.gidx[b][k] & 3))) & 0xffu : 0u;
-      gauss_adjoint<CAM>(D, in.mean[0][k], in.mean[1][k], in.mean[2][k], has_scales,
+      gauss_adjoint<NCAM>(D, in.mean[0][k], in.mean[1][k], in.mean[2][k], has_scales,
                     has_scales ? in.rot[k] : make_float4(0.f, 0.f, 0.f, 0.f),
                     has_scales ? in.scale[0][k] : 0.f, has_scales ? in.scale[1][k] : 0.f,
                     has_scales ? in.scale[2][k] : 0.f, scale_modifier, has_sh, cm,
@@ -651,16 +668,16 @@ gauss_bwd_body(int g_begin, int g_end, int spans_per_cta, int acc_row0, int D, i
       };
       if (active && rel / GB_SPAN == sp) stage(rel % GB_SPAN, false);
       if (t < n && S.slot[b][sp][t] < 0) stage(t, true);
-      if constexpr (CAM) {
+      if constexpr (NCAM > 0) {
         if (sp == 0 && active) {
 #pragma unroll
-          for (int j = 0; j < GB_CAM; j++) cam_stage[j * GB_SLOTS + t] = cam[j];
+          for (int j = 0; j < NCAM; j++) cam_stage[j * GB_SLOTS + t] = cam[j];
         }
       }
       __syncthreads();
-      if constexpr (CAM) {
+      if constexpr (NCAM > 0) {
         // thread j sums term j over the span's Gaussians in index order
-        if (t < GB_CAM) {
+        if (t < NCAM) {
           double s = 0.0;
           for (int p = 0; p < n; p++) {
             const int k = S.slot[b][sp][p];
@@ -706,12 +723,18 @@ gauss_bwd_body(int g_begin, int g_end, int spans_per_cta, int acc_row0, int D, i
       dL_dconic, dL_dopacity, dL_dcolor, dL_ddepth, dL_dmean3D, dL_dcov3D, dL_dnorm3D, dL_dsh, dL_dscale, dL_drot
 
 __global__ void __launch_bounds__(GB_THREADS, GB_CTAS_PER_SM) gauss_bwd_kernel(GB_PARAMS) {
-  gauss_bwd_body<false>(GB_ARGS, nullptr);
+  gauss_bwd_body<0>(GB_ARGS, nullptr);
 }
 
 __global__ void __launch_bounds__(GB_THREADS, GB_CTAS_PER_SM)
 gauss_bwd_camera_kernel(GB_PARAMS, double* __restrict__ cam_part) {
-  gauss_bwd_body<true>(GB_ARGS, cam_part);
+  gauss_bwd_body<GB_CAM_POSE>(GB_ARGS, cam_part);
+}
+
+// the pose terms and the focal terms: a kernel of its own, so that the pose-only camera backward keeps its code
+__global__ void __launch_bounds__(GB_THREADS, GB_CTAS_PER_SM)
+gauss_bwd_intrinsics_kernel(GB_PARAMS, double* __restrict__ cam_part) {
+  gauss_bwd_body<GB_CAM>(GB_ARGS, cam_part);
 }
 
 #undef GB_PARAMS
@@ -757,22 +780,27 @@ void sfgs_launch_acc_clear_visible(int P, const int* radii, float* acc, cudaStre
   acc_clear_visible_kernel<<<(P + 255) / 256, 256, 0, st>>>(P, radii, acc);
 }
 
-size_t sfgs_camera_scratch_bytes(int P) { return sfgs_align_up((size_t)GB_CAM * ((P + GB_SPAN - 1) / GB_SPAN) * sizeof(double)); }
-
-void sfgs_launch_camera_reduce(int P, const double* cam_part, float* dL_dcamera, cudaStream_t st) {
-  SFGS_COUNT_LAUNCH();
-  camera_reduce_kernel<<<GB_CAM, CR_THREADS, 0, st>>>((P + GB_SPAN - 1) / GB_SPAN, cam_part, dL_dcamera);
+// ncam: the number of camera terms, 35 (pose) or 37 (pose and focal)
+size_t sfgs_camera_scratch_bytes(int P, int ncam) {
+  return sfgs_align_up((size_t)ncam * ((P + GB_SPAN - 1) / GB_SPAN) * sizeof(double));
 }
 
-// cam_part: NULL for the adjoint alone; else [35][spans] doubles (sfgs_camera_scratch_bytes) that receive every span's
-// camera partials
+void sfgs_launch_camera_reduce(int P, int ncam, const double* cam_part, float* dL_dcamera, cudaStream_t st) {
+  SFGS_COUNT_LAUNCH();
+  camera_reduce_kernel<<<ncam, CR_THREADS, 0, st>>>((P + GB_SPAN - 1) / GB_SPAN, cam_part, dL_dcamera);
+}
+
+// cam_part: NULL for the adjoint alone; else [ncam][spans] doubles (sfgs_camera_scratch_bytes) that receive every
+// span's camera partials, ncam = 35 (pose terms) or 37 (pose and focal terms)
 void sfgs_launch_gauss_bwd(const sfgs_backward_args* a, const GeomLayout& g, float focal_x, float focal_y,
-                           const float* acc, int g_begin, int g_end, int acc_row0, double* cam_part, cudaStream_t st) {
+                           const float* acc, int g_begin, int g_end, int acc_row0, double* cam_part, int ncam,
+                           cudaStream_t st) {
   if (g_end <= g_begin) return;
   static SfgsPerDeviceOnce attr_once;
   if (attr_once.first_use()) {
     cudaFuncSetAttribute(gauss_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GbShared));
     cudaFuncSetAttribute(gauss_bwd_camera_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GbShared));
+    cudaFuncSetAttribute(gauss_bwd_intrinsics_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GbShared));
   }
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
@@ -791,7 +819,9 @@ void sfgs_launch_gauss_bwd(const sfgs_backward_args* a, const GeomLayout& g, flo
       focal_y, a->tan_fovx, a->tan_fovy, a->kernel_size, a->cam_pos, acc, a->dL_dmean2D, a->dL_dconic,              \
       a->dL_dopacity, a->dL_dcolor, a->dL_ddepth, a->dL_dmean3D, a->dL_dcov3D, a->dL_dnorm3D, dL_dsh, a->dL_dscale, \
       a->dL_drot
-  if (cam_part != nullptr)
+  if (cam_part != nullptr && ncam == GB_CAM)
+    gauss_bwd_intrinsics_kernel<<<blocks, GB_THREADS, sizeof(GbShared), st>>>(GB_LAUNCH_ARGS, cam_part);
+  else if (cam_part != nullptr)
     gauss_bwd_camera_kernel<<<blocks, GB_THREADS, sizeof(GbShared), st>>>(GB_LAUNCH_ARGS, cam_part);
   else
     gauss_bwd_kernel<<<blocks, GB_THREADS, sizeof(GbShared), st>>>(GB_LAUNCH_ARGS);

@@ -47,7 +47,7 @@ SUBPIXEL_OFFSET = os.environ.get("SFGS_SUBPIXEL_OFFSET", "0") == "1"
 class GaussianRasterizationSettings(NamedTuple):
     image_height: int
     image_width: int
-    tanfovx: float
+    tanfovx: float      # or a 0-d tensor: one that requires grad gets dL/dtanfovx (focal refinement)
     tanfovy: float
     kernel_size: float
     subpixel_offset: torch.Tensor  # ignored (as by the reference) unless SUBPIXEL_OFFSET is on
@@ -95,16 +95,24 @@ def _with_offset(fn):
     return lambda *a, **kw: fn(*a[:-1], subpixel_offset=a[-1], **kw)
 
 
+def _requires_grad(x):
+    return isinstance(x, torch.Tensor) and x.requires_grad
+
+
 class _RasterizeGaussians(torch.autograd.Function):
     # viewmatrix, projmatrix and campos are inputs of their own (the settings tuple is not tracked by autograd), so a
     # camera built from parameters that require grad (scene/cameras.py: Camera(..., optimizing=True)) gets gradients.
     CAMERA_INPUTS = slice(12, 15)
+    # tanfovx and tanfovy likewise, passed only when one of them is a tensor that requires grad (focal refinement);
+    # otherwise the settings' values are used, as they always were
+    INTRINSICS_INPUTS = slice(15, 17)
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                 norm3Ds_precomp, extra_attrs, raster_settings, fuse_normalize=False, viewmatrix=None, projmatrix=None,
-                campos=None):
+                campos=None, tanfovx=None, tanfovy=None):
         rs = raster_settings
+        ctx.intrinsics = None if tanfovx is None else (tanfovx, tanfovy)
         viewmatrix = rs.viewmatrix if viewmatrix is None else viewmatrix
         projmatrix = rs.projmatrix if projmatrix is None else projmatrix
         campos = rs.campos if campos is None else campos
@@ -150,7 +158,12 @@ class _RasterizeGaussians(torch.autograd.Function):
         if ctx.fused:
             bwd = lambda *a, **kw: _C.rasterize_gaussians_backward_fused(*a, norm_raw=norm_raw, **kw)  # noqa: E731
         camera_grad = any(ctx.needs_input_grad[_RasterizeGaussians.CAMERA_INPUTS])
-        if camera_grad:
+        intrinsics_grad = ctx.intrinsics is not None and any(
+            ctx.needs_input_grad[_RasterizeGaussians.INTRINSICS_INPUTS])
+        if intrinsics_grad:
+            # the focal-length gradients come with the camera gradients, from one native call
+            bwd = functools.partial(bwd, camera_grad=True, intrinsics_grad=True)
+        elif camera_grad:
             # only when asked for: a camera without requires_grad keeps the default native call
             bwd = functools.partial(bwd, camera_grad=True)
         if ctx.subpixel_offset is not None:
@@ -158,20 +171,30 @@ class _RasterizeGaussians(torch.autograd.Function):
         grads = _guarded(bwd, native_args, rs.debug, "snapshot_bw.dump", "backward")
         (g_means2D, g_colors, g_opac, g_means3D, g_cov3D, g_norm3D, g_sh, g_scales, g_rot, g_extra_attrs) = grads[:10]
         g_camera = (None, None, None)
-        if camera_grad:
+        if camera_grad or intrinsics_grad:
             g_camera = tuple(g.to(dtype=t.dtype, device=t.device) if need else None for g, t, need in
-                             zip(grads[10:], ctx.camera, ctx.needs_input_grad[_RasterizeGaussians.CAMERA_INPUTS]))
+                             zip(grads[10:13], ctx.camera, ctx.needs_input_grad[_RasterizeGaussians.CAMERA_INPUTS]))
+        g_intrinsics = ()
+        if ctx.intrinsics is not None:
+            g_intrinsics = (None, None)
+            if intrinsics_grad:
+                g_intrinsics = tuple(
+                    g.to(dtype=t.dtype, device=t.device) if need else None for g, t, need in
+                    zip(grads[13:15], ctx.intrinsics, ctx.needs_input_grad[_RasterizeGaussians.INTRINSICS_INPUTS]))
         # order of forward's inputs; the settings tuple and the fusion flag get no gradient
         return (g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rot, g_cov3D, g_norm3D, g_extra_attrs,
-                None, None) + g_camera
+                None, None) + g_camera + g_intrinsics
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                         norm3Ds_precomp, extra_attrs, raster_settings):
     rs = raster_settings
+    # tanfovx / tanfovy may be 0-d tensors; the native layer reads them with float(), which for a CUDA tensor is a
+    # host sync each forward and backward, so keep the leaves of a focal refinement on the CPU
+    intrinsics = (rs.tanfovx, rs.tanfovy) if _requires_grad(rs.tanfovx) or _requires_grad(rs.tanfovy) else ()
     color, depth, norm, alpha, radii, extra = _RasterizeGaussians.apply(
         means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, norm3Ds_precomp,
-        extra_attrs, raster_settings, FUSE_NORMALIZE, rs.viewmatrix, rs.projmatrix, rs.campos)
+        extra_attrs, raster_settings, FUSE_NORMALIZE, rs.viewmatrix, rs.projmatrix, rs.campos, *intrinsics)
     if not FUSE_NORMALIZE:
         # the reference normalises the blended normal map in torch, inside the autograd graph (diff_gauss/__init__.py:48)
         norm = torch.nn.functional.normalize(norm, p=2, dim=0)

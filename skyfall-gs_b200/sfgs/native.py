@@ -88,7 +88,8 @@ ABI_VERSION = 4   # SFGS_VERSION of include/sfgs.h these struct mirrors were wri
 EXPORTS = [
     "sfgs_rasterize_forward", "sfgs_rasterize_backward", "sfgs_rasterize_backward_deterministic", "sfgs_mark_visible",
     "sfgs_rasterize_forward_subpixel", "sfgs_rasterize_backward_subpixel", "sfgs_rasterize_backward_deterministic_subpixel",
-    "sfgs_rasterize_backward_camera", "sfgs_geom_bytes", "sfgs_image_bytes", "sfgs_binning_bytes",
+    "sfgs_rasterize_backward_camera", "sfgs_rasterize_backward_camera_intrinsics",
+    "sfgs_geom_bytes", "sfgs_image_bytes", "sfgs_binning_bytes",
     "sfgs_geom_layout", "sfgs_image_layout", "sfgs_binning_layout", "sfgs_last_capacity",
     "sfgs_fusedssim_forward", "sfgs_fusedssim_backward", "sfgs_dist2_knn3",
     "sfgs_activations_forward", "sfgs_activations_backward",
@@ -126,6 +127,8 @@ def lib() -> C.CDLL:
     L.sfgs_rasterize_backward_deterministic_subpixel.restype = C.c_int
     L.sfgs_rasterize_backward_camera.argtypes = [C.POINTER(BackwardArgs), C.c_void_p, C.c_int, C.c_void_p]
     L.sfgs_rasterize_backward_camera.restype = C.c_int
+    L.sfgs_rasterize_backward_camera_intrinsics.argtypes = [C.POINTER(BackwardArgs), C.c_void_p, C.c_int, C.c_void_p]
+    L.sfgs_rasterize_backward_camera_intrinsics.restype = C.c_int
     L.sfgs_mark_visible.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.sfgs_mark_visible.restype = C.c_int
     L.sfgs_geom_bytes.argtypes = [C.c_int]; L.sfgs_geom_bytes.restype = C.c_size_t

@@ -201,7 +201,7 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
                                  dL_dout_extra, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer,
                                  out_alpha, debug, tile_rows=None, norm_raw=None, phase=0, acc=None,
                                  gauss_range=None, acc_peers=None, peer_slice=0, subpixel_offset=None,
-                                 camera_grad=False):
+                                 camera_grad=False, intrinsics_grad=False):
     """Same positional signature and return tuple as the reference's `_C.rasterize_gaussians_backward`.  With
     `norm_raw` (the extra tensor a `fuse_normalize=True` forward returned) `dL_dout_norm` is taken w.r.t. the unit
     normal map and the adjoint of F.normalize is applied inside the blend-adjoint kernel.
@@ -221,7 +221,14 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
 
     `camera_grad=True` (one-call backward only): the same call through sfgs_rasterize_backward_camera, which also forms
     the camera gradients; the tuple then ends with (dL_dviewmatrix [4,4], dL_dprojmatrix [4,4], dL_dcampos [3]), in the
-    layout of the inputs.  Every other output is bit-identical to the call without it."""
+    layout of the inputs.  Every other output is bit-identical to the call without it.
+
+    `camera_grad=True, intrinsics_grad=True`: the same call through sfgs_rasterize_backward_camera_intrinsics, which
+    also forms the gradients with respect to the focal lengths; the tuple then ends with the three camera tensors and
+    (dL_dtanfovx, dL_dtanfovy), 0-d tensors.  Every other output, the camera tensors included, is bit-identical to the
+    call without it."""
+    if intrinsics_grad and not camera_grad:
+        raise ValueError("intrinsics_grad=True needs camera_grad=True")
     if subpixel_offset is not None:
         check_subpixel_offset(subpixel_offset, int(dL_dout_color.shape[1]), int(dL_dout_color.shape[2]))
     F = int(extra_attrs.shape[1]) if (extra_attrs is not None and extra_attrs.numel() != 0) else 0
@@ -237,7 +244,9 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
         z = lambda *s: torch.zeros(s, **fopt)  # noqa: E731
         ret = (z(P, 3), z(P, 3), z(P, 1), z(P, 3), z(P, 6), z(P, 3), z(P, M, 3), z(P, 3), z(P, 4),
                z(P, F) if F > 0 else torch.empty(0, **fopt))
-        return ret + (z(4, 4), z(4, 4), z(3)) if camera_grad else ret
+        if camera_grad:
+            ret += (z(4, 4), z(4, 4), z(3))
+        return ret + (z(), z()) if intrinsics_grad else ret
 
     with torch.cuda.device(dev), _no_fill(deterministic):
         # one allocation for all fixed-width per-Gaussian gradients (every element is written by the kernel)
@@ -313,10 +322,10 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
         if tile_rows is not None:
             a.tile_row_begin, a.tile_row_end = _band(tile_rows)
         if camera_grad:
-            dL_dcamera = torch.empty((35,), **fopt)
+            dL_dcamera = torch.empty((37 if intrinsics_grad else 35,), **fopt)
             off = _ptr(subpixel_offset, keep) if subpixel_offset is not None else None
-            N.check(L.sfgs_rasterize_backward_camera(C.byref(a), off, int(deterministic), dL_dcamera.data_ptr()),
-                    "sfgs_rasterize_backward_camera")
+            entry = "sfgs_rasterize_backward_camera_intrinsics" if intrinsics_grad else "sfgs_rasterize_backward_camera"
+            N.check(getattr(L, entry)(C.byref(a), off, int(deterministic), dL_dcamera.data_ptr()), entry)
         elif subpixel_offset is not None:
             off = _ptr(subpixel_offset, keep)
             if deterministic:
@@ -338,6 +347,8 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
            dL_dsh, outs["scales"], outs["rot"], dL_dextra)
     if camera_grad:
         ret += (dL_dcamera[0:16].view(4, 4), dL_dcamera[16:32].view(4, 4), dL_dcamera[32:35])
+    if intrinsics_grad:
+        ret += (dL_dcamera[35], dL_dcamera[36])
     return ret
 
 
