@@ -317,6 +317,24 @@ int sfgs_appearance_forward(int P, int D, int M, const float* features, const fl
                             int E, const float* W1, const float* b1, const float* W2, const float* b2,
                             const float* W3, const float* b3, const float* means3D, const float* campos,
                             float* colors, void* stream);
+/* Backward of sfgs_appearance_forward, in float32 on the CUDA cores: recomputes the forward from the same inputs (not
+ * from its output) and writes dL/d of every input from dL_dcolors [P,3].  Outputs have the inputs' shapes
+ * (dL_dfeatures [P,M,3], dL_dgemb [P,G], dL_daemb [E], dL_dW1 [128, 3+G+E], ..., dL_dmeans3D [P,3], dL_dcampos [3]).
+ * A NULL output is not computed and skips the work only it needs; every non-NULL output is fully written (no
+ * pre-zeroing).  Subgradients at ties are torch's (clamp_max passes where x <= max, clamp_min where x >= min, ReLU
+ * where its output is > 0).  Deterministic: sums over Gaussians go through per-chunk float32 partials (chunks of
+ * max(512, 64 ceil(P/65536)) Gaussians, a function of P alone) added in float64 in a fixed order and rounded once; no
+ * atomics, so repeated calls give identical bits.  P = 0 writes zero sums.  Same argument checks as the forward, also
+ * before any CUDA work; scratch_alloc must not be NULL and is called once for
+ * sfgs_appearance_backward_scratch_bytes(P) bytes = ceil(P/C) * 20876 * 4 + 1024 (about 80 MB at P = 1M). */
+size_t sfgs_appearance_backward_scratch_bytes(int P);
+int sfgs_appearance_backward(int P, int D, int M, const float* features, const float* gemb, int G, const float* aemb,
+                             int E, const float* W1, const float* b1, const float* W2, const float* b2,
+                             const float* W3, const float* b3, const float* means3D, const float* campos,
+                             const float* dL_dcolors,
+                             float* dL_dfeatures, float* dL_dgemb, float* dL_daemb, float* dL_dW1, float* dL_db1,
+                             float* dL_dW2, float* dL_db2, float* dL_dW3, float* dL_db3, float* dL_dmeans3D,
+                             float* dL_dcampos, sfgs_alloc_fn scratch_alloc, void* scratch_user, void* stream);
 
 /* ---- 3D smoothing filter (SURVEY.md 8f rank 3) -----------------------------
  * GaussianModel.compute_3D_filter (scene/gaussian_model.py:254-308) as one pass over the Gaussians: for every Gaussian

@@ -12,11 +12,18 @@ replaces, in gaussian_renderer/__init__.py:105-118,
 for any SH width the model stores: features [P, M, 3] with M = (max_sh_degree + 1)^2 = 1, 4, 9 or 16 (the README's
 training commands use --sh_degree 1, M = 4), at any active degree D with (D + 1)^2 <= M.
 
-Forward: one wgmma tensor-core kernel (csrc/sfgs_appearance.cu, `sfgs_appearance_forward`).  Backward: not fused yet —
-the autograd function recomputes the same expression with torch ops (`reference_colors`, float32) and differentiates
-that, so gradients are those of the torch formulation.  The fused forward pays off where no backward follows
-(evaluation and video renders: render_video.py, metrics).  In a training step the recompute repeats the torch forward,
-so the step pays the fused forward on top of the torch forward and backward (DESIGN.md §7).
+Forward: one wgmma tensor-core kernel (csrc/sfgs_appearance.cu, `sfgs_appearance_forward`).
+
+Backward, two choices:
+  * default: the autograd function recomputes the same expression with torch ops (`reference_colors`, float32) and
+    differentiates that, so the gradients are the torch formulation's, rounding included.  A training step then pays
+    the fused forward on top of the torch forward and backward (DESIGN.md §7).
+  * `fused_backward=True`: one float32 CUDA-core kernel (`sfgs_appearance_backward`) recomputes the forward and forms
+    every requested gradient, deterministically (fixed-order float64 sums over Gaussians, no atomics).  Its gradients
+    are float32-accurate — their error against float64 is at most 3.4x torch float32's own (measured, H100) — but they
+    are not torch's bits: on
+    a trained MLP (a multiplier head with h ~ 100 before the x0.01) the two float32 evaluations differ by up to ~15x
+    rtol = 1e-5 / atol = 1e-7 in dL/dW2, because torch float32 itself misses float64 by that much (DESIGN.md §7).
 """
 from __future__ import annotations
 
@@ -84,10 +91,53 @@ def _fwd(features, gemb, aemb, W1, b1, W2, b2, W3, b3, xyz, campos, deg):
     return out
 
 
+def _bwd(saved, deg, g, needs):
+    """Gradients of the 11 inputs from the fused float32 kernel; None where `needs` is False (and for xyz and campos at
+    degree 0, which do not reach the colours)."""
+    L = N.lib()
+    features = saved[0]
+    P, dev = int(features.shape[0]), features.device
+    needs = list(needs)
+    if deg == 0:
+        needs[9] = needs[10] = False
+    t = [x.detach().contiguous().float() for x in saved] + [g.contiguous().float()]
+    t = [x.clone() if x.data_ptr() % 16 else x for x in t]
+    outs = [torch.empty(s.shape, dtype=torch.float32, device=dev) if n else None for s, n in zip(saved, needs)]
+    ptr = [o.data_ptr() if o is not None else None for o in outs]
+    f, ge, a, w1, bb1, w2, bb2, w3, bb3, xz, cp, gc = t
+    arena = _Arena(dev)
+    with torch.cuda.device(dev):
+        N.check(L.sfgs_appearance_backward(P, int(deg), int(f.shape[1]), f.data_ptr(), ge.data_ptr(), int(ge.shape[1]),
+                                           a.data_ptr(), int(a.numel()), w1.data_ptr(), bb1.data_ptr(), w2.data_ptr(),
+                                           bb2.data_ptr(), w3.data_ptr(), bb3.data_ptr(), xz.data_ptr(), cp.data_ptr(),
+                                           gc.data_ptr(), *ptr, arena.cb, None,
+                                           torch.cuda.current_stream(dev).cuda_stream),
+                "sfgs_appearance_backward")
+    arena.tensor = None
+    return [o.to(s.dtype) if o is not None else None for o, s in zip(outs, saved)]
+
+
+class _Arena:
+    """Scratch for the backward's allocator callback: the tensor lives until the call has been queued."""
+
+    def __init__(self, device):
+        self.device = device
+        self.tensor = None
+        self.cb = N.ALLOC_FN(self._alloc)
+
+    def _alloc(self, _user, nbytes):
+        try:
+            self.tensor = torch.empty(int(nbytes), dtype=torch.uint8, device=self.device)
+            return self.tensor.data_ptr()
+        except Exception:  # noqa: BLE001 - must not raise through the C ABI
+            return None
+
+
 class _Appearance(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, features, gemb, aemb, W1, b1, W2, b2, W3, b3, xyz, campos, deg):
+    def forward(ctx, features, gemb, aemb, W1, b1, W2, b2, W3, b3, xyz, campos, deg, fused_backward=False):
         ctx.deg = int(deg)
+        ctx.fused_backward = bool(fused_backward)
         ctx.save_for_backward(features, gemb, aemb, W1, b1, W2, b2, W3, b3, xyz, campos)
         return _fwd(features, gemb, aemb, W1, b1, W2, b2, W3, b3, xyz, campos, deg)
 
@@ -95,21 +145,25 @@ class _Appearance(torch.autograd.Function):
     def backward(ctx, g):
         saved = ctx.saved_tensors
         needs = ctx.needs_input_grad[:11]
+        if ctx.fused_backward:
+            return tuple(_bwd(saved, ctx.deg, g, needs)) + (None, None)
         with torch.enable_grad():
             leaves = [s.detach().requires_grad_(n) for s, n in zip(saved, needs)]
             out = reference_colors(*leaves, ctx.deg)
             grads = torch.autograd.grad(out, [l for l, n in zip(leaves, needs) if n], g, allow_unused=True)
         it = iter(grads)
-        return tuple(next(it) if n else None for n in needs) + (None,)
+        return tuple(next(it) if n else None for n in needs) + (None, None)
 
 
-def fused_appearance_colors(features, gemb, aemb, mlp, xyz, campos, active_sh_degree):
+def fused_appearance_colors(features, gemb, aemb, mlp, xyz, campos, active_sh_degree, *, fused_backward=False):
     """features [P,M,3] (pc.get_features, M = (pc.max_sh_degree + 1)^2 = 1, 4, 9 or 16), gemb [P,24]
     (pc._embeddings), aemb [32] (the camera's appearance embedding), mlp = pc.appearance_mlp.mlp (nn.Sequential
     Linear-ReLU-Linear-ReLU-Linear) or its six tensors; active_sh_degree D needs (D + 1)^2 <= M.  Another M, or a D
-    the width cannot hold, raises native.SfgsError."""
+    the width cannot hold, raises native.SfgsError.  fused_backward=True differentiates with the fused float32
+    kernel instead of the torch recompute (see the module docstring)."""
     if isinstance(mlp, (tuple, list)):
         W1, b1, W2, b2, W3, b3 = mlp
     else:
         W1, b1, W2, b2, W3, b3 = mlp[0].weight, mlp[0].bias, mlp[2].weight, mlp[2].bias, mlp[4].weight, mlp[4].bias
-    return _Appearance.apply(features, gemb, aemb, W1, b1, W2, b2, W3, b3, xyz, campos, active_sh_degree)
+    return _Appearance.apply(features, gemb, aemb, W1, b1, W2, b2, W3, b3, xyz, campos, active_sh_degree,
+                             fused_backward)

@@ -94,7 +94,8 @@ EXPORTS = [
     "sfgs_fusedssim_forward", "sfgs_fusedssim_backward", "sfgs_dist2_knn3",
     "sfgs_activations_forward", "sfgs_activations_backward",
     "sfgs_last_error", "sfgs_version", "sfgs_launch_count", "sfgs_profile_enable", "sfgs_profile_read", "sfgs_sizeof", "sfgs_sm_clock_probe",
-    "sfgs_selftest_expf", "sfgs_overflow_reruns", "sfgs_appearance_forward", "sfgs_compute_3d_filter",
+    "sfgs_selftest_expf", "sfgs_overflow_reruns", "sfgs_appearance_forward", "sfgs_appearance_backward",
+    "sfgs_appearance_backward_scratch_bytes", "sfgs_compute_3d_filter",
     "sfgs_densification_stats", "sfgs_densify_plan_blocks", "sfgs_densify_plan", "sfgs_densify_apply",
 ]
 STAGE_NAMES = ["fwd_zero", "preprocess", "tile_scan", "emit_keys", "tile_sort", "render_fwd", "bwd_zero", "render_bwd",
@@ -160,6 +161,11 @@ def lib() -> C.CDLL:
     L.sfgs_sm_clock_probe.argtypes = [C.c_void_p, C.c_void_p]; L.sfgs_sm_clock_probe.restype = C.c_int
     L.sfgs_appearance_forward.argtypes = [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int] + [C.c_void_p] * 10
     L.sfgs_appearance_forward.restype = C.c_int
+    L.sfgs_appearance_backward.argtypes = ([C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
+                                           + [C.c_void_p] * 20 + [ALLOC_FN, C.c_void_p, C.c_void_p])
+    L.sfgs_appearance_backward.restype = C.c_int
+    L.sfgs_appearance_backward_scratch_bytes.argtypes = [C.c_int]
+    L.sfgs_appearance_backward_scratch_bytes.restype = C.c_size_t
     L.sfgs_compute_3d_filter.argtypes = [C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]
     L.sfgs_compute_3d_filter.restype = C.c_int
     L.sfgs_densification_stats.argtypes = [C.c_int] + [C.c_void_p] * 8
