@@ -214,10 +214,22 @@ int sfgs_rasterize_backward_deterministic(const sfgs_backward_args* a);
  *   - Any finite offset is allowed; a NaN or Inf offset makes the forward return SFGS_E_BADARG.
  *   - No gradient is formed with respect to the offsets.
  *   - The backward must get the same buffer, with the same contents, as the forward (like norm_raw).
- *   - ED > 0 (extra_attrs), out_peers and acc_peers return SFGS_E_UNSUPPORTED before any CUDA work. */
+ *   - A tile-row band takes offsets: the reach masks are dilated by the bound over the WHOLE frame's offsets, so a
+ *     band's lists and masks are those of the one-call frame and the bands reassemble its images bit for bit.
+ *   - ED > 0 (extra_attrs), out_peers and acc_peers return SFGS_E_UNSUPPORTED before any CUDA work; the fused peer
+ *     exchanges take offsets through the _subpixel_peers entries below. */
 int sfgs_rasterize_forward_subpixel(const sfgs_forward_args* a, const float* subpixel_offset);
 int sfgs_rasterize_backward_subpixel(const sfgs_backward_args* a, const float* subpixel_offset);
 int sfgs_rasterize_backward_deterministic_subpixel(const sfgs_backward_args* a, const float* subpixel_offset);
+
+/* ---- subpixel offsets with the fused exchanges of the tile-row sharded mode ----------------------------------------
+ * sfgs_rasterize_forward_subpixel and sfgs_rasterize_backward_subpixel that also accept out_peers (the image
+ * all-gather fused into the band forward) and acc_peers (the reduce-scatter fused into phase 1 of the backward);
+ * everything else, validation included, is theirs.  Every rank passes the whole frame's offsets.  ED > 0
+ * (extra_attrs) returns SFGS_E_UNSUPPORTED before any CUDA work.  The deterministic backward has no acc_peers form
+ * (sfgs_rasterize_backward_deterministic_subpixel keeps rejecting them). */
+int sfgs_rasterize_forward_subpixel_peers(const sfgs_forward_args* a, const float* subpixel_offset);
+int sfgs_rasterize_backward_subpixel_peers(const sfgs_backward_args* a, const float* subpixel_offset);
 
 /* ---- camera gradients (pose refinement: Camera(..., optimizing=True) of scene/cameras.py) -------------------------
  * The backward above that also writes dL_dcamera, a DEVICE [35] float array: dL/dviewmatrix[16], dL/dprojmatrix[16],
@@ -236,7 +248,8 @@ int sfgs_rasterize_backward_deterministic_subpixel(const sfgs_backward_args* a, 
  *   - scratch_alloc is required; the extra scratch is 35 * 8 * ceil(P / 96) bytes (+ alignment) on top of what the
  *     backward it follows needs.
  *   - Phase 0 only: phases 1 and 2 and acc_peers return SFGS_E_UNSUPPORTED, a NULL dL_dcamera SFGS_E_BADARG, before
- *     any CUDA work.
+ *     any CUDA work.  The two-phase (tile-row sharded) backward forms its camera gradients with
+ *     sfgs_rasterize_backward_camera_partial.
  * No gradient is formed for tan_fovx / tan_fovy (see sfgs_rasterize_backward_camera_intrinsics) or the subpixel
  * offsets. */
 int sfgs_rasterize_backward_camera(const sfgs_backward_args* a, const float* subpixel_offset, int deterministic,
@@ -254,6 +267,23 @@ int sfgs_rasterize_backward_camera(const sfgs_backward_args* a, const float* sub
  *     37 * 8 * ceil(P / 96) bytes (+ alignment). */
 int sfgs_rasterize_backward_camera_intrinsics(const sfgs_backward_args* a, const float* subpixel_offset,
                                               int deterministic, float* dL_dcamera);
+
+/* ---- camera partials of a Gaussian slice (camera gradients of the tile-row sharded backward) --------------------
+ * Phase 2 of the backward (the per-Gaussian adjoint of Gaussians [gauss_begin, gauss_end)) that also writes
+ * dL_dcamera_partial, a DEVICE [ncam] float64 array: the slice's camera terms in the layout above (ncam = 35: pose;
+ * ncam = 37: pose and focal), summed in float64 and NOT rounded.  The ranks of a sharded frame add their slices'
+ * partials and round once (sfgs/multigpu.py reduce_camera_gradients), so the frame's gradients are rounded once, as
+ * the one-call entries round them; they differ from those only by the grouping of the float64 sums.
+ *   - The slice's span partials (96 Gaussians each, counted from gauss_begin) are added in an order fixed by the slice
+ *     length alone, so with bit-reproducible `acc` the partials are bit-reproducible.  deterministic has no effect on
+ *     phase 2 (it has no reductions) and is accepted for symmetry with the other camera entries.
+ *   - Every gradient row [gauss_begin, gauss_end) is bit-identical to the same phase-2 call without camera terms.
+ *   - An empty slice (and P == 0) writes zeros.
+ *   - scratch_alloc is required; the scratch is ncam * 8 * ceil((gauss_end - gauss_begin) / 96) bytes (+ alignment).
+ *   - Before any CUDA work: a NULL args or dL_dcamera_partial, ncam other than 35 or 37, or a NULL scratch_alloc
+ *     return SFGS_E_BADARG; phase 0 or 1 and ED > 0 (extra_attrs) return SFGS_E_UNSUPPORTED. */
+int sfgs_rasterize_backward_camera_partial(const sfgs_backward_args* a, const float* subpixel_offset,
+                                           int deterministic, int ncam, double* dL_dcamera_partial);
 
 /* ---- markVisible --------------------------------------------------------- */
 int sfgs_mark_visible(int P, const float* means3D, const float* viewmatrix,

@@ -57,6 +57,7 @@ void sfgs_launch_gauss_bwd(const sfgs_backward_args* a, const GeomLayout& g, flo
                            cudaStream_t st);
 size_t sfgs_camera_scratch_bytes(int P, int ncam);
 void sfgs_launch_camera_reduce(int P, int ncam, const double* cam_part, float* dL_dcamera, cudaStream_t st);
+void sfgs_launch_camera_partial_reduce(int n, int ncam, const double* cam_part, double* dL_dcamera, cudaStream_t st);
 void sfgs_launch_acc_clear_visible(int P, const int* radii, float* acc, cudaStream_t st);
 
 namespace {
@@ -196,17 +197,21 @@ thread_local PinnedHdr t_hdr_dev[MAX_DEVICES];
 
 int rasterize_forward(const sfgs_forward_args* a, const float* off);
 int rasterize_backward(const sfgs_backward_args* a, bool deterministic, const float* off, float* dL_dcamera,
-                       int ncam);
+                       double* dL_dcamera_partial, int ncam);
 
-// the combinations the subpixel-offset entry points have no kernels for (checked before any CUDA work)
-int subpixel_unsupported_fwd(const sfgs_forward_args* a) {
+// the combinations the subpixel-offset entry points reject (checked before any CUDA work): extra_attrs, which have no
+// kernels with offsets, and -- unless the entry is a _subpixel_peers one -- the fused peer exchanges, which the
+// _subpixel entries have always rejected
+int subpixel_unsupported_fwd(const sfgs_forward_args* a, bool peers_ok) {
   if (a->ED > 0) return fail(SFGS_E_UNSUPPORTED, "forward_subpixel: extra_attrs are not supported with subpixel offsets");
-  if (a->out_peers != nullptr) return fail(SFGS_E_UNSUPPORTED, "forward_subpixel: out_peers are not supported with subpixel offsets");
+  if (!peers_ok && a->out_peers != nullptr)
+    return fail(SFGS_E_UNSUPPORTED, "forward_subpixel: out_peers are not supported by this entry; use sfgs_rasterize_forward_subpixel_peers");
   return SFGS_OK;
 }
-int subpixel_unsupported_bwd(const sfgs_backward_args* a) {
+int subpixel_unsupported_bwd(const sfgs_backward_args* a, bool peers_ok) {
   if (a->ED > 0) return fail(SFGS_E_UNSUPPORTED, "backward_subpixel: extra_attrs are not supported with subpixel offsets");
-  if (a->acc_peers != nullptr) return fail(SFGS_E_UNSUPPORTED, "backward_subpixel: acc_peers are not supported with subpixel offsets");
+  if (!peers_ok && a->acc_peers != nullptr)
+    return fail(SFGS_E_UNSUPPORTED, "backward_subpixel: acc_peers are not supported by this entry; use sfgs_rasterize_backward_subpixel_peers");
   return SFGS_OK;
 }
 
@@ -225,8 +230,22 @@ int backward_camera(const char* name, const sfgs_backward_args* a, const float* 
   if (a->acc_peers != nullptr)
     return reject(SFGS_E_UNSUPPORTED, "acc_peers (the multi-GPU backward) have no camera gradients");
   if (!a->scratch_alloc) return reject(SFGS_E_BADARG, "null scratch allocator");
-  if (off != nullptr && subpixel_unsupported_bwd(a)) return SFGS_E_UNSUPPORTED;
-  return rasterize_backward(a, deterministic != 0, off, dL_dcamera, ncam);
+  if (off != nullptr && subpixel_unsupported_bwd(a, false)) return SFGS_E_UNSUPPORTED;
+  return rasterize_backward(a, deterministic != 0, off, dL_dcamera, nullptr, ncam);
+}
+
+// the phase-2 camera partials of a Gaussian slice (the tile-row sharded backward); the checks come before any CUDA work
+int backward_camera_partial(const sfgs_backward_args* a, const float* off, int deterministic, int ncam,
+                            double* dL_dcamera_partial) {
+  if (!a) return fail(SFGS_E_BADARG, "backward_camera_partial: null args");
+  if (!dL_dcamera_partial) return fail(SFGS_E_BADARG, "backward_camera_partial: null dL_dcamera_partial");
+  if (ncam != 35 && ncam != 37) return fail(SFGS_E_BADARG, "backward_camera_partial: ncam must be 35 or 37");
+  if (a->phase != 2)
+    return fail(SFGS_E_UNSUPPORTED, "backward_camera_partial: camera partials are formed by phase 2 only");
+  if (!a->scratch_alloc) return fail(SFGS_E_BADARG, "backward_camera_partial: null scratch allocator");
+  if (a->ED > 0)
+    return fail(SFGS_E_UNSUPPORTED, "backward_camera_partial: extra_attrs are not supported by the two-phase backward");
+  return rasterize_backward(a, deterministic != 0, off, nullptr, dL_dcamera_partial, ncam);
 }
 
 }  // namespace
@@ -266,23 +285,33 @@ int sfgs_binning_layout(char* base, long long capacity, sfgs_binning_view* out) 
 }
 
 int sfgs_rasterize_forward(const sfgs_forward_args* a) { return rasterize_forward(a, nullptr); }
-int sfgs_rasterize_backward(const sfgs_backward_args* a) { return rasterize_backward(a, false, nullptr, nullptr, 0); }
-int sfgs_rasterize_backward_deterministic(const sfgs_backward_args* a) { return rasterize_backward(a, true, nullptr, nullptr, 0); }
+int sfgs_rasterize_backward(const sfgs_backward_args* a) { return rasterize_backward(a, false, nullptr, nullptr, nullptr, 0); }
+int sfgs_rasterize_backward_deterministic(const sfgs_backward_args* a) { return rasterize_backward(a, true, nullptr, nullptr, nullptr, 0); }
 
 int sfgs_rasterize_forward_subpixel(const sfgs_forward_args* a, const float* subpixel_offset) {
   if (!a) return fail(SFGS_E_BADARG, "forward: null args");
-  if (subpixel_offset != nullptr && subpixel_unsupported_fwd(a)) return SFGS_E_UNSUPPORTED;
+  if (subpixel_offset != nullptr && subpixel_unsupported_fwd(a, false)) return SFGS_E_UNSUPPORTED;
+  return rasterize_forward(a, subpixel_offset);
+}
+int sfgs_rasterize_forward_subpixel_peers(const sfgs_forward_args* a, const float* subpixel_offset) {
+  if (!a) return fail(SFGS_E_BADARG, "forward: null args");
+  if (subpixel_offset != nullptr && subpixel_unsupported_fwd(a, true)) return SFGS_E_UNSUPPORTED;
   return rasterize_forward(a, subpixel_offset);
 }
 int sfgs_rasterize_backward_subpixel(const sfgs_backward_args* a, const float* subpixel_offset) {
   if (!a) return fail(SFGS_E_BADARG, "backward: null args");
-  if (subpixel_offset != nullptr && subpixel_unsupported_bwd(a)) return SFGS_E_UNSUPPORTED;
-  return rasterize_backward(a, false, subpixel_offset, nullptr, 0);
+  if (subpixel_offset != nullptr && subpixel_unsupported_bwd(a, false)) return SFGS_E_UNSUPPORTED;
+  return rasterize_backward(a, false, subpixel_offset, nullptr, nullptr, 0);
+}
+int sfgs_rasterize_backward_subpixel_peers(const sfgs_backward_args* a, const float* subpixel_offset) {
+  if (!a) return fail(SFGS_E_BADARG, "backward: null args");
+  if (subpixel_offset != nullptr && subpixel_unsupported_bwd(a, true)) return SFGS_E_UNSUPPORTED;
+  return rasterize_backward(a, false, subpixel_offset, nullptr, nullptr, 0);
 }
 int sfgs_rasterize_backward_deterministic_subpixel(const sfgs_backward_args* a, const float* subpixel_offset) {
   if (!a) return fail(SFGS_E_BADARG, "backward: null args");
-  if (subpixel_offset != nullptr && subpixel_unsupported_bwd(a)) return SFGS_E_UNSUPPORTED;
-  return rasterize_backward(a, true, subpixel_offset, nullptr, 0);
+  if (subpixel_offset != nullptr && subpixel_unsupported_bwd(a, false)) return SFGS_E_UNSUPPORTED;
+  return rasterize_backward(a, true, subpixel_offset, nullptr, nullptr, 0);
 }
 
 int sfgs_rasterize_backward_camera(const sfgs_backward_args* a, const float* subpixel_offset, int deterministic,
@@ -293,6 +322,11 @@ int sfgs_rasterize_backward_camera(const sfgs_backward_args* a, const float* sub
 int sfgs_rasterize_backward_camera_intrinsics(const sfgs_backward_args* a, const float* subpixel_offset,
                                               int deterministic, float* dL_dcamera) {
   return backward_camera("backward_camera_intrinsics", a, subpixel_offset, deterministic, dL_dcamera, 37);
+}
+
+int sfgs_rasterize_backward_camera_partial(const sfgs_backward_args* a, const float* subpixel_offset, int deterministic,
+                                           int ncam, double* dL_dcamera_partial) {
+  return backward_camera_partial(a, subpixel_offset, deterministic, ncam, dL_dcamera_partial);
 }
 
 }  // extern "C"
@@ -409,19 +443,22 @@ int rasterize_forward(const sfgs_forward_args* a, const float* off) {
   return (int)R;
 }
 
-// dL_dcamera: NULL, or (phase 0 only, checked by the caller) the DEVICE [ncam] camera gradients to form as well:
-// ncam = 35 (pose terms) or 37 (pose and focal terms)
+// dL_dcamera: NULL, or (phase 0 only, checked by the caller) the DEVICE [ncam] camera gradients to form as well;
+// dL_dcamera_partial: NULL, or (phase 2 only, checked by the caller) the DEVICE [ncam] float64 camera sums of the
+// Gaussian slice, unrounded.  ncam = 35 (pose terms) or 37 (pose and focal terms)
 int rasterize_backward(const sfgs_backward_args* a, bool deterministic, const float* off, float* dL_dcamera,
-                       int ncam) {
+                       double* dL_dcamera_partial, int ncam) {
   if (!a) return fail(SFGS_E_BADARG, "backward: null args");
   if (a->P < 0 || a->width <= 0 || a->height <= 0) return fail(SFGS_E_BADARG, "backward: bad sizes");
   if (deterministic && a->acc_peers != nullptr)
     return fail(SFGS_E_UNSUPPORTED, "backward_deterministic: acc_peers (system-scope reductions) have no deterministic implementation");
   if (deterministic && a->ED > 0)
     return fail(SFGS_E_UNSUPPORTED, "backward_deterministic: extra_attrs have no deterministic implementation");
-  const bool cam = dL_dcamera != nullptr;
+  const bool cam = dL_dcamera != nullptr || dL_dcamera_partial != nullptr;
   if (a->P == 0) {
-    if (cam) CU(cudaMemsetAsync(dL_dcamera, 0, (size_t)ncam * sizeof(float), (cudaStream_t)a->stream));
+    if (dL_dcamera) CU(cudaMemsetAsync(dL_dcamera, 0, (size_t)ncam * sizeof(float), (cudaStream_t)a->stream));
+    if (dL_dcamera_partial)
+      CU(cudaMemsetAsync(dL_dcamera_partial, 0, (size_t)ncam * sizeof(double), (cudaStream_t)a->stream));
     return SFGS_OK;
   }
   const int phase = a->phase;
@@ -478,7 +515,7 @@ int rasterize_backward(const sfgs_backward_args* a, bool deterministic, const fl
   if ((!acc && !peer) || ordered || cam) {
     const size_t acc_bytes = !acc ? sfgs_align_up((size_t)P * 16 * sizeof(float)) : 0;
     const size_t order_bytes = ordered ? sfgs_order_scratch_bytes(P, R) : 0;
-    const size_t abytes = acc_bytes + order_bytes + (cam ? sfgs_camera_scratch_bytes(P, ncam) : 0) + SFGS_ALIGN;
+    const size_t abytes = acc_bytes + order_bytes + (cam ? sfgs_camera_scratch_bytes(g_end - g_begin, ncam) : 0) + SFGS_ALIGN;
     char* aptr = a->scratch_alloc(a->scratch_user, abytes);
     if (!aptr) return fail(SFGS_E_ALLOC, "backward: scratch allocator returned NULL");
     char* base = sfgs_align_ptr(aptr);
@@ -525,7 +562,9 @@ int rasterize_backward(const sfgs_backward_args* a, bool deterministic, const fl
   if (do_gauss) {
     PROF_BEGIN(ST_GAUSS_BWD);
     sfgs_launch_gauss_bwd(a, g, focal_x, focal_y, acc, g_begin, g_end, phase == 2 ? g_begin : 0, cam_part, ncam, st);
-    if (cam) sfgs_launch_camera_reduce(P, ncam, cam_part, dL_dcamera, st);
+    if (dL_dcamera) sfgs_launch_camera_reduce(P, ncam, cam_part, dL_dcamera, st);
+    // an empty slice has no spans: the reduction writes zeros
+    if (dL_dcamera_partial) sfgs_launch_camera_partial_reduce(g_end - g_begin, ncam, cam_part, dL_dcamera_partial, st);
     PROF_END();
     STAGE_CHECK("gauss_bwd");
   }

@@ -743,8 +743,8 @@ gauss_bwd_intrinsics_kernel(GB_PARAMS, double* __restrict__ cam_part) {
 // dL_dcamera[j] = the sum of the spans' partials of term j, rounded to float once.  The order depends on nspans only:
 // thread i adds spans i, i + CR_THREADS, ... in turn, then a fixed tree adds the threads' sums.
 constexpr int CR_THREADS = 256;
-__global__ void __launch_bounds__(CR_THREADS)
-camera_reduce_kernel(int nspans, const double* __restrict__ cam_part, float* __restrict__ dL_dcamera) {
+// the sum of term blockIdx.x over the spans, in that order, valid in thread 0
+__device__ __forceinline__ double camera_span_sum(int nspans, const double* __restrict__ cam_part) {
   __shared__ double s[CR_THREADS];
   const int j = blockIdx.x, t = threadIdx.x;
   const double* p = cam_part + (size_t)j * nspans;
@@ -757,7 +757,23 @@ camera_reduce_kernel(int nspans, const double* __restrict__ cam_part, float* __r
     if (t < w) s[t] += s[t + w];
     __syncthreads();
   }
-  if (t == 0) dL_dcamera[j] = (float)s[0];
+  return s[0];
+}
+
+__global__ void __launch_bounds__(CR_THREADS)
+camera_reduce_kernel(int nspans, const double* __restrict__ cam_part, float* __restrict__ dL_dcamera) {
+  const int j = blockIdx.x, t = threadIdx.x;
+  const double s = camera_span_sum(nspans, cam_part);
+  if (t == 0) dL_dcamera[j] = (float)s;
+}
+
+// The same sum over the spans of a phase-2 Gaussian slice, left unrounded: the ranks of a sharded frame add their
+// slices' float64 partials and round once.
+__global__ void __launch_bounds__(CR_THREADS)
+camera_partial_reduce_kernel(int nspans, const double* __restrict__ cam_part, double* __restrict__ dL_dcamera) {
+  const int j = blockIdx.x, t = threadIdx.x;
+  const double s = camera_span_sum(nspans, cam_part);
+  if (t == 0) dL_dcamera[j] = s;
 }
 
 }  // namespace
@@ -788,6 +804,12 @@ size_t sfgs_camera_scratch_bytes(int P, int ncam) {
 void sfgs_launch_camera_reduce(int P, int ncam, const double* cam_part, float* dL_dcamera, cudaStream_t st) {
   SFGS_COUNT_LAUNCH();
   camera_reduce_kernel<<<ncam, CR_THREADS, 0, st>>>((P + GB_SPAN - 1) / GB_SPAN, cam_part, dL_dcamera);
+}
+
+// n: the length of the Gaussian slice whose span partials cam_part holds (the order of the sum depends on it alone)
+void sfgs_launch_camera_partial_reduce(int n, int ncam, const double* cam_part, double* dL_dcamera, cudaStream_t st) {
+  SFGS_COUNT_LAUNCH();
+  camera_partial_reduce_kernel<<<ncam, CR_THREADS, 0, st>>>((n + GB_SPAN - 1) / GB_SPAN, cam_part, dL_dcamera);
 }
 
 // cam_part: NULL for the adjoint alone; else [ncam][spans] doubles (sfgs_camera_scratch_bytes) that receive every

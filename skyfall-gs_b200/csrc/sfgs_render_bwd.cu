@@ -386,8 +386,8 @@ render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict_
                                                    dL_dextras, ED, part, written, nullptr);
 }
 
-// subpixel offsets: device-scope reductions (ORDERED = false) or the deterministic partial rows; no extra_attrs, no
-// peers (the _subpixel entry points reject both)
+// subpixel offsets: device-scope reductions (ORDERED = false) or the deterministic partial rows; no extra_attrs (the
+// _subpixel entry points reject them)
 template <bool ORDERED>
 __global__ void __launch_bounds__(BLEND_THREADS, 3)
 render_bwd_jitter_kernel(const uint2* __restrict__ ranges, const char* __restrict__ binning_base,
@@ -404,6 +404,23 @@ render_bwd_jitter_kernel(const uint2* __restrict__ ranges, const char* __restric
                                                0, part, written, off);
 }
 
+// subpixel offsets with the reduce-scatter of the tile-row sharded mode fused in: system-scope reductions into the
+// peers' accumulator slices (a kernel of its own, so that the kernels above keep their code)
+__global__ void __launch_bounds__(BLEND_THREADS, 3)
+render_bwd_jitter_peer_kernel(const uint2* __restrict__ ranges, const char* __restrict__ binning_base,
+                              const uint32_t* __restrict__ hdr, int W, int H, int band0,
+                              const float* __restrict__ bg_color, const float* __restrict__ rec,
+                              const float* __restrict__ accum_alphas, const uint32_t* __restrict__ n_contrib,
+                              const float* __restrict__ dL_dpixels, const float* __restrict__ dL_dpixel_depths,
+                              const float* __restrict__ dL_dpixel_norms, const float* __restrict__ dL_dpixel_alphas,
+                              const float* __restrict__ norm_raw, const PeerTable peers,
+                              const float2* __restrict__ off) {
+  render_bwd_warp<true, false, false, true>(ranges, binning_base, hdr, W, H, band0, bg_color, rec, accum_alphas,
+                                            n_contrib, dL_dpixels, dL_dpixel_depths, dL_dpixel_norms,
+                                            dL_dpixel_alphas, norm_raw, nullptr, peers, nullptr, nullptr, nullptr, 0,
+                                            nullptr, nullptr, off);
+}
+
 }  // namespace
 
 void sfgs_launch_render_bwd(const sfgs_backward_args* a, const GeomLayout& g, const ImageLayout& im,
@@ -412,15 +429,30 @@ void sfgs_launch_render_bwd(const sfgs_backward_args* a, const GeomLayout& g, co
   dim3 grid;
   int band0;
   if (!blend_grid(a->tile_row_begin, a->tile_row_end, im, grid, band0)) return;
+  PeerTable pt = {};
+  const bool peer = a->acc_peers != nullptr && a->n_peers > 0;
+  if (peer) {
+    for (int r = 0; r < a->n_peers && r < 8; r++) pt.p[r] = a->acc_peers[r];
+    pt.per = a->peer_slice;
+  }
   if (off != nullptr) {
     const size_t smem_j = sizeof(WarpSmemJitter) * BLEND_WARPS;
     static SfgsPerDeviceOnce attr_once_j;
     if (attr_once_j.first_use()) {
       cudaFuncSetAttribute(render_bwd_jitter_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_j);
       cudaFuncSetAttribute(render_bwd_jitter_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_j);
+      cudaFuncSetAttribute(render_bwd_jitter_peer_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_j);
+    }
+    SFGS_COUNT_LAUNCH();
+    // peer reductions belong to the non-deterministic phase 1 (the deterministic entries reject acc_peers)
+    if (peer) {
+      render_bwd_jitter_peer_kernel<<<grid, BLEND_THREADS, smem_j, st>>>(
+          im.ranges, (const char*)b.point_list, im.hdr, a->width, a->height, band0, a->background, g.rec,
+          a->accum_alphas, im.n_contrib, a->dL_dpix, a->dL_dpix_depth, a->dL_dpix_norm, a->dL_dpix_alpha, a->norm_raw,
+          pt, reinterpret_cast<const float2*>(off));
+      return;
     }
     const auto kernel = part != nullptr ? render_bwd_jitter_kernel<true> : render_bwd_jitter_kernel<false>;
-    SFGS_COUNT_LAUNCH();
     kernel<<<grid, BLEND_THREADS, smem_j, st>>>(im.ranges, (const char*)b.point_list, im.hdr, a->width, a->height, band0,
                                                 a->background, g.rec, a->accum_alphas, im.n_contrib, a->dL_dpix,
                                                 a->dL_dpix_depth, a->dL_dpix_norm, a->dL_dpix_alpha, a->norm_raw, acc,
@@ -434,12 +466,6 @@ void sfgs_launch_render_bwd(const sfgs_backward_args* a, const GeomLayout& g, co
     cudaFuncSetAttribute(render_bwd_warp_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     cudaFuncSetAttribute(render_bwd_warp_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     cudaFuncSetAttribute(render_bwd_warp_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  }
-  PeerTable pt = {};
-  const bool peer = a->acc_peers != nullptr && a->n_peers > 0;
-  if (peer) {
-    for (int r = 0; r < a->n_peers && r < 8; r++) pt.p[r] = a->acc_peers[r];
-    pt.per = a->peer_slice;
   }
   // peer reductions belong to the two-phase backward, which rejects extra_attrs (sfgs_rasterize_backward); the
   // ordered path (part != nullptr) rejects both (sfgs_rasterize_backward_deterministic)

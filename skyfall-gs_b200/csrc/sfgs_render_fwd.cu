@@ -158,7 +158,7 @@ render_fwd_warp_kernel(const uint2* __restrict__ ranges, const uint32_t* __restr
                                     out_norm, out_norm_raw, out_alpha, n_contrib, peers, extras, ED, out_extra, nullptr);
 }
 
-// subpixel offsets: local outputs only, no extra_attrs (sfgs_rasterize_forward_subpixel rejects both)
+// subpixel offsets into local outputs; no extra_attrs (sfgs_rasterize_forward_subpixel rejects them)
 __global__ void __launch_bounds__(BLEND_THREADS)
 render_fwd_jitter_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list,
                          const unsigned char* __restrict__ inst_mask, const uint32_t* __restrict__ hdr, int W, int H,
@@ -168,6 +168,18 @@ render_fwd_jitter_kernel(const uint2* __restrict__ ranges, const uint32_t* __res
                          uint32_t* __restrict__ n_contrib, const float2* __restrict__ off) {
   render_fwd_warp<false, true>(ranges, point_list, inst_mask, hdr, W, H, band0, rec, bg_color, out_color, out_depth,
                                out_norm, out_norm_raw, out_alpha, n_contrib, OutPeers{}, nullptr, 0, nullptr, off);
+}
+
+// subpixel offsets with the fused image all-gather of the tile-row sharded mode: the band goes to every rank's
+// [8,H,W] frame block (a kernel of its own, so that the local-output kernel above keeps its code)
+__global__ void __launch_bounds__(BLEND_THREADS)
+render_fwd_jitter_peers_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list,
+                               const unsigned char* __restrict__ inst_mask, const uint32_t* __restrict__ hdr, int W,
+                               int H, int band0, const float* __restrict__ rec, const float* __restrict__ bg_color,
+                               float* __restrict__ out_norm_raw, uint32_t* __restrict__ n_contrib,
+                               const OutPeers peers, const float2* __restrict__ off) {
+  render_fwd_warp<false, true>(ranges, point_list, inst_mask, hdr, W, H, band0, rec, bg_color, nullptr, nullptr,
+                               nullptr, out_norm_raw, nullptr, n_contrib, peers, nullptr, 0, nullptr, off);
 }
 
 // max |off_x|, max |off_y| over the frame into HDR_OFF_EX / HDR_OFF_EY (non-negative floats order as their bits), and
@@ -210,6 +222,17 @@ void sfgs_launch_render_fwd(const sfgs_forward_args* a, const GeomLayout& g, con
   dim3 grid;
   int band0;
   if (!blend_grid(a->tile_row_begin, a->tile_row_end, im, grid, band0)) return;
+  OutPeers op = {};
+  if (a->out_peers != nullptr && a->n_out_peers > 0)
+    for (op.n = 0; op.n < a->n_out_peers && op.n < 8; op.n++) op.p[op.n] = a->out_peers[op.n];
+  if (off != nullptr && op.n > 0) {
+    SFGS_COUNT_LAUNCH();
+    render_fwd_jitter_peers_kernel<<<grid, BLEND_THREADS, 0, st>>>(im.ranges, b.point_list, b.inst_mask, im.hdr,
+                                                                   a->width, a->height, band0, g.rec, a->background,
+                                                                   a->out_norm_raw, im.n_contrib, op,
+                                                                   reinterpret_cast<const float2*>(off));
+    return;
+  }
   if (off != nullptr) {
     SFGS_COUNT_LAUNCH();
     render_fwd_jitter_kernel<<<grid, BLEND_THREADS, 0, st>>>(im.ranges, b.point_list, b.inst_mask, im.hdr, a->width,
@@ -218,9 +241,6 @@ void sfgs_launch_render_fwd(const sfgs_forward_args* a, const GeomLayout& g, con
                                                              im.n_contrib, reinterpret_cast<const float2*>(off));
     return;
   }
-  OutPeers op = {};
-  if (a->out_peers != nullptr && a->n_out_peers > 0)
-    for (op.n = 0; op.n < a->n_out_peers && op.n < 8; op.n++) op.p[op.n] = a->out_peers[op.n];
   SFGS_COUNT_LAUNCH();
   const auto kernel = a->ED > 0 ? render_fwd_warp_kernel<true> : render_fwd_warp_kernel<false>;
   kernel<<<grid, BLEND_THREADS, 0, st>>>(im.ranges, b.point_list, b.inst_mask, im.hdr, a->width, a->height, band0,

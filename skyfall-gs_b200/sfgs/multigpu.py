@@ -107,15 +107,26 @@ def gaussian_slices(P: int, world: int) -> List[int]:
     return [min(g * per, P) for g in range(world + 1)]
 
 
-def reduce_scatter_sums(acc: torch.Tensor, group=None) -> torch.Tensor:
+def reduce_scatter_sums(acc: torch.Tensor, group=None, ordered: bool = False) -> torch.Tensor:
     """acc: this rank's partial [P,16] blend-adjoint sums.  Returns the complete sums of this rank's slice
     ([ceil(P/world),16]; rows past P are zero).  NCCL: one reduce_scatter; backends without it (gloo): all_reduce
-    + slice."""
+    + slice.
+
+    ordered=True: the exchange is reproducible as well — one all_to_all_single hands every rank all ranks' partials of
+    its slice, which are then added in rank order.  With the deterministic phase 1 this makes the complete sums, and
+    so the phase-2 gradients, bit-identical from run to run."""
     world, rank = dist.get_world_size(group), dist.get_rank(group)
     P = acc.shape[0]
     per = (P + world - 1) // world
     if per * world != P:
         acc = torch.cat([acc, acc.new_zeros((per * world - P, acc.shape[1]))], 0)
+    if ordered:
+        parts = torch.empty((world, per, acc.shape[1]), dtype=acc.dtype, device=acc.device)
+        dist.all_to_all_single(parts, acc.contiguous(), group=group)   # parts[r]: rank r's partials of this slice
+        out = parts[0].clone()
+        for r in range(1, world):
+            out += parts[r]
+        return out
     if dist.get_backend(group) == "nccl":
         out = torch.empty((per, acc.shape[1]), dtype=acc.dtype, device=acc.device)
         dist.reduce_scatter_tensor(out, acc.contiguous(), op=dist.ReduceOp.SUM, group=group)
@@ -123,6 +134,26 @@ def reduce_scatter_sums(acc: torch.Tensor, group=None) -> torch.Tensor:
     full = acc.clone()
     dist.all_reduce(full, op=dist.ReduceOp.SUM, group=group)
     return full[rank * per:(rank + 1) * per].contiguous()
+
+
+def reduce_camera_gradients(partial: torch.Tensor, group=None):
+    """partial: this rank's float64 [35] or [37] camera partial sums (the last tensor of a phase-2
+    `rasterize_gaussians_backward(..., camera_grad=True)`).  All-gathers the ranks' partials, adds them in rank order in
+    float64 and rounds once to float32, so every rank gets the same bits and the frame's camera gradients are rounded
+    once, as the one-call backward rounds them.  Returns (dL_dviewmatrix [4,4], dL_dprojmatrix [4,4], dL_dcampos [3])
+    and, for 37 terms, also (dL_dtanfovx, dL_dtanfovy) as 0-d tensors."""
+    n = partial.numel()
+    if partial.dtype != torch.float64 or n not in (35, 37):
+        raise ValueError(f"partial must be a float64 tensor of 35 or 37 camera terms, got {partial.dtype} {tuple(partial.shape)}")
+    world = dist.get_world_size(group)
+    parts = torch.empty((world, n), dtype=torch.float64, device=partial.device)
+    dist.all_gather_into_tensor(parts.view(-1), partial.reshape(-1).contiguous(), group=group)
+    total = parts[0].clone()
+    for r in range(1, world):
+        total += parts[r]
+    g = total.float()
+    ret = (g[0:16].view(4, 4), g[16:32].view(4, 4), g[32:35])
+    return ret + (g[35], g[36]) if n == 37 else ret
 
 
 def row_histogram(ranges: torch.Tensor, tiles_x: int) -> List[int]:

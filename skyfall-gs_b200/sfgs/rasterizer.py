@@ -83,7 +83,9 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
 
     `subpixel_offset` ([H,W,2] CUDA float32, or None): pixel (x, y) samples the splats at (x + off[y,x,0],
     y + off[y,x,1]) (sfgs_rasterize_forward_subpixel); the backward must be given the same tensor.  Offsets must be
-    finite; a NaN or Inf raises."""
+    finite; a NaN or Inf raises.  They combine with `tile_rows` and `out_peers`: every rank passes the whole frame's
+    offsets, and the bands reassemble the one-call frame bit for bit (with `out_peers` through
+    sfgs_rasterize_forward_subpixel_peers)."""
     if means3D.ndim != 2 or means3D.shape[1] != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")
     H, W, F = int(image_height), int(image_width), int(attr_degree)
@@ -156,8 +158,8 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
         if tile_rows is not None:
             a.tile_row_begin, a.tile_row_end = _band(tile_rows)
         if subpixel_offset is not None:
-            rendered = N.check(L.sfgs_rasterize_forward_subpixel(C.byref(a), _ptr(subpixel_offset, keep)),
-                               "sfgs_rasterize_forward_subpixel")
+            entry = "sfgs_rasterize_forward_subpixel" + ("_peers" if out_peers is not None else "")
+            rendered = N.check(getattr(L, entry)(C.byref(a), _ptr(subpixel_offset, keep)), entry)
         else:
             rendered = N.check(L.sfgs_rasterize_forward(C.byref(a)), "sfgs_rasterize_forward")
     ret = (rendered, out_color, out_depth, out_norm, out_alpha, radii, out_extra,
@@ -217,7 +219,8 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     warn and run the default backward.
 
     `subpixel_offset`: the tensor the forward was given (sfgs_rasterize_backward_subpixel and its deterministic form);
-    no gradient is formed with respect to it.
+    no gradient is formed with respect to it.  It combines with both phases and with `acc_peers` (through
+    sfgs_rasterize_backward_subpixel_peers).
 
     `camera_grad=True` (one-call backward only): the same call through sfgs_rasterize_backward_camera, which also forms
     the camera gradients; the tuple then ends with (dL_dviewmatrix [4,4], dL_dprojmatrix [4,4], dL_dcampos [3]), in the
@@ -226,7 +229,12 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     `camera_grad=True, intrinsics_grad=True`: the same call through sfgs_rasterize_backward_camera_intrinsics, which
     also forms the gradients with respect to the focal lengths; the tuple then ends with the three camera tensors and
     (dL_dtanfovx, dL_dtanfovy), 0-d tensors.  Every other output, the camera tensors included, is bit-identical to the
-    call without it."""
+    call without it.
+
+    `phase=2, camera_grad=True[, intrinsics_grad=True]` (sfgs_rasterize_backward_camera_partial): the tuple ends with
+    ONE float64 tensor of 35 [37] camera terms, the unrounded sums over the Gaussians of `gauss_range`.  The ranks of a
+    sharded frame add these partials and round once (sfgs.multigpu.reduce_camera_gradients).  The gradient rows are
+    bit-identical to the phase-2 call without it."""
     if intrinsics_grad and not camera_grad:
         raise ValueError("intrinsics_grad=True needs camera_grad=True")
     if subpixel_offset is not None:
@@ -244,6 +252,8 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
         z = lambda *s: torch.zeros(s, **fopt)  # noqa: E731
         ret = (z(P, 3), z(P, 3), z(P, 1), z(P, 3), z(P, 6), z(P, 3), z(P, M, 3), z(P, 3), z(P, 4),
                z(P, F) if F > 0 else torch.empty(0, **fopt))
+        if camera_grad and phase == 2:
+            return ret + (torch.zeros((37 if intrinsics_grad else 35,), dtype=torch.float64, device=dev),)
         if camera_grad:
             ret += (z(4, 4), z(4, 4), z(3))
         return ret + (z(), z()) if intrinsics_grad else ret
@@ -321,7 +331,14 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
         a.stream = torch.cuda.current_stream(dev).cuda_stream
         if tile_rows is not None:
             a.tile_row_begin, a.tile_row_end = _band(tile_rows)
-        if camera_grad:
+        if camera_grad and phase == 2:
+            ncam = 37 if intrinsics_grad else 35
+            dL_dcamera = torch.empty((ncam,), dtype=torch.float64, device=dev)
+            off = _ptr(subpixel_offset, keep) if subpixel_offset is not None else None
+            N.check(L.sfgs_rasterize_backward_camera_partial(C.byref(a), off, int(deterministic), ncam,
+                                                             dL_dcamera.data_ptr()),
+                    "sfgs_rasterize_backward_camera_partial")
+        elif camera_grad:
             dL_dcamera = torch.empty((37 if intrinsics_grad else 35,), **fopt)
             off = _ptr(subpixel_offset, keep) if subpixel_offset is not None else None
             entry = "sfgs_rasterize_backward_camera_intrinsics" if intrinsics_grad else "sfgs_rasterize_backward_camera"
@@ -332,7 +349,8 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
                 N.check(L.sfgs_rasterize_backward_deterministic_subpixel(C.byref(a), off),
                         "sfgs_rasterize_backward_deterministic_subpixel")
             else:
-                N.check(L.sfgs_rasterize_backward_subpixel(C.byref(a), off), "sfgs_rasterize_backward_subpixel")
+                entry = "sfgs_rasterize_backward_subpixel" + ("_peers" if acc_peers is not None else "")
+                N.check(getattr(L, entry)(C.byref(a), off), entry)
         elif deterministic:
             N.check(L.sfgs_rasterize_backward_deterministic(C.byref(a)), "sfgs_rasterize_backward_deterministic")
         else:
@@ -345,6 +363,8 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
         return acc      # None when the sums went straight to the peers' slices
     ret = (outs["means2D"], outs["colors"], outs["opacity"], outs["means3D"], outs["cov3D"], outs["norm3D"],
            dL_dsh, outs["scales"], outs["rot"], dL_dextra)
+    if camera_grad and phase == 2:
+        return ret + (dL_dcamera,)
     if camera_grad:
         ret += (dL_dcamera[0:16].view(4, 4), dL_dcamera[16:32].view(4, 4), dL_dcamera[32:35])
     if intrinsics_grad:
