@@ -285,6 +285,47 @@ int sfgs_rasterize_backward_camera_intrinsics(const sfgs_backward_args* a, const
 int sfgs_rasterize_backward_camera_partial(const sfgs_backward_args* a, const float* subpixel_offset,
                                            int deterministic, int ncam, double* dL_dcamera_partial);
 
+/* ---- CUDA-graph capture (torch.cuda.graph) ------------------------------------------------------------------------
+ * The one-call forward and backward in a form that can be captured into a CUDA graph and replayed: nothing on the host
+ * waits for the device, nothing is copied back, and the camera intrinsics may live in device memory, so one captured
+ * graph renders any camera whose buffers the caller refills before each replay.  Every option of the one-call entries
+ * is an argument: subpixel_offset (NULL or as sfgs_rasterize_forward_subpixel), deterministic and the camera terms.
+ *
+ * Forward.  a->capacity_hint > 0 is required and is the binning capacity; the forward is never re-run and the running
+ * capacity estimate (sfgs_capacity_estimate) and sfgs_last_capacity / sfgs_overflow_reruns are not updated.  Returns
+ * SFGS_OK, not num_rendered.  After the tile scan a one-thread kernel ORs the frame's error flags into *status, a
+ * DEVICE word the caller owns and clears (sticky across calls):
+ *   SFGS_STATUS_OVERFLOW   the frame has more tile instances than the capacity: its images are not written, and the
+ *                          backward of the frame writes zero blend-adjoint sums (the gradients through the blend are 0);
+ *   SFGS_STATUS_PREFILTER  `prefiltered` was set but a Gaussian failed the frustum test (the eager forward's BADARG);
+ *   SFGS_STATUS_OFFSET     a subpixel offset is NaN or Inf (the eager forward's BADARG).
+ * No kernel reads or writes past the capacity after an overflow.
+ * tan_fov: NULL (a->tan_fovx / a->tan_fovy are used and baked into a captured graph) or a DEVICE float [2]
+ * {tan_fovx, tan_fovy}, read by the kernels at run time; the focal lengths W / (2 tan_fovx), H / (2 tan_fovy) and the
+ * 1.3 tan frustum clamp are formed from it on the device, bit for bit as the host forms them from the floats.
+ * Before any CUDA work: a NULL status or debug != 0 (it synchronises) return SFGS_E_BADARG, capacity_hint <= 0
+ * SFGS_E_BADARG; a tile-row band or out_peers SFGS_E_UNSUPPORTED; the remaining validation is the one-call forward's.
+ *
+ * Backward.  a->R must be the capacity the forward was given (> 0): it only sizes scratch (the deterministic order
+ * scratch is sized and its flags cleared by capacity); the frame's own instance count is read on the device.  The
+ * blend adjoint is always launched, and it and the deterministic ordering kernels return at once when the forward
+ * overflowed.  deterministic != 0 selects sfgs_rasterize_backward_deterministic; ncam = 0 (no camera terms), 35
+ * (sfgs_rasterize_backward_camera) or 37 (sfgs_rasterize_backward_camera_intrinsics), with dL_dcamera the DEVICE [ncam]
+ * output (NULL when ncam = 0); at 37 the focal terms use tan_fov when it is given.  Outputs are bit-identical to the
+ * matching eager entry's for the same inputs (with deterministic != 0; otherwise up to its atomics).
+ * Before any CUDA work: debug != 0, a->R <= 0, a NULL dL_dcamera with ncam > 0 or another ncam return SFGS_E_BADARG;
+ * phases 1 and 2, acc_peers and a tile-row band SFGS_E_UNSUPPORTED. */
+#define SFGS_STATUS_OVERFLOW 1u
+#define SFGS_STATUS_PREFILTER 2u
+#define SFGS_STATUS_OFFSET 4u
+int sfgs_rasterize_forward_graph(const sfgs_forward_args* a, const float* subpixel_offset, const float* tan_fov,
+                                 unsigned int* status);
+int sfgs_rasterize_backward_graph(const sfgs_backward_args* a, const float* subpixel_offset, int deterministic,
+                                  const float* tan_fov, float* dL_dcamera, int ncam);
+/* The running estimate of the instance count the eager forward keeps for (device, P, width, height) over the whole
+ * image, from its earlier calls; -1 when there is none.  Read-only: the graph entries size their capacity from it. */
+long long sfgs_capacity_estimate(int device, int P, int width, int height);
+
 /* ---- markVisible --------------------------------------------------------- */
 int sfgs_mark_visible(int P, const float* means3D, const float* viewmatrix,
                       const float* projmatrix, unsigned char* present, void* stream);

@@ -25,10 +25,11 @@ std::atomic<long long> g_sfgs_launches{0};
 
 void sfgs_launch_preprocess(const sfgs_forward_args* a, const GeomLayout& g, const ImageLayout& im,
                             const BinningLayout& b, unsigned long long capacity, float focal_x, float focal_y,
-                            cudaStream_t st);
+                            const float* tan_fov, cudaStream_t st);
 void sfgs_launch_mark_visible(int P, const float* means3D, const float* viewmatrix, unsigned char* present,
                               cudaStream_t st);
 void sfgs_launch_tile_scan(const ImageLayout& im, unsigned long long capacity, cudaStream_t st);
+void sfgs_launch_forward_status(const ImageLayout& im, unsigned int* status, cudaStream_t st);
 void sfgs_launch_scatter(const GeomLayout& g, const ImageLayout& im, const BinningLayout& b, int P,
                          unsigned long long capacity, bool dilate, cudaStream_t st);
 void sfgs_launch_tile_sort(const GeomLayout& g, const ImageLayout& im, const BinningLayout& b, int P, bool dilate,
@@ -38,13 +39,14 @@ void sfgs_launch_render_fwd(const sfgs_forward_args* a, const GeomLayout& g, con
                             const BinningLayout& b, const float* off, cudaStream_t st);
 void sfgs_launch_render_bwd(const sfgs_backward_args* a, const GeomLayout& g, const ImageLayout& im,
                             const BinningLayout& b, float* acc, float* part, unsigned char* written, const float* off,
-                            cudaStream_t st);
+                            bool guarded, cudaStream_t st);
 size_t sfgs_order_scratch_bytes(int P, long long R);
 SfgsOrderScratch sfgs_order_scratch(char* base, int P, long long R);
 void sfgs_launch_order_prepare(int P, const GeomLayout& g, const ImageLayout& im, const BinningLayout& b,
-                               const int* radii, int band0, int band1, const SfgsOrderScratch& o, cudaStream_t st);
+                               const int* radii, int band0, int band1, const SfgsOrderScratch& o, bool guarded,
+                               cudaStream_t st);
 void sfgs_launch_order_reduce(int P, const GeomLayout& g, const int* radii, bool all_rows, const SfgsOrderScratch& o,
-                              float* acc, cudaStream_t st);
+                              float* acc, const uint32_t* hdr_guard, cudaStream_t st);
 int sfgs_launch_activations_fwd(int P, const float* opacity_raw, const float* scaling_raw, const float* rotation_raw,
                                 const double* filter_3D, float* opacity, float* scales, float* rotations,
                                 cudaStream_t st);
@@ -54,7 +56,7 @@ int sfgs_launch_activations_bwd(int P, const float* opacity_raw, const float* sc
                                 float* g_rotation_raw, cudaStream_t st);
 void sfgs_launch_gauss_bwd(const sfgs_backward_args* a, const GeomLayout& g, float focal_x, float focal_y,
                            const float* acc, int g_begin, int g_end, int acc_row0, double* cam_part, int ncam,
-                           cudaStream_t st);
+                           const float* tan_fov, cudaStream_t st);
 size_t sfgs_camera_scratch_bytes(int P, int ncam);
 void sfgs_launch_camera_reduce(int P, int ncam, const double* cam_part, float* dL_dcamera, cudaStream_t st);
 void sfgs_launch_camera_partial_reduce(int n, int ncam, const double* cam_part, double* dL_dcamera, cudaStream_t st);
@@ -195,9 +197,10 @@ struct PinnedHdr {
 constexpr int MAX_DEVICES = 64;
 thread_local PinnedHdr t_hdr_dev[MAX_DEVICES];
 
-int rasterize_forward(const sfgs_forward_args* a, const float* off);
+int rasterize_forward(const sfgs_forward_args* a, const float* off, const float* tan_fov = nullptr,
+                      unsigned int* status = nullptr);
 int rasterize_backward(const sfgs_backward_args* a, bool deterministic, const float* off, float* dL_dcamera,
-                       double* dL_dcamera_partial, int ncam);
+                       double* dL_dcamera_partial, int ncam, bool graph = false, const float* tan_fov = nullptr);
 
 // the combinations the subpixel-offset entry points reject (checked before any CUDA work): extra_attrs, which have no
 // kernels with offsets, and -- unless the entry is a _subpixel_peers one -- the fused peer exchanges, which the
@@ -329,11 +332,51 @@ int sfgs_rasterize_backward_camera_partial(const sfgs_backward_args* a, const fl
   return backward_camera_partial(a, subpixel_offset, deterministic, ncam, dL_dcamera_partial);
 }
 
+int sfgs_rasterize_forward_graph(const sfgs_forward_args* a, const float* subpixel_offset, const float* tan_fov,
+                                 unsigned int* status) {
+  if (!a) return fail(SFGS_E_BADARG, "forward_graph: null args");
+  if (!status) return fail(SFGS_E_BADARG, "forward_graph: null status word");
+  if (a->debug) return fail(SFGS_E_BADARG, "forward_graph: debug synchronises after every stage and cannot be captured");
+  if (a->capacity_hint <= 0)
+    return fail(SFGS_E_BADARG, "forward_graph: capacity_hint must be > 0 (the binning capacity of the captured frame)");
+  if (a->tile_row_begin != 0 || a->tile_row_end != 0)
+    return fail(SFGS_E_UNSUPPORTED, "forward_graph: tile-row bands are not supported under graph capture");
+  if (a->out_peers != nullptr) return fail(SFGS_E_UNSUPPORTED, "forward_graph: out_peers are not supported under graph capture");
+  if (subpixel_offset != nullptr && a->ED > 0)
+    return fail(SFGS_E_UNSUPPORTED, "forward_graph: extra_attrs are not supported with subpixel offsets");
+  return rasterize_forward(a, subpixel_offset, tan_fov, status);
+}
+
+int sfgs_rasterize_backward_graph(const sfgs_backward_args* a, const float* subpixel_offset, int deterministic,
+                                  const float* tan_fov, float* dL_dcamera, int ncam) {
+  if (!a) return fail(SFGS_E_BADARG, "backward_graph: null args");
+  if (a->debug) return fail(SFGS_E_BADARG, "backward_graph: debug synchronises after every stage and cannot be captured");
+  if (a->R <= 0) return fail(SFGS_E_BADARG, "backward_graph: R must be the forward's binning capacity (> 0)");
+  if (ncam != 0 && ncam != 35 && ncam != 37) return fail(SFGS_E_BADARG, "backward_graph: ncam must be 0, 35 or 37");
+  if (ncam != 0 && !dL_dcamera) return fail(SFGS_E_BADARG, "backward_graph: null dL_dcamera");
+  if (a->phase != 0)
+    return fail(SFGS_E_UNSUPPORTED, "backward_graph: phases 1 and 2 (the two-phase backward) are not supported under graph capture");
+  if (a->acc_peers != nullptr) return fail(SFGS_E_UNSUPPORTED, "backward_graph: acc_peers are not supported under graph capture");
+  if (a->tile_row_begin != 0 || a->tile_row_end != 0)
+    return fail(SFGS_E_UNSUPPORTED, "backward_graph: tile-row bands are not supported under graph capture");
+  if (subpixel_offset != nullptr && a->ED > 0)
+    return fail(SFGS_E_UNSUPPORTED, "backward_graph: extra_attrs are not supported with subpixel offsets");
+  if (ncam != 0 && !a->scratch_alloc) return fail(SFGS_E_BADARG, "backward_graph: null scratch allocator");
+  return rasterize_backward(a, deterministic != 0, subpixel_offset, ncam != 0 ? dL_dcamera : nullptr, nullptr, ncam, true,
+                            tan_fov);
+}
+
+long long sfgs_capacity_estimate(int device, int P, int width, int height) {
+  return cap_lookup(CapKey{device, P, width, height, 0, 0});
+}
+
 }  // extern "C"
 
 namespace {
 
-int rasterize_forward(const sfgs_forward_args* a, const float* off) {
+// tan_fov, status: the graph forward (sfgs_rasterize_forward_graph, checked by the caller): status != NULL queues the
+// pipeline once at capacity_hint with no host wait, and a kernel ORs the header's error flags into *status
+int rasterize_forward(const sfgs_forward_args* a, const float* off, const float* tan_fov, unsigned int* status) {
   if (!a) return fail(SFGS_E_BADARG, "forward: null args");
   if (a->P < 0 || a->width <= 0 || a->height <= 0) return fail(SFGS_E_BADARG, "forward: bad sizes");
   if (a->ED < 0 || a->ED > SFGS_MAX_EXTRA) return fail(SFGS_E_BADARG, "forward: ED out of range");
@@ -371,6 +414,60 @@ int rasterize_forward(const sfgs_forward_args* a, const float* off) {
   if (!iptr) return fail(SFGS_E_ALLOC, "forward: image allocator returned NULL");
   ImageLayout im(sfgs_align_ptr(iptr), a->width, a->height);
 
+  // The whole pipeline for one binning capacity.  `after_scan` runs right after the tile scan, when num_rendered and
+  // the error flags are final: the eager forward starts the header's copy to the host there, the graph forward
+  // launches its status kernel.
+  auto queue = [&](long long capacity, auto&& after_scan) -> int {
+    const size_t bbytes = BinningLayout(nullptr, (size_t)capacity).bytes;
+    char* bptr = a->binning_alloc(a->binning_user, bbytes);
+    if (!bptr) return fail(SFGS_E_ALLOC, "forward: binning allocator returned NULL");
+    BinningLayout b(sfgs_align_ptr(bptr), (size_t)capacity);
+
+    // tile histogram + header start at zero
+    PROF_BEGIN(ST_FWD_ZERO);
+    CU(cudaMemsetAsync(im.hdr, 0, im.zero_bytes, st));   // header + tile histogram are adjacent
+    if (off) sfgs_launch_offset_bound(im, a->width, a->height, off, st);   // the masks' dilation, before the key scatter
+    PROF_END();
+
+    if (P > 0) {
+      PROF_BEGIN(ST_PREPROCESS);
+      sfgs_launch_preprocess(a, g, im, b, (unsigned long long)capacity, focal_x, focal_y, tan_fov, st);
+      PROF_END();
+      STAGE_CHECK("preprocess");
+    }
+    PROF_BEGIN(ST_SCAN);
+    sfgs_launch_tile_scan(im, (unsigned long long)capacity, st);
+    PROF_END();
+    STAGE_CHECK("tile_scan");
+    const int rc = after_scan();
+    if (rc != SFGS_OK) return rc;
+    if (P > 0) {
+      PROF_BEGIN(ST_EMIT);
+      sfgs_launch_scatter(g, im, b, a->P, (unsigned long long)capacity, off != nullptr, st);
+      PROF_END();
+      STAGE_CHECK("scatter_keys");
+      PROF_BEGIN(ST_SORT);
+      sfgs_launch_tile_sort(g, im, b, a->P, off != nullptr, st);
+      PROF_END();
+      STAGE_CHECK("tile_sort");
+    }
+    PROF_BEGIN(ST_RENDER_FWD);
+    sfgs_launch_render_fwd(a, g, im, b, off, st);
+    PROF_END();
+    STAGE_CHECK("render_fwd");
+    return SFGS_OK;
+  };
+
+  if (status != nullptr) {
+    // captured: one pass at the caller's capacity; the overflow flag reaches the caller through *status, and every
+    // kernel after the scan returns at once on it
+    return queue(a->capacity_hint, [&]() -> int {
+      sfgs_launch_forward_status(im, status, st);
+      STAGE_CHECK("forward_status");
+      return SFGS_OK;
+    });
+  }
+
   int dev = 0;
   CU(cudaGetDevice(&dev));
   if (dev < 0 || dev >= MAX_DEVICES) return fail(SFGS_E_UNSUPPORTED, "forward: device ordinal >= 64");
@@ -386,45 +483,14 @@ int rasterize_forward(const sfgs_forward_args* a, const float* off) {
 
   long long R = 0;
   for (int attempt = 0; attempt < 3; attempt++) {
-    const size_t bbytes = BinningLayout(nullptr, (size_t)capacity).bytes;
-    char* bptr = a->binning_alloc(a->binning_user, bbytes);
-    if (!bptr) return fail(SFGS_E_ALLOC, "forward: binning allocator returned NULL");
-    BinningLayout b(sfgs_align_ptr(bptr), (size_t)capacity);
-
-    // tile histogram + header start at zero
-    PROF_BEGIN(ST_FWD_ZERO);
-    CU(cudaMemsetAsync(im.hdr, 0, im.zero_bytes, st));   // header + tile histogram are adjacent
-    if (off) sfgs_launch_offset_bound(im, a->width, a->height, off, st);   // the masks' dilation, before the key scatter
-    PROF_END();
-
-    if (P > 0) {
-      PROF_BEGIN(ST_PREPROCESS);
-      sfgs_launch_preprocess(a, g, im, b, (unsigned long long)capacity, focal_x, focal_y, st);
-      PROF_END();
-      STAGE_CHECK("preprocess");
-    }
-    PROF_BEGIN(ST_SCAN);
-    sfgs_launch_tile_scan(im, (unsigned long long)capacity, st);
-    PROF_END();
-    STAGE_CHECK("tile_scan");
     // num_rendered and the overflow flag are final after the scan: start their copy now and let the host wait
     // on this event only, so it returns (and the caller can queue the backward) while sort + blend still run
-    CU(cudaMemcpyAsync(hhdr, im.hdr, HDR_COPY_WORDS * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-    CU(cudaEventRecord(t_hdr.ev, st));
-    if (P > 0) {
-      PROF_BEGIN(ST_EMIT);
-      sfgs_launch_scatter(g, im, b, a->P, (unsigned long long)capacity, off != nullptr, st);
-      PROF_END();
-      STAGE_CHECK("scatter_keys");
-      PROF_BEGIN(ST_SORT);
-      sfgs_launch_tile_sort(g, im, b, a->P, off != nullptr, st);
-      PROF_END();
-      STAGE_CHECK("tile_sort");
-    }
-    PROF_BEGIN(ST_RENDER_FWD);
-    sfgs_launch_render_fwd(a, g, im, b, off, st);
-    PROF_END();
-    STAGE_CHECK("render_fwd");
+    const int rc = queue(capacity, [&]() -> int {
+      CU(cudaMemcpyAsync(hhdr, im.hdr, HDR_COPY_WORDS * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+      CU(cudaEventRecord(t_hdr.ev, st));
+      return SFGS_OK;
+    });
+    if (rc != SFGS_OK) return rc;
 
     CU(cudaEventSynchronize(t_hdr.ev));
     if (debug) CU(cudaStreamSynchronize(st));
@@ -445,9 +511,12 @@ int rasterize_forward(const sfgs_forward_args* a, const float* off) {
 
 // dL_dcamera: NULL, or (phase 0 only, checked by the caller) the DEVICE [ncam] camera gradients to form as well;
 // dL_dcamera_partial: NULL, or (phase 2 only, checked by the caller) the DEVICE [ncam] float64 camera sums of the
-// Gaussian slice, unrounded.  ncam = 35 (pose terms) or 37 (pose and focal terms)
+// Gaussian slice, unrounded.  ncam = 35 (pose terms) or 37 (pose and focal terms).
+// graph (sfgs_rasterize_backward_graph, phase 0 only, checked by the caller): a->R is the forward's binning capacity and
+// only sizes scratch; the blend adjoint is always launched and it and the ordering kernels check the overflow flag
+// first.  tan_fov: NULL or the DEVICE [2] intrinsics the per-Gaussian adjoint reads.
 int rasterize_backward(const sfgs_backward_args* a, bool deterministic, const float* off, float* dL_dcamera,
-                       double* dL_dcamera_partial, int ncam) {
+                       double* dL_dcamera_partial, int ncam, bool graph, const float* tan_fov) {
   if (!a) return fail(SFGS_E_BADARG, "backward: null args");
   if (a->P < 0 || a->width <= 0 || a->height <= 0) return fail(SFGS_E_BADARG, "backward: bad sizes");
   if (deterministic && a->acc_peers != nullptr)
@@ -529,16 +598,16 @@ int rasterize_backward(const sfgs_backward_args* a, bool deterministic, const fl
     PROF_BEGIN(ST_BWD_ZERO);
     if (R > 0) CU(cudaMemsetAsync(order.written, 0, (size_t)R * BWD_BLOCKS, st));
     PROF_END();
-    if (R > 0) {
+    if (R > 0) {   // graph: R is the capacity (> 0), so the adjoint always runs
       PROF_BEGIN(ST_RENDER_BWD);
-      sfgs_launch_render_bwd(a, g, im, b, acc, order.part, order.written, off, st);
+      sfgs_launch_render_bwd(a, g, im, b, acc, order.part, order.written, off, graph, st);
       PROF_END();
       STAGE_CHECK("render_bwd");
     }
     const SfgsBand band = sfgs_band(a->tile_row_begin, a->tile_row_end, im.tiles_y);
     PROF_BEGIN(ST_BWD_ORDER);
-    sfgs_launch_order_prepare(P, g, im, b, a->radii, band.b0, band.b1, order, st);
-    sfgs_launch_order_reduce(P, g, a->radii, phase == 1, order, acc, st);
+    sfgs_launch_order_prepare(P, g, im, b, a->radii, band.b0, band.b1, order, graph, st);
+    sfgs_launch_order_reduce(P, g, a->radii, phase == 1, order, acc, graph ? im.hdr : nullptr, st);
     PROF_END();
     STAGE_CHECK("bwd_order");
   } else if (do_blend) {
@@ -552,16 +621,17 @@ int rasterize_backward(const sfgs_backward_args* a, bool deterministic, const fl
     else CU(cudaMemsetAsync(acc, 0, (size_t)P * 16 * sizeof(float), st));
     if (a->ED > 0) CU(cudaMemsetAsync(a->dL_dextra, 0, (size_t)P * a->ED * sizeof(float), st));
     PROF_END();
-    if (a->R > 0) {
+    if (a->R > 0 || graph) {
       PROF_BEGIN(ST_RENDER_BWD);
-      sfgs_launch_render_bwd(a, g, im, b, acc, nullptr, nullptr, off, st);
+      sfgs_launch_render_bwd(a, g, im, b, acc, nullptr, nullptr, off, graph, st);
       PROF_END();
       STAGE_CHECK("render_bwd");
     }
   }
   if (do_gauss) {
     PROF_BEGIN(ST_GAUSS_BWD);
-    sfgs_launch_gauss_bwd(a, g, focal_x, focal_y, acc, g_begin, g_end, phase == 2 ? g_begin : 0, cam_part, ncam, st);
+    sfgs_launch_gauss_bwd(a, g, focal_x, focal_y, acc, g_begin, g_end, phase == 2 ? g_begin : 0, cam_part, ncam, tan_fov,
+                          st);
     if (dL_dcamera) sfgs_launch_camera_reduce(P, ncam, cam_part, dL_dcamera, st);
     // an empty slice has no spans: the reduction writes zeros
     if (dL_dcamera_partial) sfgs_launch_camera_partial_reduce(g_end - g_begin, ncam, cam_part, dL_dcamera_partial, st);

@@ -521,6 +521,22 @@ void sfgs_launch_tile_scan(const ImageLayout& im, unsigned long long capacity, c
   tile_scan_kernel<<<1, SCAN_THREADS, 0, st>>>(im.tiles, im.tile_count, im.ranges, im.hdr, capacity);
 }
 
+namespace {
+// The graph forward's replacement for the host's read of the header: the frame's error flags, ORed into a sticky
+// status word the caller reads when it chooses (sfgs_rasterize_forward_graph).  Runs after the tile scan, when
+// HDR_OVERFLOW, HDR_PREFILTER and HDR_OFF_BAD are final.
+__global__ void forward_status_kernel(const uint32_t* __restrict__ hdr, unsigned int* __restrict__ status) {
+  const unsigned s = (hdr[HDR_OVERFLOW] ? SFGS_STATUS_OVERFLOW : 0u) | (hdr[HDR_PREFILTER] ? SFGS_STATUS_PREFILTER : 0u) |
+                     (hdr[HDR_OFF_BAD] ? SFGS_STATUS_OFFSET : 0u);
+  if (s) atomicOr(status, s);
+}
+}  // namespace
+
+void sfgs_launch_forward_status(const ImageLayout& im, unsigned int* status, cudaStream_t st) {
+  SFGS_COUNT_LAUNCH();
+  forward_status_kernel<<<1, 1, 0, st>>>(im.hdr, status);
+}
+
 // Gaussian ids below 2^24 ride in the key together with the reach mask (see scatter_keys_kernel)
 static inline bool sfgs_keys_packed(int P) {
   // SFGS_KEYS_PACKED=0 forces the unpacked path (what P > 2^24 takes) so that the tests can run it on small scenes

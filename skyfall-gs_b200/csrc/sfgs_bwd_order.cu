@@ -89,11 +89,15 @@ __global__ void __launch_bounds__(256) off_apply_kernel(int P, const uint32_t* _
   }
 }
 
-// inv[off[g] + rank(g, tile)] = sorted instance, one CTA per tile of the band
+// inv[off[g] + rank(g, tile)] = sorted instance, one CTA per tile of the band.
+// GUARD (the graph backward, sfgs_rasterize_backward_graph): nothing is done when the forward overflowed its binning
+// capacity (image header `hdr`), because the ranges then run past point_list and inv; without it `hdr` is not read.
+template <bool GUARD>
 __global__ void __launch_bounds__(256) inv_map_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list,
                                                       const float* __restrict__ rec, const int* __restrict__ radii,
                                                       const uint32_t* __restrict__ off, int gx, int gy, int band0,
-                                                      uint32_t* __restrict__ inv) {
+                                                      uint32_t* __restrict__ inv, const uint32_t* __restrict__ hdr) {
+  if (GUARD && hdr[HDR_OVERFLOW]) return;
   const int tx = blockIdx.x, ty = blockIdx.y + band0;
   const uint2 range = ranges[ty * gx + tx];
   for (uint32_t i = range.x + threadIdx.x; i < range.y; i += blockDim.x) {
@@ -110,19 +114,21 @@ __global__ void __launch_bounds__(256) inv_map_kernel(const uint2* __restrict__ 
 // acc[g] = sum of Gaussian g's written rows, in (rank, block) order, in float64.  16 lanes per Gaussian, lane c = word
 // c.  The slots of a Gaussian are taken 16 at a time (lane k reads slot k's instance and flags); the rows of four
 // slots are loaded before they are added, so their latencies overlap.
+// GUARD: after an overflowed forward every Gaussian is taken to have no slots (inv was not written), so acc gets zeros.
+template <bool GUARD>
 __global__ void __launch_bounds__(256) ordered_reduce_kernel(int P, const uint32_t* __restrict__ tt,
                                                              const uint32_t* __restrict__ off,
                                                              const uint32_t* __restrict__ inv,
                                                              const uint2* __restrict__ written,
                                                              const float* __restrict__ part,
                                                              const int* __restrict__ radii, int all_rows,
-                                                             float* __restrict__ acc) {
+                                                             float* __restrict__ acc, const uint32_t* __restrict__ hdr) {
   const int g = blockIdx.x * 16 + (threadIdx.x >> 4);
   if (g >= P) return;
   if (!all_rows && radii[g] <= 0) return;          // rows the per-Gaussian adjoint never reads
   const int c = threadIdx.x & 15;
   const unsigned hmask = 0xFFFFu << (threadIdx.x & 16);
-  const uint32_t n = tt[g];
+  const uint32_t n = (GUARD && hdr[HDR_OVERFLOW]) ? 0u : tt[g];
   const uint32_t base = n ? off[g] : 0u;
   double s = 0.0;
   for (uint32_t k0 = 0; k0 < n; k0 += 16) {
@@ -179,22 +185,25 @@ SfgsOrderScratch sfgs_order_scratch(char* base, int P, long long R) {
 }
 
 void sfgs_launch_order_prepare(int P, const GeomLayout& g, const ImageLayout& im, const BinningLayout& b,
-                               const int* radii, int band0, int band1, const SfgsOrderScratch& o, cudaStream_t st) {
+                               const int* radii, int band0, int band1, const SfgsOrderScratch& o, bool guarded,
+                               cudaStream_t st) {
   const int nb = (P + SCAN_SPAN - 1) / SCAN_SPAN;
   SFGS_COUNT_LAUNCH(); off_block_sum_kernel<<<nb, 256, 0, st>>>(P, g.tiles_touched, o.bsum);
   SFGS_COUNT_LAUNCH(); off_block_scan_kernel<<<1, 1024, 0, st>>>(nb, o.bsum);
   SFGS_COUNT_LAUNCH(); off_apply_kernel<<<nb, 256, 0, st>>>(P, g.tiles_touched, o.bsum, o.off);
   if (band1 > band0) {
     SFGS_COUNT_LAUNCH();
-    inv_map_kernel<<<dim3(im.tiles_x, band1 - band0), 256, 0, st>>>(im.ranges, b.point_list, g.rec, radii, o.off,
-                                                                    im.tiles_x, im.tiles_y, band0, o.inv);
+    const auto kernel = guarded ? inv_map_kernel<true> : inv_map_kernel<false>;
+    kernel<<<dim3(im.tiles_x, band1 - band0), 256, 0, st>>>(im.ranges, b.point_list, g.rec, radii, o.off, im.tiles_x,
+                                                            im.tiles_y, band0, o.inv, im.hdr);
   }
 }
 
+// hdr_guard: NULL, or the image header whose overflow flag the graph backward's kernel checks first
 void sfgs_launch_order_reduce(int P, const GeomLayout& g, const int* radii, bool all_rows, const SfgsOrderScratch& o,
-                              float* acc, cudaStream_t st) {
+                              float* acc, const uint32_t* hdr_guard, cudaStream_t st) {
   SFGS_COUNT_LAUNCH();
-  ordered_reduce_kernel<<<(P + 15) / 16, 256, 0, st>>>(P, g.tiles_touched, o.off, o.inv,
-                                                       reinterpret_cast<const uint2*>(o.written), o.part, radii,
-                                                       all_rows ? 1 : 0, acc);
+  const auto kernel = hdr_guard != nullptr ? ordered_reduce_kernel<true> : ordered_reduce_kernel<false>;
+  kernel<<<(P + 15) / 16, 256, 0, st>>>(P, g.tiles_touched, o.off, o.inv, reinterpret_cast<const uint2*>(o.written),
+                                        o.part, radii, all_rows ? 1 : 0, acc, hdr_guard);
 }

@@ -737,6 +737,19 @@ gauss_bwd_intrinsics_kernel(GB_PARAMS, double* __restrict__ cam_part) {
   gauss_bwd_body<GB_CAM>(GB_ARGS, cam_part);
 }
 
+// Device-resident intrinsics (the graph backward, sfgs_rasterize_backward_graph): tan_fov [2] is read from device
+// memory and the focal lengths are formed from it as the host forms them (W / (2 tan_fovx), H / (2 tan_fovy)); then the
+// body of gauss_bwd_kernel (NCAM = 0), gauss_bwd_camera_kernel (35) or gauss_bwd_intrinsics_kernel (37) runs as is.
+template <int NCAM>
+__global__ void __launch_bounds__(GB_THREADS, GB_CTAS_PER_SM)
+gauss_bwd_devfov_kernel(GB_PARAMS, double* __restrict__ cam_part, const float* __restrict__ tan_fov, int W, int H) {
+  tan_fovx = tan_fov[0];
+  tan_fovy = tan_fov[1];
+  h_y = H / (2.0f * tan_fovy);
+  h_x = W / (2.0f * tan_fovx);
+  gauss_bwd_body<NCAM>(GB_ARGS, NCAM > 0 ? cam_part : nullptr);
+}
+
 #undef GB_PARAMS
 #undef GB_ARGS
 
@@ -814,15 +827,20 @@ void sfgs_launch_camera_partial_reduce(int n, int ncam, const double* cam_part, 
 
 // cam_part: NULL for the adjoint alone; else [ncam][spans] doubles (sfgs_camera_scratch_bytes) that receive every
 // span's camera partials, ncam = 35 (pose terms) or 37 (pose and focal terms)
+// tan_fov: NULL (the launch parameters a->tan_fovx / a->tan_fovy, focal_x, focal_y are used) or DEVICE float [2], read
+// by the kernel (gauss_bwd_devfov_kernel)
 void sfgs_launch_gauss_bwd(const sfgs_backward_args* a, const GeomLayout& g, float focal_x, float focal_y,
                            const float* acc, int g_begin, int g_end, int acc_row0, double* cam_part, int ncam,
-                           cudaStream_t st) {
+                           const float* tan_fov, cudaStream_t st) {
   if (g_end <= g_begin) return;
   static SfgsPerDeviceOnce attr_once;
   if (attr_once.first_use()) {
     cudaFuncSetAttribute(gauss_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GbShared));
     cudaFuncSetAttribute(gauss_bwd_camera_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GbShared));
     cudaFuncSetAttribute(gauss_bwd_intrinsics_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GbShared));
+    cudaFuncSetAttribute(gauss_bwd_devfov_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GbShared));
+    cudaFuncSetAttribute(gauss_bwd_devfov_kernel<GB_CAM_POSE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GbShared));
+    cudaFuncSetAttribute(gauss_bwd_devfov_kernel<GB_CAM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GbShared));
   }
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
@@ -841,7 +859,12 @@ void sfgs_launch_gauss_bwd(const sfgs_backward_args* a, const GeomLayout& g, flo
       focal_y, a->tan_fovx, a->tan_fovy, a->kernel_size, a->cam_pos, acc, a->dL_dmean2D, a->dL_dconic,              \
       a->dL_dopacity, a->dL_dcolor, a->dL_ddepth, a->dL_dmean3D, a->dL_dcov3D, a->dL_dnorm3D, dL_dsh, a->dL_dscale, \
       a->dL_drot
-  if (cam_part != nullptr && ncam == GB_CAM)
+  if (tan_fov != nullptr) {
+    const auto kernel = cam_part == nullptr ? gauss_bwd_devfov_kernel<0>
+                        : ncam == GB_CAM    ? gauss_bwd_devfov_kernel<GB_CAM>
+                                            : gauss_bwd_devfov_kernel<GB_CAM_POSE>;
+    kernel<<<blocks, GB_THREADS, sizeof(GbShared), st>>>(GB_LAUNCH_ARGS, cam_part, tan_fov, a->width, a->height);
+  } else if (cam_part != nullptr && ncam == GB_CAM)
     gauss_bwd_intrinsics_kernel<<<blocks, GB_THREADS, sizeof(GbShared), st>>>(GB_LAUNCH_ARGS, cam_part);
   else if (cam_part != nullptr)
     gauss_bwd_camera_kernel<<<blocks, GB_THREADS, sizeof(GbShared), st>>>(GB_LAUNCH_ARGS, cam_part);

@@ -202,6 +202,10 @@ __device__ __forceinline__ float radius_bound(float trace_sigma, float view_z, f
   return 3.f * sqrtf(tr2d) + 3.f;
 }
 
+// DEV_FOV: tan_fov [2] is read from device memory (the graph forward, sfgs_rasterize_forward_graph, whose camera
+// intrinsics are refilled between replays) and tan_fovx, tan_fovy, focal_x, focal_y are derived from it exactly as the
+// host derives them; without it the trailing pointer is not read and the code is that of the launch-parameter form.
+template <bool DEV_FOV>
 __global__ void __launch_bounds__(PRE_THREADS, 3)
 preprocess_kernel(int P, int D, int M,
                   const float* __restrict__ means3D, const float* __restrict__ scales, float scale_modifier,
@@ -215,7 +219,12 @@ preprocess_kernel(int P, int D, int M,
                   int* __restrict__ radii, float* __restrict__ rec, float* __restrict__ cov3D_out,
                   unsigned char* __restrict__ clamped, uint32_t* __restrict__ tiles_touched,
                   uint32_t* __restrict__ tile_count, uint32_t* __restrict__ hdr, uint4* __restrict__ tmp,
-                  unsigned long long capacity) {
+                  unsigned long long capacity, const float* __restrict__ tan_fov) {
+  if (DEV_FOV) {
+    tan_fovx = tan_fov[0]; tan_fovy = tan_fov[1];
+    focal_y = H / (2.0f * tan_fovy);
+    focal_x = W / (2.0f * tan_fovx);
+  }
   extern __shared__ __align__(16) unsigned char pre_smem[];
   float4* s_sh = reinterpret_cast<float4*>(pre_smem);                                    // [12][PRE_THREADS]
   uint32_t* s_incl = reinterpret_cast<uint32_t*>(pre_smem + 12 * PRE_THREADS * sizeof(float4));
@@ -491,23 +500,25 @@ __global__ void mark_visible_kernel(int P, const float* __restrict__ means3D,
 
 void sfgs_launch_preprocess(const sfgs_forward_args* a, const GeomLayout& g, const ImageLayout& im,
                             const BinningLayout& b, unsigned long long capacity, float focal_x, float focal_y,
-                            cudaStream_t st) {
+                            const float* tan_fov, cudaStream_t st) {
   const int blocks = (a->P + PRE_SPAN - 1) / PRE_SPAN;
   constexpr size_t smem = PRE_THREADS * (12 * sizeof(float4) + sizeof(uint32_t) + sizeof(int4) + sizeof(uint32_t)) +
                           PRE_SPAN * sizeof(unsigned short);
   static SfgsPerDeviceOnce attr_once;   // function attributes are per device
   if (attr_once.first_use()) {
-    cudaFuncSetAttribute(preprocess_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(preprocess_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(preprocess_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   }
   const SfgsBand band = sfgs_band(a->tile_row_begin, a->tile_row_end, im.tiles_y);
   const int band0 = band.b0, band1 = band.b1;
   SFGS_COUNT_LAUNCH();
-  preprocess_kernel<<<blocks, PRE_THREADS, smem, st>>>(
+  const auto kernel = tan_fov != nullptr ? preprocess_kernel<true> : preprocess_kernel<false>;
+  kernel<<<blocks, PRE_THREADS, smem, st>>>(
       a->P, a->D, a->M, a->means3D, a->scales, a->scale_modifier, a->rotations, a->opacities, a->shs,
       a->cov3D_precomp, a->norm3D_precomp, a->colors_precomp, a->viewmatrix, a->projmatrix, a->cam_pos,
       a->width, a->height, a->tan_fovx, a->tan_fovy, focal_x, focal_y, a->kernel_size, im.tiles_x, im.tiles_y,
       band0, band1, a->prefiltered,
-      a->radii, g.rec, g.cov3D, g.clamped, g.tiles_touched, im.tile_count, im.hdr, b.tmp, capacity);
+      a->radii, g.rec, g.cov3D, g.clamped, g.tiles_touched, im.tile_count, im.hdr, b.tmp, capacity, tan_fov);
 }
 
 void sfgs_launch_mark_visible(int P, const float* means3D, const float* viewmatrix, unsigned char* present,

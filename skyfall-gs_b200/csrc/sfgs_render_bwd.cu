@@ -421,14 +421,65 @@ render_bwd_jitter_peer_kernel(const uint2* __restrict__ ranges, const char* __re
                                             nullptr, nullptr, off);
 }
 
+// The graph backward's blend adjoint (sfgs_rasterize_backward_graph): launched whatever the frame's instance count,
+// so it first checks the forward's overflow flag -- after an overflow the ranges run past the binning capacity and
+// nothing may read point_list or write partial rows.  A kernel of its own, so that the kernels above keep their code.
+template <bool HAS_EXTRA, bool ORDERED, bool JITTER>
+__global__ void __launch_bounds__(BLEND_THREADS, 3)
+render_bwd_guarded_kernel(const uint2* __restrict__ ranges, const char* __restrict__ binning_base,
+                          const uint32_t* __restrict__ hdr, int W, int H, int band0,
+                          const float* __restrict__ bg_color, const float* __restrict__ rec,
+                          const float* __restrict__ accum_alphas, const uint32_t* __restrict__ n_contrib,
+                          const float* __restrict__ dL_dpixels, const float* __restrict__ dL_dpixel_depths,
+                          const float* __restrict__ dL_dpixel_norms, const float* __restrict__ dL_dpixel_alphas,
+                          const float* __restrict__ norm_raw, float* __restrict__ acc,
+                          const float* __restrict__ extras, const float* __restrict__ dL_dpixel_extras,
+                          float* __restrict__ dL_dextras, int ED, float* __restrict__ part,
+                          unsigned char* __restrict__ written, const float2* __restrict__ off) {
+  if (hdr[HDR_OVERFLOW]) return;
+  render_bwd_warp<false, HAS_EXTRA, ORDERED, JITTER>(ranges, binning_base, hdr, W, H, band0, bg_color, rec,
+                                                     accum_alphas, n_contrib, dL_dpixels, dL_dpixel_depths,
+                                                     dL_dpixel_norms, dL_dpixel_alphas, norm_raw, acc, PeerTable{},
+                                                     extras, dL_dpixel_extras, dL_dextras, ED, part, written, off);
+}
+
 }  // namespace
 
+// the graph backward's blend adjoint: no peers (sfgs_rasterize_backward_graph rejects acc_peers); extra_attrs only
+// without offsets and without the ordered form, as for the eager entries
+static void launch_render_bwd_guarded(const sfgs_backward_args* a, const GeomLayout& g, const ImageLayout& im,
+                                      const BinningLayout& b, float* acc, float* part, unsigned char* written,
+                                      const float* off, dim3 grid, int band0, cudaStream_t st) {
+  const size_t smem = sizeof(WarpSmem) * BLEND_WARPS, smem_j = sizeof(WarpSmemJitter) * BLEND_WARPS;
+  static SfgsPerDeviceOnce attr_once;
+  if (attr_once.first_use()) {
+    cudaFuncSetAttribute(render_bwd_guarded_kernel<false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(render_bwd_guarded_kernel<true, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(render_bwd_guarded_kernel<false, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(render_bwd_guarded_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_j);
+    cudaFuncSetAttribute(render_bwd_guarded_kernel<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_j);
+  }
+  const bool ordered = part != nullptr;
+  const auto kernel = off != nullptr ? (ordered ? render_bwd_guarded_kernel<false, true, true>
+                                                : render_bwd_guarded_kernel<false, false, true>)
+                      : ordered      ? render_bwd_guarded_kernel<false, true, false>
+                      : a->ED > 0    ? render_bwd_guarded_kernel<true, false, false>
+                                     : render_bwd_guarded_kernel<false, false, false>;
+  SFGS_COUNT_LAUNCH();
+  kernel<<<grid, BLEND_THREADS, off != nullptr ? smem_j : smem, st>>>(
+      im.ranges, (const char*)b.point_list, im.hdr, a->width, a->height, band0, a->background, g.rec, a->accum_alphas,
+      im.n_contrib, a->dL_dpix, a->dL_dpix_depth, a->dL_dpix_norm, a->dL_dpix_alpha, a->norm_raw, acc, a->extra_attrs,
+      a->dL_dpix_extra, a->dL_dextra, a->ED, part, written, reinterpret_cast<const float2*>(off));
+}
+
+// guarded: the graph backward's kernels (launch_render_bwd_guarded)
 void sfgs_launch_render_bwd(const sfgs_backward_args* a, const GeomLayout& g, const ImageLayout& im,
                             const BinningLayout& b, float* acc, float* part, unsigned char* written, const float* off,
-                            cudaStream_t st) {
+                            bool guarded, cudaStream_t st) {
   dim3 grid;
   int band0;
   if (!blend_grid(a->tile_row_begin, a->tile_row_end, im, grid, band0)) return;
+  if (guarded) { launch_render_bwd_guarded(a, g, im, b, acc, part, written, off, grid, band0, st); return; }
   PeerTable pt = {};
   const bool peer = a->acc_peers != nullptr && a->n_peers > 0;
   if (peer) {

@@ -4,6 +4,7 @@ Exposes the same three callables with the same positional signatures; the work
 is done by libsfgs.so through the C ABI in include/sfgs.h.
 """
 from sfgs.rasterizer import mark_visible, rasterize_gaussians, rasterize_gaussians_backward  # noqa: F401
+from sfgs.native import SfgsError  # noqa: F401
 from sfgs.native import lib as _lib
 
 

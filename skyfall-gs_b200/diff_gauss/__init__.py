@@ -27,6 +27,7 @@ if _pkg_root not in sys.path:  # make the sibling `sfgs` package importable when
     sys.path.insert(0, _pkg_root)
 
 from . import _C  # noqa: E402
+from sfgs import graphs as _graphs  # noqa: E402
 
 MAX_EXTRA_DIMS = 34  # RAST/cuda_rasterizer/auxiliary.h:20
 
@@ -125,6 +126,17 @@ class _RasterizeGaussians(torch.autograd.Function):
         ctx.fused = bool(fuse_normalize)
         off = _subpixel_offset(rs)
         fwd = _C.rasterize_gaussians_fused if ctx.fused else _C.rasterize_gaussians
+        # under stream capture (torch.cuda.graph) the capture-safe entries run: no host wait, intrinsics that are 0-d
+        # CUDA tensors read at replay time, a capacity fixed at capture (sfgs.graphs)
+        ctx.graph = means3D.is_cuda and torch.cuda.is_current_stream_capturing()
+        capacity = 0
+        if ctx.graph:
+            if rs.debug:
+                raise _C.SfgsError("diff_gauss: debug=True synchronises after every stage and cannot be captured in a "
+                                   "CUDA graph")
+            P = int(means3D.shape[0])
+            capacity = _graphs.resolve_capacity(means3D.device, P, rs.image_width, rs.image_height) if P > 0 else 1
+            fwd = functools.partial(fwd, capacity_hint=capacity, graph=True)
         if off is not None:
             # the offsets travel as the last argument, so that the debug snapshot holds them too
             fwd, native_args = _with_offset(fwd), native_args + (off,)
@@ -138,7 +150,8 @@ class _RasterizeGaussians(torch.autograd.Function):
         ctx.subpixel_offset = off
         ctx.raster_settings = rs
         ctx.camera = (viewmatrix, projmatrix, campos)
-        ctx.num_rendered = num_rendered
+        # the graph backward is given the capacity in place of num_rendered (not known on the host under capture)
+        ctx.num_rendered = capacity if ctx.graph else num_rendered
         ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, norm3Ds_precomp, radii,
                               extra_attrs, sh, geom_buf, binning_buf, img_buf, alpha, norm_raw)
         ctx.mark_non_differentiable(radii)
@@ -166,6 +179,8 @@ class _RasterizeGaussians(torch.autograd.Function):
         elif camera_grad:
             # only when asked for: a camera without requires_grad keeps the default native call
             bwd = functools.partial(bwd, camera_grad=True)
+        if ctx.graph:
+            bwd = functools.partial(bwd, graph=True)
         if ctx.subpixel_offset is not None:
             bwd, native_args = _with_offset(bwd), native_args + (ctx.subpixel_offset,)
         grads = _guarded(bwd, native_args, rs.debug, "snapshot_bw.dump", "backward")

@@ -98,6 +98,7 @@ EXPORTS = [
     "sfgs_selftest_expf", "sfgs_overflow_reruns", "sfgs_appearance_forward", "sfgs_appearance_backward",
     "sfgs_appearance_backward_scratch_bytes", "sfgs_compute_3d_filter",
     "sfgs_densification_stats", "sfgs_densify_plan_blocks", "sfgs_densify_plan", "sfgs_densify_apply",
+    "sfgs_rasterize_forward_graph", "sfgs_rasterize_backward_graph", "sfgs_capacity_estimate",
 ]
 STAGE_NAMES = ["fwd_zero", "preprocess", "tile_scan", "emit_keys", "tile_sort", "render_fwd", "bwd_zero", "render_bwd",
                "gauss_bwd", "bwd_order"]
@@ -138,6 +139,13 @@ def lib() -> C.CDLL:
     L.sfgs_rasterize_backward_camera_partial.argtypes = [C.POINTER(BackwardArgs), C.c_void_p, C.c_int, C.c_int,
                                                          C.c_void_p]
     L.sfgs_rasterize_backward_camera_partial.restype = C.c_int
+    L.sfgs_rasterize_forward_graph.argtypes = [C.POINTER(ForwardArgs), C.c_void_p, C.c_void_p, C.c_void_p]
+    L.sfgs_rasterize_forward_graph.restype = C.c_int
+    L.sfgs_rasterize_backward_graph.argtypes = [C.POINTER(BackwardArgs), C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                                C.c_int]
+    L.sfgs_rasterize_backward_graph.restype = C.c_int
+    L.sfgs_capacity_estimate.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int]
+    L.sfgs_capacity_estimate.restype = C.c_longlong
     L.sfgs_mark_visible.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.sfgs_mark_visible.restype = C.c_int
     L.sfgs_geom_bytes.argtypes = [C.c_int]; L.sfgs_geom_bytes.restype = C.c_size_t

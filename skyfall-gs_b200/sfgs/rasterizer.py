@@ -72,11 +72,38 @@ def check_subpixel_offset(subpixel_offset, H, W):
         raise ValueError(f"subpixel_offset must be a CUDA float32 tensor of shape ({H}, {W}, 2), got {what}")
 
 
+def _tan_fov(tan_fovx, tan_fovy, dev):
+    """(host floats, device [2] tensor or None) for the graph entries: 0-d CUDA tensors are read by the kernels at run
+    time (never with float(), which would synchronise); with two Python numbers they are baked in as launch
+    parameters."""
+    tensors = [isinstance(t, torch.Tensor) for t in (tan_fovx, tan_fovy)]
+    if not any(tensors):
+        return float(tan_fovx), float(tan_fovy), None
+    parts = []
+    for t, is_t in zip((tan_fovx, tan_fovy), tensors):
+        if is_t:
+            if not t.is_cuda or t.numel() != 1:
+                raise ValueError("under graph capture tanfovx / tanfovy must be Python numbers or 0-d CUDA tensors")
+            parts.append(t.detach().reshape(()).to(device=dev, dtype=torch.float32))
+        else:
+            parts.append(torch.full((), float(t), dtype=torch.float32, device=dev))
+    return 1.0, 1.0, torch.stack(parts)
+
+
+def _graph_unsupported(where, debug, tile_rows=None, peers=None, phase=0):
+    """The options a captured call cannot take, as a readable error raised before any work is queued."""
+    what = (["debug=True (it synchronises after every stage)"] * bool(debug) +
+            ["tile_rows"] * (tile_rows is not None) + [peers] * (peers is not None) +
+            [f"phase={phase} (the two-phase backward)"] * (phase != 0))
+    if what:
+        raise N.SfgsError(f"{where}: {', '.join(what)} cannot be captured in a CUDA graph")
+
+
 def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations, scale_modifier,
                         cov3Ds_precomp, norm3Ds_precomp, extra_attrs, attr_degree, viewmatrix, projmatrix,
                         tan_fovx, tan_fovy, kernel_size, image_height, image_width, sh, degree, campos,
                         prefiltered, debug, capacity_hint=0, tile_rows=None, fuse_normalize=False, out_planes=None,
-                        out_peers=None, subpixel_offset=None):
+                        out_peers=None, subpixel_offset=None, graph=False):
     """Same positional signature and return tuple as the reference's `_C.rasterize_gaussians`.  With
     `fuse_normalize=True` the returned normal map is already F.normalize(., dim=0) (the reference's torch post-op,
     diff_gauss/__init__.py:48) and the un-normalised blend is appended to the tuple for the backward.
@@ -85,9 +112,19 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
     y + off[y,x,1]) (sfgs_rasterize_forward_subpixel); the backward must be given the same tensor.  Offsets must be
     finite; a NaN or Inf raises.  They combine with `tile_rows` and `out_peers`: every rank passes the whole frame's
     offsets, and the bands reassemble the one-call frame bit for bit (with `out_peers` through
-    sfgs_rasterize_forward_subpixel_peers)."""
+    sfgs_rasterize_forward_subpixel_peers).
+
+    `graph=True`: the capture-safe forward (sfgs_rasterize_forward_graph) for torch.cuda.graph.  `capacity_hint` (> 0)
+    is the binning capacity; `tan_fovx` / `tan_fovy` may be 0-d CUDA tensors, read on the device at every replay; the
+    frame's error flags go to the sticky status word of sfgs.graphs instead of raising, and the first element of the
+    tuple is -1 (num_rendered is not known on the host).  debug, tile_rows and out_peers raise."""
     if means3D.ndim != 2 or means3D.shape[1] != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")
+    if graph:
+        _graph_unsupported("rasterize_gaussians(graph=True)", debug, tile_rows,
+                           "out_peers" if out_peers is not None else None)
+        if int(capacity_hint) <= 0:
+            raise N.SfgsError("rasterize_gaussians(graph=True) needs capacity_hint > 0 (see sfgs.graphs.capacity)")
     H, W, F = int(image_height), int(image_width), int(attr_degree)
     if subpixel_offset is not None:
         check_subpixel_offset(subpixel_offset, H, W)
@@ -140,7 +177,11 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
         a.viewmatrix = _ptr(viewmatrix, keep)
         a.projmatrix = _ptr(projmatrix, keep)
         a.cam_pos = _ptr(campos, keep)
-        a.tan_fovx, a.tan_fovy, a.kernel_size = float(tan_fovx), float(tan_fovy), float(kernel_size)
+        if graph:
+            a.tan_fovx, a.tan_fovy, tan_fov = _tan_fov(tan_fovx, tan_fovy, dev)
+            a.kernel_size = float(kernel_size)
+        else:
+            a.tan_fovx, a.tan_fovy, a.kernel_size = float(tan_fovx), float(tan_fovy), float(kernel_size)
         a.prefiltered = int(bool(prefiltered))
         a.out_color, a.out_depth = out_color.data_ptr(), out_depth.data_ptr()
         a.out_norm, a.out_alpha = out_norm.data_ptr(), out_alpha.data_ptr()
@@ -157,7 +198,14 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
         a.capacity_hint = int(capacity_hint)
         if tile_rows is not None:
             a.tile_row_begin, a.tile_row_end = _band(tile_rows)
-        if subpixel_offset is not None:
+        if graph:
+            from . import graphs
+            off = _ptr(subpixel_offset, keep) if subpixel_offset is not None else None
+            N.check(L.sfgs_rasterize_forward_graph(C.byref(a), off, tan_fov.data_ptr() if tan_fov is not None else None,
+                                                   graphs.status_word(dev).data_ptr()),
+                    "sfgs_rasterize_forward_graph")
+            rendered = -1
+        elif subpixel_offset is not None:
             entry = "sfgs_rasterize_forward_subpixel" + ("_peers" if out_peers is not None else "")
             rendered = N.check(getattr(L, entry)(C.byref(a), _ptr(subpixel_offset, keep)), entry)
         else:
@@ -203,7 +251,7 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
                                  dL_dout_extra, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer,
                                  out_alpha, debug, tile_rows=None, norm_raw=None, phase=0, acc=None,
                                  gauss_range=None, acc_peers=None, peer_slice=0, subpixel_offset=None,
-                                 camera_grad=False, intrinsics_grad=False):
+                                 camera_grad=False, intrinsics_grad=False, graph=False):
     """Same positional signature and return tuple as the reference's `_C.rasterize_gaussians_backward`.  With
     `norm_raw` (the extra tensor a `fuse_normalize=True` forward returned) `dL_dout_norm` is taken w.r.t. the unit
     normal map and the adjoint of F.normalize is applied inside the blend-adjoint kernel.
@@ -234,9 +282,17 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     `phase=2, camera_grad=True[, intrinsics_grad=True]` (sfgs_rasterize_backward_camera_partial): the tuple ends with
     ONE float64 tensor of 35 [37] camera terms, the unrounded sums over the Gaussians of `gauss_range`.  The ranks of a
     sharded frame add these partials and round once (sfgs.multigpu.reduce_camera_gradients).  The gradient rows are
-    bit-identical to the phase-2 call without it."""
+    bit-identical to the phase-2 call without it.
+
+    `graph=True`: the capture-safe backward (sfgs_rasterize_backward_graph) of a `graph=True` forward; `R` is the
+    capacity that forward was given, and `tan_fovx` / `tan_fovy` may be 0-d CUDA tensors.  Every option of the
+    one-call backward is taken (offsets, deterministic mode, camera and focal gradients); phases 1 and 2, acc_peers,
+    tile_rows and debug raise."""
     if intrinsics_grad and not camera_grad:
         raise ValueError("intrinsics_grad=True needs camera_grad=True")
+    if graph:
+        _graph_unsupported("rasterize_gaussians_backward(graph=True)", debug, tile_rows,
+                           "acc_peers" if acc_peers is not None else None, int(phase))
     if subpixel_offset is not None:
         check_subpixel_offset(subpixel_offset, int(dL_dout_color.shape[1]), int(dL_dout_color.shape[2]))
     F = int(extra_attrs.shape[1]) if (extra_attrs is not None and extra_attrs.numel() != 0) else 0
@@ -302,7 +358,11 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
         a.viewmatrix = _ptr(viewmatrix, keep)
         a.projmatrix = _ptr(projmatrix, keep)
         a.cam_pos = _ptr(campos, keep)
-        a.tan_fovx, a.tan_fovy, a.kernel_size = float(tan_fovx), float(tan_fovy), float(kernel_size)
+        if graph:
+            a.tan_fovx, a.tan_fovy, tan_fov = _tan_fov(tan_fovx, tan_fovy, dev)
+            a.kernel_size = float(kernel_size)
+        else:
+            a.tan_fovx, a.tan_fovy, a.kernel_size = float(tan_fovx), float(tan_fovy), float(kernel_size)
         a.radii = _ptr(radii, keep)
         a.geom_buffer = _ptr(geomBuffer, keep)
         a.binning_buffer = _ptr(binningBuffer, keep)
@@ -331,7 +391,15 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
         a.stream = torch.cuda.current_stream(dev).cuda_stream
         if tile_rows is not None:
             a.tile_row_begin, a.tile_row_end = _band(tile_rows)
-        if camera_grad and phase == 2:
+        if graph:
+            ncam = (37 if intrinsics_grad else 35) if camera_grad else 0
+            dL_dcamera = torch.empty((ncam,), **fopt) if ncam else None
+            off = _ptr(subpixel_offset, keep) if subpixel_offset is not None else None
+            N.check(L.sfgs_rasterize_backward_graph(C.byref(a), off, int(deterministic),
+                                                    tan_fov.data_ptr() if tan_fov is not None else None,
+                                                    dL_dcamera.data_ptr() if ncam else None, ncam),
+                    "sfgs_rasterize_backward_graph")
+        elif camera_grad and phase == 2:
             ncam = 37 if intrinsics_grad else 35
             dL_dcamera = torch.empty((ncam,), dtype=torch.float64, device=dev)
             off = _ptr(subpixel_offset, keep) if subpixel_offset is not None else None
