@@ -121,6 +121,11 @@ int fail(int code, const char* what, cudaError_t e = cudaSuccess) {
   else snprintf(t_err, sizeof(t_err), "%s", what);
   return code;
 }
+// a rejection by an entry point's checks
+int fail_in(const char* entry, int code, const char* what) {
+  snprintf(t_err, sizeof(t_err), "%s: %s", entry, what);
+  return code;
+}
 
 #define CU(call)                                                   \
   do {                                                             \
@@ -197,59 +202,31 @@ struct PinnedHdr {
 constexpr int MAX_DEVICES = 64;
 thread_local PinnedHdr t_hdr_dev[MAX_DEVICES];
 
-int rasterize_forward(const sfgs_forward_args* a, const float* off, const float* tan_fov = nullptr,
-                      unsigned int* status = nullptr);
-int rasterize_backward(const sfgs_backward_args* a, bool deterministic, const float* off, float* dL_dcamera,
-                       double* dL_dcamera_partial, int ncam, bool graph = false, const float* tan_fov = nullptr);
+// What one rasterizer entry point asks for, beyond its sfgs_forward_args / sfgs_backward_args.  The entry's checks
+// (check_forward, check_backward) and the stages read their options from here.
+struct FwdCall {
+  const char* name;                   // the entry point without its sfgs_rasterize_ prefix: the errors name it
+  bool graph;                         // sfgs_rasterize_forward_graph: one pass at capacity_hint, no host wait
+  const float* off = nullptr;         // subpixel offsets [H,W,2], or NULL
+  bool peers_with_off = false;        // out_peers may come with offsets (the _subpixel_peers entry)
+  const float* tan_fov = nullptr;     // graph: NULL or the DEVICE [2] intrinsics
+  unsigned int* status = nullptr;     // graph: the DEVICE status word the frame's error flags are ORed into
+};
 
-// the combinations the subpixel-offset entry points reject (checked before any CUDA work): extra_attrs, which have no
-// kernels with offsets, and -- unless the entry is a _subpixel_peers one -- the fused peer exchanges, which the
-// _subpixel entries have always rejected
-int subpixel_unsupported_fwd(const sfgs_forward_args* a, bool peers_ok) {
-  if (a->ED > 0) return fail(SFGS_E_UNSUPPORTED, "forward_subpixel: extra_attrs are not supported with subpixel offsets");
-  if (!peers_ok && a->out_peers != nullptr)
-    return fail(SFGS_E_UNSUPPORTED, "forward_subpixel: out_peers are not supported by this entry; use sfgs_rasterize_forward_subpixel_peers");
-  return SFGS_OK;
-}
-int subpixel_unsupported_bwd(const sfgs_backward_args* a, bool peers_ok) {
-  if (a->ED > 0) return fail(SFGS_E_UNSUPPORTED, "backward_subpixel: extra_attrs are not supported with subpixel offsets");
-  if (!peers_ok && a->acc_peers != nullptr)
-    return fail(SFGS_E_UNSUPPORTED, "backward_subpixel: acc_peers are not supported by this entry; use sfgs_rasterize_backward_subpixel_peers");
-  return SFGS_OK;
-}
+struct BwdCall {
+  const char* name;                   // the entry point without its sfgs_rasterize_ prefix: the errors name it
+  enum Kind { EAGER, CAMERA, CAMERA_PARTIAL, GRAPH } kind;
+  const float* off = nullptr;         // subpixel offsets [H,W,2] (the forward's), or NULL
+  bool peers_with_off = false;        // acc_peers may come with offsets (the _subpixel_peers entry)
+  bool deterministic = false;
+  int ncam = 0;                       // camera terms: 0, 35 (pose) or 37 (pose and focal)
+  float* dL_dcamera = nullptr;        // CAMERA, GRAPH: the DEVICE [ncam] camera gradients
+  double* dL_dcamera_partial = nullptr;   // CAMERA_PARTIAL: the DEVICE [ncam] float64 sums of the Gaussian slice
+  const float* tan_fov = nullptr;     // GRAPH: NULL or the DEVICE [2] intrinsics the per-Gaussian adjoint reads
+};
 
-// the camera entries: ncam = 35 (pose terms) or 37 (pose and focal terms); the checks come before any CUDA work
-int backward_camera(const char* name, const sfgs_backward_args* a, const float* off, int deterministic,
-                    float* dL_dcamera, int ncam) {
-  auto reject = [name](int code, const char* what) {
-    char m[160];
-    snprintf(m, sizeof(m), "%s: %s", name, what);
-    return fail(code, m);
-  };
-  if (!a) return reject(SFGS_E_BADARG, "null args");
-  if (!dL_dcamera) return reject(SFGS_E_BADARG, "null dL_dcamera");
-  if (a->phase != 0)
-    return reject(SFGS_E_UNSUPPORTED, "camera gradients are formed by the one-call backward (phase 0) only");
-  if (a->acc_peers != nullptr)
-    return reject(SFGS_E_UNSUPPORTED, "acc_peers (the multi-GPU backward) have no camera gradients");
-  if (!a->scratch_alloc) return reject(SFGS_E_BADARG, "null scratch allocator");
-  if (off != nullptr && subpixel_unsupported_bwd(a, false)) return SFGS_E_UNSUPPORTED;
-  return rasterize_backward(a, deterministic != 0, off, dL_dcamera, nullptr, ncam);
-}
-
-// the phase-2 camera partials of a Gaussian slice (the tile-row sharded backward); the checks come before any CUDA work
-int backward_camera_partial(const sfgs_backward_args* a, const float* off, int deterministic, int ncam,
-                            double* dL_dcamera_partial) {
-  if (!a) return fail(SFGS_E_BADARG, "backward_camera_partial: null args");
-  if (!dL_dcamera_partial) return fail(SFGS_E_BADARG, "backward_camera_partial: null dL_dcamera_partial");
-  if (ncam != 35 && ncam != 37) return fail(SFGS_E_BADARG, "backward_camera_partial: ncam must be 35 or 37");
-  if (a->phase != 2)
-    return fail(SFGS_E_UNSUPPORTED, "backward_camera_partial: camera partials are formed by phase 2 only");
-  if (!a->scratch_alloc) return fail(SFGS_E_BADARG, "backward_camera_partial: null scratch allocator");
-  if (a->ED > 0)
-    return fail(SFGS_E_UNSUPPORTED, "backward_camera_partial: extra_attrs are not supported by the two-phase backward");
-  return rasterize_backward(a, deterministic != 0, off, nullptr, dL_dcamera_partial, ncam);
-}
+int rasterize_forward(const sfgs_forward_args* a, const FwdCall& c);
+int rasterize_backward(const sfgs_backward_args* a, const BwdCall& c);
 
 }  // namespace
 
@@ -287,83 +264,55 @@ int sfgs_binning_layout(char* base, long long capacity, sfgs_binning_view* out) 
   return SFGS_OK;
 }
 
-int sfgs_rasterize_forward(const sfgs_forward_args* a) { return rasterize_forward(a, nullptr); }
-int sfgs_rasterize_backward(const sfgs_backward_args* a) { return rasterize_backward(a, false, nullptr, nullptr, nullptr, 0); }
-int sfgs_rasterize_backward_deterministic(const sfgs_backward_args* a) { return rasterize_backward(a, true, nullptr, nullptr, nullptr, 0); }
+int sfgs_rasterize_forward(const sfgs_forward_args* a) { return rasterize_forward(a, {"forward", false}); }
+int sfgs_rasterize_backward(const sfgs_backward_args* a) { return rasterize_backward(a, {"backward", BwdCall::EAGER}); }
+int sfgs_rasterize_backward_deterministic(const sfgs_backward_args* a) {
+  return rasterize_backward(a, {"backward_deterministic", BwdCall::EAGER, nullptr, false, true});
+}
 
 int sfgs_rasterize_forward_subpixel(const sfgs_forward_args* a, const float* subpixel_offset) {
-  if (!a) return fail(SFGS_E_BADARG, "forward: null args");
-  if (subpixel_offset != nullptr && subpixel_unsupported_fwd(a, false)) return SFGS_E_UNSUPPORTED;
-  return rasterize_forward(a, subpixel_offset);
+  return rasterize_forward(a, {"forward_subpixel", false, subpixel_offset});
 }
 int sfgs_rasterize_forward_subpixel_peers(const sfgs_forward_args* a, const float* subpixel_offset) {
-  if (!a) return fail(SFGS_E_BADARG, "forward: null args");
-  if (subpixel_offset != nullptr && subpixel_unsupported_fwd(a, true)) return SFGS_E_UNSUPPORTED;
-  return rasterize_forward(a, subpixel_offset);
+  return rasterize_forward(a, {"forward_subpixel_peers", false, subpixel_offset, true});
 }
 int sfgs_rasterize_backward_subpixel(const sfgs_backward_args* a, const float* subpixel_offset) {
-  if (!a) return fail(SFGS_E_BADARG, "backward: null args");
-  if (subpixel_offset != nullptr && subpixel_unsupported_bwd(a, false)) return SFGS_E_UNSUPPORTED;
-  return rasterize_backward(a, false, subpixel_offset, nullptr, nullptr, 0);
+  return rasterize_backward(a, {"backward_subpixel", BwdCall::EAGER, subpixel_offset});
 }
 int sfgs_rasterize_backward_subpixel_peers(const sfgs_backward_args* a, const float* subpixel_offset) {
-  if (!a) return fail(SFGS_E_BADARG, "backward: null args");
-  if (subpixel_offset != nullptr && subpixel_unsupported_bwd(a, true)) return SFGS_E_UNSUPPORTED;
-  return rasterize_backward(a, false, subpixel_offset, nullptr, nullptr, 0);
+  return rasterize_backward(a, {"backward_subpixel_peers", BwdCall::EAGER, subpixel_offset, true});
 }
 int sfgs_rasterize_backward_deterministic_subpixel(const sfgs_backward_args* a, const float* subpixel_offset) {
-  if (!a) return fail(SFGS_E_BADARG, "backward: null args");
-  if (subpixel_offset != nullptr && subpixel_unsupported_bwd(a, false)) return SFGS_E_UNSUPPORTED;
-  return rasterize_backward(a, true, subpixel_offset, nullptr, nullptr, 0);
+  return rasterize_backward(a, {"backward_deterministic_subpixel", BwdCall::EAGER, subpixel_offset, false, true});
 }
 
 int sfgs_rasterize_backward_camera(const sfgs_backward_args* a, const float* subpixel_offset, int deterministic,
                                    float* dL_dcamera) {
-  return backward_camera("backward_camera", a, subpixel_offset, deterministic, dL_dcamera, 35);
+  return rasterize_backward(a, {"backward_camera", BwdCall::CAMERA, subpixel_offset, false, deterministic != 0, 35,
+                                dL_dcamera});
 }
 
 int sfgs_rasterize_backward_camera_intrinsics(const sfgs_backward_args* a, const float* subpixel_offset,
                                               int deterministic, float* dL_dcamera) {
-  return backward_camera("backward_camera_intrinsics", a, subpixel_offset, deterministic, dL_dcamera, 37);
+  return rasterize_backward(a, {"backward_camera_intrinsics", BwdCall::CAMERA, subpixel_offset, false,
+                                deterministic != 0, 37, dL_dcamera});
 }
 
 int sfgs_rasterize_backward_camera_partial(const sfgs_backward_args* a, const float* subpixel_offset, int deterministic,
                                            int ncam, double* dL_dcamera_partial) {
-  return backward_camera_partial(a, subpixel_offset, deterministic, ncam, dL_dcamera_partial);
+  return rasterize_backward(a, {"backward_camera_partial", BwdCall::CAMERA_PARTIAL, subpixel_offset, false,
+                                deterministic != 0, ncam, nullptr, dL_dcamera_partial});
 }
 
 int sfgs_rasterize_forward_graph(const sfgs_forward_args* a, const float* subpixel_offset, const float* tan_fov,
                                  unsigned int* status) {
-  if (!a) return fail(SFGS_E_BADARG, "forward_graph: null args");
-  if (!status) return fail(SFGS_E_BADARG, "forward_graph: null status word");
-  if (a->debug) return fail(SFGS_E_BADARG, "forward_graph: debug synchronises after every stage and cannot be captured");
-  if (a->capacity_hint <= 0)
-    return fail(SFGS_E_BADARG, "forward_graph: capacity_hint must be > 0 (the binning capacity of the captured frame)");
-  if (a->tile_row_begin != 0 || a->tile_row_end != 0)
-    return fail(SFGS_E_UNSUPPORTED, "forward_graph: tile-row bands are not supported under graph capture");
-  if (a->out_peers != nullptr) return fail(SFGS_E_UNSUPPORTED, "forward_graph: out_peers are not supported under graph capture");
-  if (subpixel_offset != nullptr && a->ED > 0)
-    return fail(SFGS_E_UNSUPPORTED, "forward_graph: extra_attrs are not supported with subpixel offsets");
-  return rasterize_forward(a, subpixel_offset, tan_fov, status);
+  return rasterize_forward(a, {"forward_graph", true, subpixel_offset, false, tan_fov, status});
 }
 
 int sfgs_rasterize_backward_graph(const sfgs_backward_args* a, const float* subpixel_offset, int deterministic,
                                   const float* tan_fov, float* dL_dcamera, int ncam) {
-  if (!a) return fail(SFGS_E_BADARG, "backward_graph: null args");
-  if (a->debug) return fail(SFGS_E_BADARG, "backward_graph: debug synchronises after every stage and cannot be captured");
-  if (a->R <= 0) return fail(SFGS_E_BADARG, "backward_graph: R must be the forward's binning capacity (> 0)");
-  if (ncam != 0 && ncam != 35 && ncam != 37) return fail(SFGS_E_BADARG, "backward_graph: ncam must be 0, 35 or 37");
-  if (ncam != 0 && !dL_dcamera) return fail(SFGS_E_BADARG, "backward_graph: null dL_dcamera");
-  if (a->phase != 0)
-    return fail(SFGS_E_UNSUPPORTED, "backward_graph: phases 1 and 2 (the two-phase backward) are not supported under graph capture");
-  if (a->acc_peers != nullptr) return fail(SFGS_E_UNSUPPORTED, "backward_graph: acc_peers are not supported under graph capture");
-  if (a->tile_row_begin != 0 || a->tile_row_end != 0)
-    return fail(SFGS_E_UNSUPPORTED, "backward_graph: tile-row bands are not supported under graph capture");
-  if (subpixel_offset != nullptr && a->ED > 0)
-    return fail(SFGS_E_UNSUPPORTED, "backward_graph: extra_attrs are not supported with subpixel offsets");
-  if (ncam != 0 && !a->scratch_alloc) return fail(SFGS_E_BADARG, "backward_graph: null scratch allocator");
-  return rasterize_backward(a, deterministic != 0, subpixel_offset, ncam != 0 ? dL_dcamera : nullptr, nullptr, ncam, true,
-                            tan_fov);
+  return rasterize_backward(a, {"backward_graph", BwdCall::GRAPH, subpixel_offset, false, deterministic != 0, ncam,
+                                ncam != 0 ? dL_dcamera : nullptr, nullptr, tan_fov});
 }
 
 long long sfgs_capacity_estimate(int device, int P, int width, int height) {
@@ -374,29 +323,57 @@ long long sfgs_capacity_estimate(int device, int P, int width, int height) {
 
 namespace {
 
-// tan_fov, status: the graph forward (sfgs_rasterize_forward_graph, checked by the caller): status != NULL queues the
-// pipeline once at capacity_hint with no host wait, and a kernel ORs the header's error flags into *status
-int rasterize_forward(const sfgs_forward_args* a, const float* off, const float* tan_fov, unsigned int* status) {
-  if (!a) return fail(SFGS_E_BADARG, "forward: null args");
-  if (a->P < 0 || a->width <= 0 || a->height <= 0) return fail(SFGS_E_BADARG, "forward: bad sizes");
-  if (a->ED < 0 || a->ED > SFGS_MAX_EXTRA) return fail(SFGS_E_BADARG, "forward: ED out of range");
-  if (a->tile_row_begin < 0 || a->tile_row_end < a->tile_row_begin) return fail(SFGS_E_BADARG, "forward: bad tile-row band");
+// Every rejection of the forward entries, in the order that decides which one an entry reports; all before any CUDA
+// work.  Messages are "<entry>: <what>".
+int check_forward(const sfgs_forward_args* a, const FwdCall& c) {
+  const auto reject = [&c](int code, const char* what) { return fail_in(c.name, code, what); };
+  if (!a) return reject(SFGS_E_BADARG, "null args");
+  if (c.graph) {
+    if (!c.status) return reject(SFGS_E_BADARG, "null status word");
+    if (a->debug) return reject(SFGS_E_BADARG, "debug synchronises after every stage and cannot be captured");
+    if (a->capacity_hint <= 0)
+      return reject(SFGS_E_BADARG, "capacity_hint must be > 0 (the binning capacity of the captured frame)");
+    if (a->tile_row_begin != 0 || a->tile_row_end != 0)
+      return reject(SFGS_E_UNSUPPORTED, "tile-row bands are not supported under graph capture");
+    if (a->out_peers != nullptr) return reject(SFGS_E_UNSUPPORTED, "out_peers are not supported under graph capture");
+  }
+  if (c.off != nullptr) {
+    // extra_attrs have no kernels with offsets; the _subpixel entry has always rejected the fused peer exchange
+    if (a->ED > 0) return reject(SFGS_E_UNSUPPORTED, "extra_attrs are not supported with subpixel offsets");
+    if (!c.peers_with_off && a->out_peers != nullptr)
+      return reject(SFGS_E_UNSUPPORTED,
+                    "out_peers are not supported by this entry; use sfgs_rasterize_forward_subpixel_peers");
+  }
+  if (a->P < 0 || a->width <= 0 || a->height <= 0) return reject(SFGS_E_BADARG, "bad sizes");
+  if (a->ED < 0 || a->ED > SFGS_MAX_EXTRA) return reject(SFGS_E_BADARG, "ED out of range");
+  if (a->tile_row_begin < 0 || a->tile_row_end < a->tile_row_begin) return reject(SFGS_E_BADARG, "bad tile-row band");
   const bool peer_out = a->out_peers != nullptr && a->n_out_peers > 0;
-  if (peer_out && a->n_out_peers > 8) return fail(SFGS_E_BADARG, "forward: at most 8 out_peers");
+  if (peer_out && a->n_out_peers > 8) return reject(SFGS_E_BADARG, "at most 8 out_peers");
   if ((!peer_out && (!a->out_color || !a->out_depth || !a->out_norm || !a->out_alpha)) || (a->P > 0 && !a->radii))
-    return fail(SFGS_E_BADARG, "forward: null output");
-  if (!a->geom_alloc || !a->binning_alloc || !a->image_alloc) return fail(SFGS_E_BADARG, "forward: null allocator");
+    return reject(SFGS_E_BADARG, "null output");
+  if (!a->geom_alloc || !a->binning_alloc || !a->image_alloc) return reject(SFGS_E_BADARG, "null allocator");
   if (a->P > 0) {
     if (!a->means3D || !a->opacities || !a->viewmatrix || !a->projmatrix || !a->cam_pos || !a->background)
-      return fail(SFGS_E_BADARG, "forward: null input");
-    if (!a->shs && !a->colors_precomp) return fail(SFGS_E_BADARG, "forward: need shs or colors_precomp");
+      return reject(SFGS_E_BADARG, "null input");
+    if (!a->shs && !a->colors_precomp) return reject(SFGS_E_BADARG, "need shs or colors_precomp");
     if (a->colors_precomp == nullptr && (a->M <= 0 || a->D < 0 || a->D > 3 || (a->D + 1) * (a->D + 1) > a->M))
-      return fail(SFGS_E_BADARG, "forward: SH degree/M mismatch");
-    if (!a->cov3D_precomp && (!a->scales || !a->rotations)) return fail(SFGS_E_BADARG, "forward: need scales+rotations or cov3D_precomp");
-    if (!a->norm3D_precomp && (!a->scales || !a->rotations)) return fail(SFGS_E_BADARG, "forward: need scales+rotations or norm3D_precomp");
-    if (a->ED > 0 && (!a->extra_attrs || !a->out_extra)) return fail(SFGS_E_BADARG, "forward: extra attrs missing");
-    if (a->rotations && (reinterpret_cast<uintptr_t>(a->rotations) & 15)) return fail(SFGS_E_BADARG, "forward: rotations must be 16-byte aligned");
+      return reject(SFGS_E_BADARG, "SH degree/M mismatch");
+    if (!a->cov3D_precomp && (!a->scales || !a->rotations))
+      return reject(SFGS_E_BADARG, "need scales+rotations or cov3D_precomp");
+    if (!a->norm3D_precomp && (!a->scales || !a->rotations))
+      return reject(SFGS_E_BADARG, "need scales+rotations or norm3D_precomp");
+    if (a->ED > 0 && (!a->extra_attrs || !a->out_extra)) return reject(SFGS_E_BADARG, "extra attrs missing");
+    if (a->rotations && (reinterpret_cast<uintptr_t>(a->rotations) & 15))
+      return reject(SFGS_E_BADARG, "rotations must be 16-byte aligned");
   }
+  return SFGS_OK;
+}
+
+// graph: the pipeline is queued once at capacity_hint with no host wait, and a kernel ORs the header's error flags
+// into *status
+int rasterize_forward(const sfgs_forward_args* a, const FwdCall& c) {
+  if (const int rc = check_forward(a, c)) return rc;
+  const float* off = c.off;
   cudaStream_t st = (cudaStream_t)a->stream;
   const bool debug = a->debug != 0;
   const int P = a->P;
@@ -431,7 +408,7 @@ int rasterize_forward(const sfgs_forward_args* a, const float* off, const float*
 
     if (P > 0) {
       PROF_BEGIN(ST_PREPROCESS);
-      sfgs_launch_preprocess(a, g, im, b, (unsigned long long)capacity, focal_x, focal_y, tan_fov, st);
+      sfgs_launch_preprocess(a, g, im, b, (unsigned long long)capacity, focal_x, focal_y, c.tan_fov, st);
       PROF_END();
       STAGE_CHECK("preprocess");
     }
@@ -458,11 +435,11 @@ int rasterize_forward(const sfgs_forward_args* a, const float* off, const float*
     return SFGS_OK;
   };
 
-  if (status != nullptr) {
+  if (c.graph) {
     // captured: one pass at the caller's capacity; the overflow flag reaches the caller through *status, and every
     // kernel after the scan returns at once on it
     return queue(a->capacity_hint, [&]() -> int {
-      sfgs_launch_forward_status(im, status, st);
+      sfgs_launch_forward_status(im, c.status, st);
       STAGE_CHECK("forward_status");
       return SFGS_OK;
     });
@@ -509,20 +486,99 @@ int rasterize_forward(const sfgs_forward_args* a, const float* off, const float*
   return (int)R;
 }
 
-// dL_dcamera: NULL, or (phase 0 only, checked by the caller) the DEVICE [ncam] camera gradients to form as well;
-// dL_dcamera_partial: NULL, or (phase 2 only, checked by the caller) the DEVICE [ncam] float64 camera sums of the
-// Gaussian slice, unrounded.  ncam = 35 (pose terms) or 37 (pose and focal terms).
-// graph (sfgs_rasterize_backward_graph, phase 0 only, checked by the caller): a->R is the forward's binning capacity and
-// only sizes scratch; the blend adjoint is always launched and it and the ordering kernels check the overflow flag
-// first.  tan_fov: NULL or the DEVICE [2] intrinsics the per-Gaussian adjoint reads.
-int rasterize_backward(const sfgs_backward_args* a, bool deterministic, const float* off, float* dL_dcamera,
-                       double* dL_dcamera_partial, int ncam, bool graph, const float* tan_fov) {
-  if (!a) return fail(SFGS_E_BADARG, "backward: null args");
-  if (a->P < 0 || a->width <= 0 || a->height <= 0) return fail(SFGS_E_BADARG, "backward: bad sizes");
-  if (deterministic && a->acc_peers != nullptr)
-    return fail(SFGS_E_UNSUPPORTED, "backward_deterministic: acc_peers (system-scope reductions) have no deterministic implementation");
-  if (deterministic && a->ED > 0)
-    return fail(SFGS_E_UNSUPPORTED, "backward_deterministic: extra_attrs have no deterministic implementation");
+// Every rejection of the backward entries, in the order that decides which one an entry reports; all before any CUDA
+// work.  Messages are "<entry>: <what>".  P == 0 passes once the checks that hold for it have run.
+int check_backward(const sfgs_backward_args* a, const BwdCall& c) {
+  const auto reject = [&c](int code, const char* what) { return fail_in(c.name, code, what); };
+  if (!a) return reject(SFGS_E_BADARG, "null args");
+  if (c.kind == BwdCall::CAMERA) {
+    if (!c.dL_dcamera) return reject(SFGS_E_BADARG, "null dL_dcamera");
+    if (a->phase != 0)
+      return reject(SFGS_E_UNSUPPORTED, "camera gradients are formed by the one-call backward (phase 0) only");
+    if (a->acc_peers != nullptr)
+      return reject(SFGS_E_UNSUPPORTED, "acc_peers (the multi-GPU backward) have no camera gradients");
+    if (!a->scratch_alloc) return reject(SFGS_E_BADARG, "null scratch allocator");
+  } else if (c.kind == BwdCall::CAMERA_PARTIAL) {
+    if (!c.dL_dcamera_partial) return reject(SFGS_E_BADARG, "null dL_dcamera_partial");
+    if (c.ncam != 35 && c.ncam != 37) return reject(SFGS_E_BADARG, "ncam must be 35 or 37");
+    if (a->phase != 2) return reject(SFGS_E_UNSUPPORTED, "camera partials are formed by phase 2 only");
+    if (!a->scratch_alloc) return reject(SFGS_E_BADARG, "null scratch allocator");
+    if (a->ED > 0) return reject(SFGS_E_UNSUPPORTED, "extra_attrs are not supported by the two-phase backward");
+  } else if (c.kind == BwdCall::GRAPH) {
+    if (a->debug) return reject(SFGS_E_BADARG, "debug synchronises after every stage and cannot be captured");
+    if (a->R <= 0) return reject(SFGS_E_BADARG, "R must be the forward's binning capacity (> 0)");
+    if (c.ncam != 0 && c.ncam != 35 && c.ncam != 37) return reject(SFGS_E_BADARG, "ncam must be 0, 35 or 37");
+    if (c.ncam != 0 && !c.dL_dcamera) return reject(SFGS_E_BADARG, "null dL_dcamera");
+    if (a->phase != 0)
+      return reject(SFGS_E_UNSUPPORTED,
+                    "phases 1 and 2 (the two-phase backward) are not supported under graph capture");
+    if (a->acc_peers != nullptr) return reject(SFGS_E_UNSUPPORTED, "acc_peers are not supported under graph capture");
+    if (a->tile_row_begin != 0 || a->tile_row_end != 0)
+      return reject(SFGS_E_UNSUPPORTED, "tile-row bands are not supported under graph capture");
+  }
+  // extra_attrs have no kernels with offsets; the _subpixel entries have always rejected the fused peer exchange (the
+  // partial entry rejects extra_attrs above, and acc_peers by their phase below)
+  if (c.off != nullptr && c.kind != BwdCall::CAMERA_PARTIAL) {
+    if (a->ED > 0) return reject(SFGS_E_UNSUPPORTED, "extra_attrs are not supported with subpixel offsets");
+    if (!c.peers_with_off && a->acc_peers != nullptr)
+      return reject(SFGS_E_UNSUPPORTED,
+                    "acc_peers are not supported by this entry; use sfgs_rasterize_backward_subpixel_peers");
+  }
+  if (c.kind == BwdCall::GRAPH && c.ncam != 0 && !a->scratch_alloc)
+    return reject(SFGS_E_BADARG, "null scratch allocator");
+  if (a->P < 0 || a->width <= 0 || a->height <= 0) return reject(SFGS_E_BADARG, "bad sizes");
+  if (c.deterministic && a->acc_peers != nullptr)
+    return reject(SFGS_E_UNSUPPORTED, "acc_peers (system-scope reductions) have no deterministic implementation");
+  if (c.deterministic && a->ED > 0)
+    return reject(SFGS_E_UNSUPPORTED, "extra_attrs have no deterministic implementation");
+  if (a->P == 0) return SFGS_OK;
+  const int phase = a->phase;
+  if (phase < 0 || phase > 2) return reject(SFGS_E_BADARG, "phase must be 0, 1 or 2");
+  const bool do_blend = phase != 2, do_gauss = phase != 1;
+  if (!a->geom_buffer || !a->binning_buffer || !a->image_buffer) return reject(SFGS_E_BADARG, "null scratch buffer");
+  if (do_blend && (!a->dL_dpix || !a->dL_dpix_depth || !a->dL_dpix_norm || !a->dL_dpix_alpha || !a->accum_alphas))
+    return reject(SFGS_E_BADARG, "null pixel gradient");
+  if (do_gauss && (!a->dL_dmean2D || !a->dL_dconic || !a->dL_dopacity || !a->dL_dcolor || !a->dL_ddepth ||
+                   !a->dL_dmean3D || !a->dL_dcov3D || !a->dL_dnorm3D || !a->dL_dscale || !a->dL_drot))
+    return reject(SFGS_E_BADARG, "null output");
+  if (do_gauss && !a->radii) return reject(SFGS_E_BADARG, "radii missing");
+  if (do_gauss && a->M > 0 && a->shs && !a->dL_dsh) return reject(SFGS_E_BADARG, "dL_dsh missing");
+  if (a->ED < 0 || a->ED > SFGS_MAX_EXTRA) return reject(SFGS_E_BADARG, "ED out of range");
+  // extra-attribute gradients are accumulated by the blend stage only and are never exchanged between ranks: the
+  // two-phase (multi-GPU) form would return them partial or uninitialised
+  if (a->ED > 0 && phase != 0)
+    return reject(SFGS_E_UNSUPPORTED, "extra_attrs are not supported by the two-phase backward");
+  if (a->tile_row_begin < 0 || a->tile_row_end < a->tile_row_begin) return reject(SFGS_E_BADARG, "bad tile-row band");
+  if (a->ED > 0 && (!a->dL_dextra || !a->dL_dpix_extra || !a->extra_attrs))
+    return reject(SFGS_E_BADARG, "extra attrs missing");
+  const bool peer = a->acc_peers != nullptr;
+  if (peer && (phase != 1 || a->n_peers < 1 || a->n_peers > 8 || a->peer_slice < 1 ||
+               (long long)a->n_peers * a->peer_slice < a->P))
+    return reject(SFGS_E_BADARG, "acc_peers needs phase 1, 1..8 peers and n_peers*peer_slice >= P");
+  if (phase != 0 && !a->acc && !peer) return reject(SFGS_E_BADARG, "phases 1 and 2 need the caller's acc buffer");
+  if (phase == 0 && !a->acc && !a->scratch_alloc) return reject(SFGS_E_BADARG, "null scratch allocator");
+  if (a->acc && (reinterpret_cast<uintptr_t>(a->acc) & 15)) return reject(SFGS_E_BADARG, "acc must be 16-byte aligned");
+  if (a->rotations && (reinterpret_cast<uintptr_t>(a->rotations) & 15))
+    return reject(SFGS_E_BADARG, "rotations must be 16-byte aligned");
+  // the ordered blend adjoint places each partial by the Gaussian's tile rectangle (radii) in scratch_alloc's memory
+  const bool ordered = c.deterministic && do_blend;
+  if (ordered && !a->radii) return reject(SFGS_E_BADARG, "radii missing");
+  if (ordered && !a->scratch_alloc) return reject(SFGS_E_BADARG, "null scratch allocator");
+  if (phase == 2 && (a->gauss_begin < 0 || a->gauss_end > a->P || a->gauss_begin > a->gauss_end))
+    return reject(SFGS_E_BADARG, "bad Gaussian range");
+  return SFGS_OK;
+}
+
+// CAMERA, GRAPH with ncam > 0: the [ncam] camera gradients are formed as well; CAMERA_PARTIAL: phase 2 leaves the
+// slice's [ncam] float64 camera sums unrounded.  GRAPH: a->R is the forward's binning capacity and only sizes scratch;
+// the blend adjoint is always launched and it and the ordering kernels check the overflow flag first.
+int rasterize_backward(const sfgs_backward_args* a, const BwdCall& c) {
+  if (const int rc = check_backward(a, c)) return rc;
+  const bool graph = c.kind == BwdCall::GRAPH;
+  float* const dL_dcamera = c.dL_dcamera;
+  double* const dL_dcamera_partial = c.dL_dcamera_partial;
+  const int ncam = c.ncam;
+  const float* const off = c.off;
   const bool cam = dL_dcamera != nullptr || dL_dcamera_partial != nullptr;
   if (a->P == 0) {
     if (dL_dcamera) CU(cudaMemsetAsync(dL_dcamera, 0, (size_t)ncam * sizeof(float), (cudaStream_t)a->stream));
@@ -531,42 +587,13 @@ int rasterize_backward(const sfgs_backward_args* a, bool deterministic, const fl
     return SFGS_OK;
   }
   const int phase = a->phase;
-  if (phase < 0 || phase > 2) return fail(SFGS_E_BADARG, "backward: phase must be 0, 1 or 2");
   const bool do_blend = phase != 2, do_gauss = phase != 1;
-  if (!a->geom_buffer || !a->binning_buffer || !a->image_buffer) return fail(SFGS_E_BADARG, "backward: null scratch buffer");
-  if (do_blend && (!a->dL_dpix || !a->dL_dpix_depth || !a->dL_dpix_norm || !a->dL_dpix_alpha || !a->accum_alphas))
-    return fail(SFGS_E_BADARG, "backward: null pixel gradient");
-  if (do_gauss && (!a->dL_dmean2D || !a->dL_dconic || !a->dL_dopacity || !a->dL_dcolor || !a->dL_ddepth || !a->dL_dmean3D ||
-                   !a->dL_dcov3D || !a->dL_dnorm3D || !a->dL_dscale || !a->dL_drot))
-    return fail(SFGS_E_BADARG, "backward: null output");
-  if (do_gauss && !a->radii) return fail(SFGS_E_BADARG, "backward: radii missing");
-  if (do_gauss && a->M > 0 && a->shs && !a->dL_dsh) return fail(SFGS_E_BADARG, "backward: dL_dsh missing");
-  if (a->ED < 0 || a->ED > SFGS_MAX_EXTRA) return fail(SFGS_E_BADARG, "backward: ED out of range");
-  // extra-attribute gradients are accumulated by the blend stage only and are never exchanged between ranks: the
-  // two-phase (multi-GPU) form would return them partial or uninitialised
-  if (a->ED > 0 && phase != 0) return fail(SFGS_E_UNSUPPORTED, "backward: extra_attrs are not supported by the two-phase backward");
-  if (a->tile_row_begin < 0 || a->tile_row_end < a->tile_row_begin) return fail(SFGS_E_BADARG, "backward: bad tile-row band");
-  if (a->ED > 0 && (!a->dL_dextra || !a->dL_dpix_extra || !a->extra_attrs)) return fail(SFGS_E_BADARG, "backward: extra attrs missing");
   const bool peer = a->acc_peers != nullptr;
-  if (peer && (phase != 1 || a->n_peers < 1 || a->n_peers > 8 || a->peer_slice < 1 ||
-               (long long)a->n_peers * a->peer_slice < a->P))
-    return fail(SFGS_E_BADARG, "backward: acc_peers needs phase 1, 1..8 peers and n_peers*peer_slice >= P");
-  if (phase != 0 && !a->acc && !peer) return fail(SFGS_E_BADARG, "backward: phases 1 and 2 need the caller's acc buffer");
-  if (phase == 0 && !a->acc && !a->scratch_alloc) return fail(SFGS_E_BADARG, "backward: null scratch allocator");
-  if (a->acc && (reinterpret_cast<uintptr_t>(a->acc) & 15)) return fail(SFGS_E_BADARG, "backward: acc must be 16-byte aligned");
-  if (a->rotations && (reinterpret_cast<uintptr_t>(a->rotations) & 15)) return fail(SFGS_E_BADARG, "backward: rotations must be 16-byte aligned");
-  // the ordered blend adjoint places each partial by the Gaussian's tile rectangle (radii) in scratch_alloc's memory
-  const bool ordered = deterministic && do_blend;
-  if (ordered && !a->radii) return fail(SFGS_E_BADARG, "backward_deterministic: radii missing");
-  if (ordered && !a->scratch_alloc) return fail(SFGS_E_BADARG, "backward_deterministic: null scratch allocator");
+  const bool ordered = c.deterministic && do_blend;
   cudaStream_t st = (cudaStream_t)a->stream;
   const bool debug = a->debug != 0;
   const int P = a->P;
-  int g_begin = 0, g_end = P;
-  if (phase == 2) {
-    g_begin = a->gauss_begin; g_end = a->gauss_end;
-    if (g_begin < 0 || g_end > P || g_begin > g_end) return fail(SFGS_E_BADARG, "backward: bad Gaussian range");
-  }
+  const int g_begin = phase == 2 ? a->gauss_begin : 0, g_end = phase == 2 ? a->gauss_end : P;
 
   GeomLayout g(sfgs_align_ptr(a->geom_buffer), (size_t)P);
   ImageLayout im(sfgs_align_ptr(a->image_buffer), a->width, a->height);
@@ -630,8 +657,8 @@ int rasterize_backward(const sfgs_backward_args* a, bool deterministic, const fl
   }
   if (do_gauss) {
     PROF_BEGIN(ST_GAUSS_BWD);
-    sfgs_launch_gauss_bwd(a, g, focal_x, focal_y, acc, g_begin, g_end, phase == 2 ? g_begin : 0, cam_part, ncam, tan_fov,
-                          st);
+    sfgs_launch_gauss_bwd(a, g, focal_x, focal_y, acc, g_begin, g_end, phase == 2 ? g_begin : 0, cam_part, ncam,
+                          c.tan_fov, st);
     if (dL_dcamera) sfgs_launch_camera_reduce(P, ncam, cam_part, dL_dcamera, st);
     // an empty slice has no spans: the reduction writes zeros
     if (dL_dcamera_partial) sfgs_launch_camera_partial_reduce(g_end - g_begin, ncam, cam_part, dL_dcamera_partial, st);

@@ -500,21 +500,30 @@ static_assert(sizeof(float) * (GB_CAM_STAGE + GB_CAM * GB_SLOTS) <= sizeof(GbInp
 
 // The per-Gaussian adjoint over spans [g_begin, g_end).  NCAM > 0: also the first NCAM camera terms; span s (counted
 // from g_begin) writes cam_part[j * nspans + s], the float64 sum of its rasterized Gaussians' camera term j in index
-// order.
-template <int NCAM>
-__device__ __forceinline__ void
-gauss_bwd_body(int g_begin, int g_end, int spans_per_cta, int acc_row0, int D, int M,
-               const float* __restrict__ means3D, const int* __restrict__ radii, const float* __restrict__ shs,
-               const unsigned char* __restrict__ clamped, const float* __restrict__ scales,
-               const float* __restrict__ rotations, float scale_modifier, const float* __restrict__ cov3Ds,
-               const float* __restrict__ rec, const float* __restrict__ norm3D_precomp,
-               const float* __restrict__ view, const float* __restrict__ proj, float h_x, float h_y,
-               float tan_fovx, float tan_fovy, float kernel_size, const float* __restrict__ campos,
-               const float* __restrict__ acc, float* __restrict__ dL_dmean2D, float* __restrict__ dL_dconic,
-               float* __restrict__ dL_dopacity, float* __restrict__ dL_dcolor, float* __restrict__ dL_ddepth,
-               float* __restrict__ dL_dmean3D, float* __restrict__ dL_dcov3D, float* __restrict__ dL_dnorm3D,
-               float* __restrict__ dL_dsh, float* __restrict__ dL_dscale, float* __restrict__ dL_drot,
-               double* __restrict__ cam_part) {
+// order.  DEV_FOV: device-resident intrinsics (the graph backward, sfgs_rasterize_backward_graph): tan_fov [2] is read
+// from device memory and the focal lengths are formed from it as the host forms them (W / (2 tan_fovx),
+// H / (2 tan_fovy)), as in preprocess_kernel<DEV_FOV>.  A trailing parameter an instantiation does not read costs
+// nothing, and new parameters go at the end of the list.
+template <int NCAM, bool DEV_FOV>
+__global__ void __launch_bounds__(GB_THREADS, GB_CTAS_PER_SM)
+gauss_bwd_kernel(int g_begin, int g_end, int spans_per_cta, int acc_row0, int D, int M,
+                 const float* __restrict__ means3D, const int* __restrict__ radii, const float* __restrict__ shs,
+                 const unsigned char* __restrict__ clamped, const float* __restrict__ scales,
+                 const float* __restrict__ rotations, float scale_modifier, const float* __restrict__ cov3Ds,
+                 const float* __restrict__ rec, const float* __restrict__ norm3D_precomp,
+                 const float* __restrict__ view, const float* __restrict__ proj, float h_x, float h_y,
+                 float tan_fovx, float tan_fovy, float kernel_size, const float* __restrict__ campos,
+                 const float* __restrict__ acc, float* __restrict__ dL_dmean2D, float* __restrict__ dL_dconic,
+                 float* __restrict__ dL_dopacity, float* __restrict__ dL_dcolor, float* __restrict__ dL_ddepth,
+                 float* __restrict__ dL_dmean3D, float* __restrict__ dL_dcov3D, float* __restrict__ dL_dnorm3D,
+                 float* __restrict__ dL_dsh, float* __restrict__ dL_dscale, float* __restrict__ dL_drot,
+                 double* __restrict__ cam_part, const float* __restrict__ tan_fov, int W, int H) {
+  if constexpr (DEV_FOV) {
+    tan_fovx = tan_fov[0];
+    tan_fovy = tan_fov[1];
+    h_y = H / (2.0f * tan_fovy);
+    h_x = W / (2.0f * tan_fovx);
+  }
   extern __shared__ __align__(16) unsigned char gb_smem[];
   GbShared& S = *reinterpret_cast<GbShared*>(gb_smem);
   const int t = threadIdx.x, lane = t & 31, wid = t >> 5;
@@ -706,53 +715,6 @@ gauss_bwd_body(int g_begin, int g_end, int spans_per_cta, int acc_row0, int D, i
   }
 }
 
-#define GB_PARAMS                                                                                                    \
-  int g_begin, int g_end, int spans_per_cta, int acc_row0, int D, int M, const float* __restrict__ means3D,         \
-      const int* __restrict__ radii, const float* __restrict__ shs, const unsigned char* __restrict__ clamped,      \
-      const float* __restrict__ scales, const float* __restrict__ rotations, float scale_modifier,                  \
-      const float* __restrict__ cov3Ds, const float* __restrict__ rec, const float* __restrict__ norm3D_precomp,    \
-      const float* __restrict__ view, const float* __restrict__ proj, float h_x, float h_y, float tan_fovx,         \
-      float tan_fovy, float kernel_size, const float* __restrict__ campos, const float* __restrict__ acc,           \
-      float* __restrict__ dL_dmean2D, float* __restrict__ dL_dconic, float* __restrict__ dL_dopacity,               \
-      float* __restrict__ dL_dcolor, float* __restrict__ dL_ddepth, float* __restrict__ dL_dmean3D,                 \
-      float* __restrict__ dL_dcov3D, float* __restrict__ dL_dnorm3D, float* __restrict__ dL_dsh,                    \
-      float* __restrict__ dL_dscale, float* __restrict__ dL_drot
-#define GB_ARGS                                                                                                      \
-  g_begin, g_end, spans_per_cta, acc_row0, D, M, means3D, radii, shs, clamped, scales, rotations, scale_modifier,   \
-      cov3Ds, rec, norm3D_precomp, view, proj, h_x, h_y, tan_fovx, tan_fovy, kernel_size, campos, acc, dL_dmean2D,  \
-      dL_dconic, dL_dopacity, dL_dcolor, dL_ddepth, dL_dmean3D, dL_dcov3D, dL_dnorm3D, dL_dsh, dL_dscale, dL_drot
-
-__global__ void __launch_bounds__(GB_THREADS, GB_CTAS_PER_SM) gauss_bwd_kernel(GB_PARAMS) {
-  gauss_bwd_body<0>(GB_ARGS, nullptr);
-}
-
-__global__ void __launch_bounds__(GB_THREADS, GB_CTAS_PER_SM)
-gauss_bwd_camera_kernel(GB_PARAMS, double* __restrict__ cam_part) {
-  gauss_bwd_body<GB_CAM_POSE>(GB_ARGS, cam_part);
-}
-
-// the pose terms and the focal terms: a kernel of its own, so that the pose-only camera backward keeps its code
-__global__ void __launch_bounds__(GB_THREADS, GB_CTAS_PER_SM)
-gauss_bwd_intrinsics_kernel(GB_PARAMS, double* __restrict__ cam_part) {
-  gauss_bwd_body<GB_CAM>(GB_ARGS, cam_part);
-}
-
-// Device-resident intrinsics (the graph backward, sfgs_rasterize_backward_graph): tan_fov [2] is read from device
-// memory and the focal lengths are formed from it as the host forms them (W / (2 tan_fovx), H / (2 tan_fovy)); then the
-// body of gauss_bwd_kernel (NCAM = 0), gauss_bwd_camera_kernel (35) or gauss_bwd_intrinsics_kernel (37) runs as is.
-template <int NCAM>
-__global__ void __launch_bounds__(GB_THREADS, GB_CTAS_PER_SM)
-gauss_bwd_devfov_kernel(GB_PARAMS, double* __restrict__ cam_part, const float* __restrict__ tan_fov, int W, int H) {
-  tan_fovx = tan_fov[0];
-  tan_fovy = tan_fov[1];
-  h_y = H / (2.0f * tan_fovy);
-  h_x = W / (2.0f * tan_fovx);
-  gauss_bwd_body<NCAM>(GB_ARGS, NCAM > 0 ? cam_part : nullptr);
-}
-
-#undef GB_PARAMS
-#undef GB_ARGS
-
 // dL_dcamera[j] = the sum of the spans' partials of term j, rounded to float once.  The order depends on nspans only:
 // thread i adds spans i, i + CR_THREADS, ... in turn, then a fixed tree adds the threads' sums.
 constexpr int CR_THREADS = 256;
@@ -828,20 +790,20 @@ void sfgs_launch_camera_partial_reduce(int n, int ncam, const double* cam_part, 
 // cam_part: NULL for the adjoint alone; else [ncam][spans] doubles (sfgs_camera_scratch_bytes) that receive every
 // span's camera partials, ncam = 35 (pose terms) or 37 (pose and focal terms)
 // tan_fov: NULL (the launch parameters a->tan_fovx / a->tan_fovy, focal_x, focal_y are used) or DEVICE float [2], read
-// by the kernel (gauss_bwd_devfov_kernel)
+// by the kernel (DEV_FOV)
 void sfgs_launch_gauss_bwd(const sfgs_backward_args* a, const GeomLayout& g, float focal_x, float focal_y,
                            const float* acc, int g_begin, int g_end, int acc_row0, double* cam_part, int ncam,
                            const float* tan_fov, cudaStream_t st) {
   if (g_end <= g_begin) return;
-  static SfgsPerDeviceOnce attr_once;
-  if (attr_once.first_use()) {
-    cudaFuncSetAttribute(gauss_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GbShared));
-    cudaFuncSetAttribute(gauss_bwd_camera_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GbShared));
-    cudaFuncSetAttribute(gauss_bwd_intrinsics_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GbShared));
-    cudaFuncSetAttribute(gauss_bwd_devfov_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GbShared));
-    cudaFuncSetAttribute(gauss_bwd_devfov_kernel<GB_CAM_POSE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GbShared));
-    cudaFuncSetAttribute(gauss_bwd_devfov_kernel<GB_CAM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GbShared));
-  }
+  const bool dev_fov = tan_fov != nullptr;
+  const size_t smem = sizeof(GbShared);
+  const auto kernel =
+      cam_part == nullptr ? (dev_fov ? sfgs_smem_kernel<gauss_bwd_kernel<0, true>>(smem)
+                                     : sfgs_smem_kernel<gauss_bwd_kernel<0, false>>(smem))
+      : ncam == GB_CAM    ? (dev_fov ? sfgs_smem_kernel<gauss_bwd_kernel<GB_CAM, true>>(smem)
+                                     : sfgs_smem_kernel<gauss_bwd_kernel<GB_CAM, false>>(smem))
+                          : (dev_fov ? sfgs_smem_kernel<gauss_bwd_kernel<GB_CAM_POSE, true>>(smem)
+                                     : sfgs_smem_kernel<gauss_bwd_kernel<GB_CAM_POSE, false>>(smem));
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   { int v = 0; if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && v > 0) sms = v; }
@@ -853,22 +815,10 @@ void sfgs_launch_gauss_bwd(const sfgs_backward_args* a, const GeomLayout& g, flo
   const float* cov3D_ptr = a->cov3D_precomp != nullptr ? a->cov3D_precomp : g.cov3D;
   float* dL_dsh = a->M > 0 ? a->dL_dsh : nullptr;
   SFGS_COUNT_LAUNCH();
-#define GB_LAUNCH_ARGS                                                                                               \
-  g_begin, g_end, spans_per_cta, acc_row0, a->D, a->M, a->means3D, a->radii, a->shs, g.clamped, a->scales,          \
-      a->rotations, a->scale_modifier, cov3D_ptr, g.rec, a->norm3D_precomp, a->viewmatrix, a->projmatrix, focal_x,  \
-      focal_y, a->tan_fovx, a->tan_fovy, a->kernel_size, a->cam_pos, acc, a->dL_dmean2D, a->dL_dconic,              \
-      a->dL_dopacity, a->dL_dcolor, a->dL_ddepth, a->dL_dmean3D, a->dL_dcov3D, a->dL_dnorm3D, dL_dsh, a->dL_dscale, \
-      a->dL_drot
-  if (tan_fov != nullptr) {
-    const auto kernel = cam_part == nullptr ? gauss_bwd_devfov_kernel<0>
-                        : ncam == GB_CAM    ? gauss_bwd_devfov_kernel<GB_CAM>
-                                            : gauss_bwd_devfov_kernel<GB_CAM_POSE>;
-    kernel<<<blocks, GB_THREADS, sizeof(GbShared), st>>>(GB_LAUNCH_ARGS, cam_part, tan_fov, a->width, a->height);
-  } else if (cam_part != nullptr && ncam == GB_CAM)
-    gauss_bwd_intrinsics_kernel<<<blocks, GB_THREADS, sizeof(GbShared), st>>>(GB_LAUNCH_ARGS, cam_part);
-  else if (cam_part != nullptr)
-    gauss_bwd_camera_kernel<<<blocks, GB_THREADS, sizeof(GbShared), st>>>(GB_LAUNCH_ARGS, cam_part);
-  else
-    gauss_bwd_kernel<<<blocks, GB_THREADS, sizeof(GbShared), st>>>(GB_LAUNCH_ARGS);
-#undef GB_LAUNCH_ARGS
+  kernel<<<blocks, GB_THREADS, smem, st>>>(
+      g_begin, g_end, spans_per_cta, acc_row0, a->D, a->M, a->means3D, a->radii, a->shs, g.clamped, a->scales,
+      a->rotations, a->scale_modifier, cov3D_ptr, g.rec, a->norm3D_precomp, a->viewmatrix, a->projmatrix, focal_x,
+      focal_y, a->tan_fovx, a->tan_fovy, a->kernel_size, a->cam_pos, acc, a->dL_dmean2D, a->dL_dconic, a->dL_dopacity,
+      a->dL_dcolor, a->dL_ddepth, a->dL_dmean3D, a->dL_dcov3D, a->dL_dnorm3D, dL_dsh, a->dL_dscale, a->dL_drot,
+      cam_part, tan_fov, a->width, a->height);
 }

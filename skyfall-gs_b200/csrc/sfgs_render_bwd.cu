@@ -368,165 +368,71 @@ render_bwd_warp(const uint2* __restrict__ ranges, const char* __restrict__ binni
   });
 }
 
-template <bool PEER, bool HAS_EXTRA, bool ORDERED = false>
+// The one blend adjoint.  Each option is a template argument; a trailing parameter an instantiation does not read costs
+// nothing, and new parameters go at the end of the list.  GUARDED (the graph backward, sfgs_rasterize_backward_graph):
+// launched whatever the frame's instance count, so it first checks the forward's overflow flag -- after an overflow the
+// ranges run past the binning capacity and nothing may read point_list or write partial rows.
+template <bool PEER, bool HAS_EXTRA, bool ORDERED, bool JITTER, bool GUARDED>
 __global__ void __launch_bounds__(BLEND_THREADS, 3)
-render_bwd_warp_kernel(const uint2* __restrict__ ranges, const char* __restrict__ binning_base,
-                       const uint32_t* __restrict__ hdr, int W, int H, int band0,
-                       const float* __restrict__ bg_color, const float* __restrict__ rec,
-                       const float* __restrict__ accum_alphas, const uint32_t* __restrict__ n_contrib,
-                       const float* __restrict__ dL_dpixels, const float* __restrict__ dL_dpixel_depths,
-                       const float* __restrict__ dL_dpixel_norms, const float* __restrict__ dL_dpixel_alphas,
-                       const float* __restrict__ norm_raw, float* __restrict__ acc /* [P,16] zero-initialised */,
-                       const PeerTable peers, const float* __restrict__ extras,
-                       const float* __restrict__ dL_dpixel_extras, float* __restrict__ dL_dextras, int ED,
-                       float* __restrict__ part, unsigned char* __restrict__ written) {
-  render_bwd_warp<PEER, HAS_EXTRA, ORDERED, false>(ranges, binning_base, hdr, W, H, band0, bg_color, rec, accum_alphas,
-                                                   n_contrib, dL_dpixels, dL_dpixel_depths, dL_dpixel_norms,
-                                                   dL_dpixel_alphas, norm_raw, acc, peers, extras, dL_dpixel_extras,
-                                                   dL_dextras, ED, part, written, nullptr);
+render_bwd_kernel(const uint2* __restrict__ ranges, const char* __restrict__ binning_base,
+                  const uint32_t* __restrict__ hdr, int W, int H, int band0,
+                  const float* __restrict__ bg_color, const float* __restrict__ rec,
+                  const float* __restrict__ accum_alphas, const uint32_t* __restrict__ n_contrib,
+                  const float* __restrict__ dL_dpixels, const float* __restrict__ dL_dpixel_depths,
+                  const float* __restrict__ dL_dpixel_norms, const float* __restrict__ dL_dpixel_alphas,
+                  const float* __restrict__ norm_raw, float* __restrict__ acc /* [P,16] zero-initialised */,
+                  const PeerTable peers, const float* __restrict__ extras,
+                  const float* __restrict__ dL_dpixel_extras, float* __restrict__ dL_dextras, int ED,
+                  float* __restrict__ part, unsigned char* __restrict__ written, const float2* __restrict__ off) {
+  if (GUARDED && hdr[HDR_OVERFLOW]) return;
+  render_bwd_warp<PEER, HAS_EXTRA, ORDERED, JITTER>(ranges, binning_base, hdr, W, H, band0, bg_color, rec, accum_alphas,
+                                                    n_contrib, dL_dpixels, dL_dpixel_depths, dL_dpixel_norms,
+                                                    dL_dpixel_alphas, norm_raw, acc, peers, extras, dL_dpixel_extras,
+                                                    dL_dextras, ED, part, written, off);
 }
 
-// subpixel offsets: device-scope reductions (ORDERED = false) or the deterministic partial rows; no extra_attrs (the
-// _subpixel entry points reject them)
-template <bool ORDERED>
-__global__ void __launch_bounds__(BLEND_THREADS, 3)
-render_bwd_jitter_kernel(const uint2* __restrict__ ranges, const char* __restrict__ binning_base,
-                         const uint32_t* __restrict__ hdr, int W, int H, int band0,
-                         const float* __restrict__ bg_color, const float* __restrict__ rec,
-                         const float* __restrict__ accum_alphas, const uint32_t* __restrict__ n_contrib,
-                         const float* __restrict__ dL_dpixels, const float* __restrict__ dL_dpixel_depths,
-                         const float* __restrict__ dL_dpixel_norms, const float* __restrict__ dL_dpixel_alphas,
-                         const float* __restrict__ norm_raw, float* __restrict__ acc, float* __restrict__ part,
-                         unsigned char* __restrict__ written, const float2* __restrict__ off) {
-  render_bwd_warp<false, false, ORDERED, true>(ranges, binning_base, hdr, W, H, band0, bg_color, rec, accum_alphas,
-                                               n_contrib, dL_dpixels, dL_dpixel_depths, dL_dpixel_norms,
-                                               dL_dpixel_alphas, norm_raw, acc, PeerTable{}, nullptr, nullptr, nullptr,
-                                               0, part, written, off);
-}
-
-// subpixel offsets with the reduce-scatter of the tile-row sharded mode fused in: system-scope reductions into the
-// peers' accumulator slices (a kernel of its own, so that the kernels above keep their code)
-__global__ void __launch_bounds__(BLEND_THREADS, 3)
-render_bwd_jitter_peer_kernel(const uint2* __restrict__ ranges, const char* __restrict__ binning_base,
-                              const uint32_t* __restrict__ hdr, int W, int H, int band0,
-                              const float* __restrict__ bg_color, const float* __restrict__ rec,
-                              const float* __restrict__ accum_alphas, const uint32_t* __restrict__ n_contrib,
-                              const float* __restrict__ dL_dpixels, const float* __restrict__ dL_dpixel_depths,
-                              const float* __restrict__ dL_dpixel_norms, const float* __restrict__ dL_dpixel_alphas,
-                              const float* __restrict__ norm_raw, const PeerTable peers,
-                              const float2* __restrict__ off) {
-  render_bwd_warp<true, false, false, true>(ranges, binning_base, hdr, W, H, band0, bg_color, rec, accum_alphas,
-                                            n_contrib, dL_dpixels, dL_dpixel_depths, dL_dpixel_norms,
-                                            dL_dpixel_alphas, norm_raw, nullptr, peers, nullptr, nullptr, nullptr, 0,
-                                            nullptr, nullptr, off);
-}
-
-// The graph backward's blend adjoint (sfgs_rasterize_backward_graph): launched whatever the frame's instance count,
-// so it first checks the forward's overflow flag -- after an overflow the ranges run past the binning capacity and
-// nothing may read point_list or write partial rows.  A kernel of its own, so that the kernels above keep their code.
-template <bool HAS_EXTRA, bool ORDERED, bool JITTER>
-__global__ void __launch_bounds__(BLEND_THREADS, 3)
-render_bwd_guarded_kernel(const uint2* __restrict__ ranges, const char* __restrict__ binning_base,
-                          const uint32_t* __restrict__ hdr, int W, int H, int band0,
-                          const float* __restrict__ bg_color, const float* __restrict__ rec,
-                          const float* __restrict__ accum_alphas, const uint32_t* __restrict__ n_contrib,
-                          const float* __restrict__ dL_dpixels, const float* __restrict__ dL_dpixel_depths,
-                          const float* __restrict__ dL_dpixel_norms, const float* __restrict__ dL_dpixel_alphas,
-                          const float* __restrict__ norm_raw, float* __restrict__ acc,
-                          const float* __restrict__ extras, const float* __restrict__ dL_dpixel_extras,
-                          float* __restrict__ dL_dextras, int ED, float* __restrict__ part,
-                          unsigned char* __restrict__ written, const float2* __restrict__ off) {
-  if (hdr[HDR_OVERFLOW]) return;
-  render_bwd_warp<false, HAS_EXTRA, ORDERED, JITTER>(ranges, binning_base, hdr, W, H, band0, bg_color, rec,
-                                                     accum_alphas, n_contrib, dL_dpixels, dL_dpixel_depths,
-                                                     dL_dpixel_norms, dL_dpixel_alphas, norm_raw, acc, PeerTable{},
-                                                     extras, dL_dpixel_extras, dL_dextras, ED, part, written, off);
+template <bool PEER, bool HAS_EXTRA, bool ORDERED, bool JITTER, bool GUARDED>
+auto render_bwd_instance() {
+  return sfgs_smem_kernel<render_bwd_kernel<PEER, HAS_EXTRA, ORDERED, JITTER, GUARDED>>(
+      BLEND_WARPS * (JITTER ? sizeof(WarpSmemJitter) : sizeof(WarpSmem)));
 }
 
 }  // namespace
 
-// the graph backward's blend adjoint: no peers (sfgs_rasterize_backward_graph rejects acc_peers); extra_attrs only
-// without offsets and without the ordered form, as for the eager entries
-static void launch_render_bwd_guarded(const sfgs_backward_args* a, const GeomLayout& g, const ImageLayout& im,
-                                      const BinningLayout& b, float* acc, float* part, unsigned char* written,
-                                      const float* off, dim3 grid, int band0, cudaStream_t st) {
-  const size_t smem = sizeof(WarpSmem) * BLEND_WARPS, smem_j = sizeof(WarpSmemJitter) * BLEND_WARPS;
-  static SfgsPerDeviceOnce attr_once;
-  if (attr_once.first_use()) {
-    cudaFuncSetAttribute(render_bwd_guarded_kernel<false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaFuncSetAttribute(render_bwd_guarded_kernel<true, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaFuncSetAttribute(render_bwd_guarded_kernel<false, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaFuncSetAttribute(render_bwd_guarded_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_j);
-    cudaFuncSetAttribute(render_bwd_guarded_kernel<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_j);
-  }
-  const bool ordered = part != nullptr;
-  const auto kernel = off != nullptr ? (ordered ? render_bwd_guarded_kernel<false, true, true>
-                                                : render_bwd_guarded_kernel<false, false, true>)
-                      : ordered      ? render_bwd_guarded_kernel<false, true, false>
-                      : a->ED > 0    ? render_bwd_guarded_kernel<true, false, false>
-                                     : render_bwd_guarded_kernel<false, false, false>;
-  SFGS_COUNT_LAUNCH();
-  kernel<<<grid, BLEND_THREADS, off != nullptr ? smem_j : smem, st>>>(
-      im.ranges, (const char*)b.point_list, im.hdr, a->width, a->height, band0, a->background, g.rec, a->accum_alphas,
-      im.n_contrib, a->dL_dpix, a->dL_dpix_depth, a->dL_dpix_norm, a->dL_dpix_alpha, a->norm_raw, acc, a->extra_attrs,
-      a->dL_dpix_extra, a->dL_dextra, a->ED, part, written, reinterpret_cast<const float2*>(off));
-}
-
-// guarded: the graph backward's kernels (launch_render_bwd_guarded)
+// guarded: the graph backward's blend adjoint.  The entry points' checks leave these combinations: peers only in the
+// eager non-deterministic backward; extra_attrs only without offsets and without the ordered form (part != nullptr).
 void sfgs_launch_render_bwd(const sfgs_backward_args* a, const GeomLayout& g, const ImageLayout& im,
                             const BinningLayout& b, float* acc, float* part, unsigned char* written, const float* off,
                             bool guarded, cudaStream_t st) {
   dim3 grid;
   int band0;
   if (!blend_grid(a->tile_row_begin, a->tile_row_end, im, grid, band0)) return;
-  if (guarded) { launch_render_bwd_guarded(a, g, im, b, acc, part, written, off, grid, band0, st); return; }
   PeerTable pt = {};
   const bool peer = a->acc_peers != nullptr && a->n_peers > 0;
   if (peer) {
     for (int r = 0; r < a->n_peers && r < 8; r++) pt.p[r] = a->acc_peers[r];
     pt.per = a->peer_slice;
   }
-  if (off != nullptr) {
-    const size_t smem_j = sizeof(WarpSmemJitter) * BLEND_WARPS;
-    static SfgsPerDeviceOnce attr_once_j;
-    if (attr_once_j.first_use()) {
-      cudaFuncSetAttribute(render_bwd_jitter_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_j);
-      cudaFuncSetAttribute(render_bwd_jitter_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_j);
-      cudaFuncSetAttribute(render_bwd_jitter_peer_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_j);
-    }
-    SFGS_COUNT_LAUNCH();
-    // peer reductions belong to the non-deterministic phase 1 (the deterministic entries reject acc_peers)
-    if (peer) {
-      render_bwd_jitter_peer_kernel<<<grid, BLEND_THREADS, smem_j, st>>>(
-          im.ranges, (const char*)b.point_list, im.hdr, a->width, a->height, band0, a->background, g.rec,
-          a->accum_alphas, im.n_contrib, a->dL_dpix, a->dL_dpix_depth, a->dL_dpix_norm, a->dL_dpix_alpha, a->norm_raw,
-          pt, reinterpret_cast<const float2*>(off));
-      return;
-    }
-    const auto kernel = part != nullptr ? render_bwd_jitter_kernel<true> : render_bwd_jitter_kernel<false>;
-    kernel<<<grid, BLEND_THREADS, smem_j, st>>>(im.ranges, (const char*)b.point_list, im.hdr, a->width, a->height, band0,
-                                                a->background, g.rec, a->accum_alphas, im.n_contrib, a->dL_dpix,
-                                                a->dL_dpix_depth, a->dL_dpix_norm, a->dL_dpix_alpha, a->norm_raw, acc,
-                                                part, written, reinterpret_cast<const float2*>(off));
-    return;
-  }
-  const size_t smem = sizeof(WarpSmem) * BLEND_WARPS;
-  static SfgsPerDeviceOnce attr_once;   // function attributes are per device
-  if (attr_once.first_use()) {
-    cudaFuncSetAttribute(render_bwd_warp_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaFuncSetAttribute(render_bwd_warp_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaFuncSetAttribute(render_bwd_warp_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaFuncSetAttribute(render_bwd_warp_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  }
-  // peer reductions belong to the two-phase backward, which rejects extra_attrs (sfgs_rasterize_backward); the
-  // ordered path (part != nullptr) rejects both (sfgs_rasterize_backward_deterministic)
-  const auto kernel = part != nullptr ? render_bwd_warp_kernel<false, false, true>
-                      : a->ED > 0     ? render_bwd_warp_kernel<false, true>
-                      : peer          ? render_bwd_warp_kernel<true, false>
-                                      : render_bwd_warp_kernel<false, false>;
+  const bool ordered = part != nullptr, extra = a->ED > 0;
+  // render_bwd_instance<PEER, HAS_EXTRA, ORDERED, JITTER, GUARDED>
+  const auto kernel =
+      guarded ? (off != nullptr ? (ordered ? render_bwd_instance<false, false, true, true, true>()
+                                           : render_bwd_instance<false, false, false, true, true>())
+                 : ordered      ? render_bwd_instance<false, false, true, false, true>()
+                 : extra        ? render_bwd_instance<false, true, false, false, true>()
+                                : render_bwd_instance<false, false, false, false, true>())
+      : off != nullptr ? (peer      ? render_bwd_instance<true, false, false, true, false>()
+                          : ordered ? render_bwd_instance<false, false, true, true, false>()
+                                    : render_bwd_instance<false, false, false, true, false>())
+      : ordered ? render_bwd_instance<false, false, true, false, false>()
+      : extra   ? render_bwd_instance<false, true, false, false, false>()
+      : peer    ? render_bwd_instance<true, false, false, false, false>()
+                : render_bwd_instance<false, false, false, false, false>();
+  const size_t smem = BLEND_WARPS * (off != nullptr ? sizeof(WarpSmemJitter) : sizeof(WarpSmem));
   SFGS_COUNT_LAUNCH();
   kernel<<<grid, BLEND_THREADS, smem, st>>>(im.ranges, (const char*)b.point_list, im.hdr, a->width, a->height, band0,
                                           a->background, g.rec, a->accum_alphas, im.n_contrib, a->dL_dpix,
                                           a->dL_dpix_depth, a->dL_dpix_norm, a->dL_dpix_alpha, a->norm_raw, acc, pt,
-                                          a->extra_attrs, a->dL_dpix_extra, a->dL_dextra, a->ED, part, written);
+                                          a->extra_attrs, a->dL_dpix_extra, a->dL_dextra, a->ED, part, written,
+                                          reinterpret_cast<const float2*>(off));
 }

@@ -146,40 +146,28 @@ render_fwd_warp(const uint2* __restrict__ ranges, const uint32_t* __restrict__ p
   }
 }
 
-template <bool HAS_EXTRA>
-__global__ void __launch_bounds__(BLEND_THREADS)
-render_fwd_warp_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list,
-                       const unsigned char* __restrict__ inst_mask, const uint32_t* __restrict__ hdr, int W, int H,
-                       int band0, const float* __restrict__ rec, const float* __restrict__ bg_color,
-                       float* __restrict__ out_color, float* __restrict__ out_depth, float* __restrict__ out_norm,
-                       float* __restrict__ out_norm_raw, float* __restrict__ out_alpha, uint32_t* __restrict__ n_contrib,
-                       const OutPeers peers, const float* __restrict__ extras, int ED, float* __restrict__ out_extra) {
-  render_fwd_warp<HAS_EXTRA, false>(ranges, point_list, inst_mask, hdr, W, H, band0, rec, bg_color, out_color, out_depth,
-                                    out_norm, out_norm_raw, out_alpha, n_contrib, peers, extras, ED, out_extra, nullptr);
-}
+// Where the pixels' results go: the default kernels choose at run time between the local outputs and the ranks'
+// [8,H,W] frame blocks (out_peers, the fused image all-gather of the tile-row sharded mode); each jitter kernel has one
+// of the two compiled in.
+enum class FwdOut { LOCAL_OR_PEERS, LOCAL, PEERS };
 
-// subpixel offsets into local outputs; no extra_attrs (sfgs_rasterize_forward_subpixel rejects them)
+// The one blend forward.  Each option is a template argument; a trailing parameter an instantiation does not read
+// (off without JITTER, extras without HAS_EXTRA) costs nothing, and new parameters go at the end of the list.
+template <bool HAS_EXTRA, bool JITTER, FwdOut OUT>
 __global__ void __launch_bounds__(BLEND_THREADS)
-render_fwd_jitter_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list,
-                         const unsigned char* __restrict__ inst_mask, const uint32_t* __restrict__ hdr, int W, int H,
-                         int band0, const float* __restrict__ rec, const float* __restrict__ bg_color,
-                         float* __restrict__ out_color, float* __restrict__ out_depth, float* __restrict__ out_norm,
-                         float* __restrict__ out_norm_raw, float* __restrict__ out_alpha,
-                         uint32_t* __restrict__ n_contrib, const float2* __restrict__ off) {
-  render_fwd_warp<false, true>(ranges, point_list, inst_mask, hdr, W, H, band0, rec, bg_color, out_color, out_depth,
-                               out_norm, out_norm_raw, out_alpha, n_contrib, OutPeers{}, nullptr, 0, nullptr, off);
-}
-
-// subpixel offsets with the fused image all-gather of the tile-row sharded mode: the band goes to every rank's
-// [8,H,W] frame block (a kernel of its own, so that the local-output kernel above keeps its code)
-__global__ void __launch_bounds__(BLEND_THREADS)
-render_fwd_jitter_peers_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list,
-                               const unsigned char* __restrict__ inst_mask, const uint32_t* __restrict__ hdr, int W,
-                               int H, int band0, const float* __restrict__ rec, const float* __restrict__ bg_color,
-                               float* __restrict__ out_norm_raw, uint32_t* __restrict__ n_contrib,
-                               const OutPeers peers, const float2* __restrict__ off) {
-  render_fwd_warp<false, true>(ranges, point_list, inst_mask, hdr, W, H, band0, rec, bg_color, nullptr, nullptr,
-                               nullptr, out_norm_raw, nullptr, n_contrib, peers, nullptr, 0, nullptr, off);
+render_fwd_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list,
+                  const unsigned char* __restrict__ inst_mask, const uint32_t* __restrict__ hdr, int W, int H,
+                  int band0, const float* __restrict__ rec, const float* __restrict__ bg_color,
+                  float* __restrict__ out_color, float* __restrict__ out_depth, float* __restrict__ out_norm,
+                  float* __restrict__ out_norm_raw, float* __restrict__ out_alpha, uint32_t* __restrict__ n_contrib,
+                  const OutPeers peers, const float* __restrict__ extras, int ED, float* __restrict__ out_extra,
+                  const float2* __restrict__ off) {
+  constexpr bool local = OUT != FwdOut::PEERS;
+  const OutPeers none{};
+  render_fwd_warp<HAS_EXTRA, JITTER>(ranges, point_list, inst_mask, hdr, W, H, band0, rec, bg_color,
+                                     local ? out_color : nullptr, local ? out_depth : nullptr,
+                                     local ? out_norm : nullptr, out_norm_raw, local ? out_alpha : nullptr, n_contrib,
+                                     OUT == FwdOut::LOCAL ? none : peers, extras, ED, out_extra, off);
 }
 
 // max |off_x|, max |off_y| over the frame into HDR_OFF_EX / HDR_OFF_EY (non-negative floats order as their bits), and
@@ -225,25 +213,14 @@ void sfgs_launch_render_fwd(const sfgs_forward_args* a, const GeomLayout& g, con
   OutPeers op = {};
   if (a->out_peers != nullptr && a->n_out_peers > 0)
     for (op.n = 0; op.n < a->n_out_peers && op.n < 8; op.n++) op.p[op.n] = a->out_peers[op.n];
-  if (off != nullptr && op.n > 0) {
-    SFGS_COUNT_LAUNCH();
-    render_fwd_jitter_peers_kernel<<<grid, BLEND_THREADS, 0, st>>>(im.ranges, b.point_list, b.inst_mask, im.hdr,
-                                                                   a->width, a->height, band0, g.rec, a->background,
-                                                                   a->out_norm_raw, im.n_contrib, op,
-                                                                   reinterpret_cast<const float2*>(off));
-    return;
-  }
-  if (off != nullptr) {
-    SFGS_COUNT_LAUNCH();
-    render_fwd_jitter_kernel<<<grid, BLEND_THREADS, 0, st>>>(im.ranges, b.point_list, b.inst_mask, im.hdr, a->width,
-                                                             a->height, band0, g.rec, a->background, a->out_color,
-                                                             a->out_depth, a->out_norm, a->out_norm_raw, a->out_alpha,
-                                                             im.n_contrib, reinterpret_cast<const float2*>(off));
-    return;
-  }
+  // extra_attrs only without offsets (the _subpixel entries reject them)
+  const auto kernel = off != nullptr ? (op.n > 0 ? render_fwd_kernel<false, true, FwdOut::PEERS>
+                                                 : render_fwd_kernel<false, true, FwdOut::LOCAL>)
+                      : a->ED > 0    ? render_fwd_kernel<true, false, FwdOut::LOCAL_OR_PEERS>
+                                     : render_fwd_kernel<false, false, FwdOut::LOCAL_OR_PEERS>;
   SFGS_COUNT_LAUNCH();
-  const auto kernel = a->ED > 0 ? render_fwd_warp_kernel<true> : render_fwd_warp_kernel<false>;
   kernel<<<grid, BLEND_THREADS, 0, st>>>(im.ranges, b.point_list, b.inst_mask, im.hdr, a->width, a->height, band0,
                                          g.rec, a->background, a->out_color, a->out_depth, a->out_norm, a->out_norm_raw,
-                                         a->out_alpha, im.n_contrib, op, a->extra_attrs, a->ED, a->out_extra);
+                                         a->out_alpha, im.n_contrib, op, a->extra_attrs, a->ED, a->out_extra,
+                                         reinterpret_cast<const float2*>(off));
 }
