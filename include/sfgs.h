@@ -326,6 +326,25 @@ int sfgs_rasterize_backward_graph(const sfgs_backward_args* a, const float* subp
  * image, from its earlier calls; -1 when there is none.  Read-only: the graph entries size their capacity from it. */
 long long sfgs_capacity_estimate(int device, int P, int width, int height);
 
+/* ---- Orthographic camera -----------------------------------------------------------------------------------------
+ * The one-call forward and backward for an orthographic view, e.g. a nadir height map of a satellite scene.  The
+ * structs are the pinhole ones, read differently:
+ *   - tan_fovx / tan_fovy are the half-extents s_x, s_y of the view volume in view-space units; the pixel scales are
+ *     h_x = W / (2 s_x), h_y = H / (2 s_y).  s <= 0 or non-finite returns SFGS_E_BADARG.
+ *   - The projected centre is ndc = ([m, 1]·projmatrix).xy with no divide (p.w is not read); projmatrix = viewmatrix · O
+ *     with O the orthographic projection (sfgs/ortho.py: projection_matrix), which carries the principal point.
+ *   - The EWA Jacobian is the constant [[h_x, 0, 0], [0, h_y, 0]]: no frustum clamp.  Depth, the t_z <= 0.2 cull,
+ *     `prefiltered`, the Mip filter, radii and tiles are as for a pinhole camera.
+ *   - The view direction of SH and of the normal's sign flip is the view's +z axis in world space, one per frame, in
+ *     place of m - campos.  cam_pos is not read but must not be NULL.
+ * subpixel_offset: NULL (no jitter) or as sfgs_rasterize_forward_subpixel.  The backward must be given the same camera
+ * form and the same offsets as the forward; deterministic != 0 selects the deterministic backward.  It writes the ten
+ * outputs of sfgs_rasterize_backward; dL_dmean2D keeps its layout (·W/2, ·H/2, sum |.|).  There are no camera terms.
+ * Before any CUDA work: tile-row bands, out_peers, acc_peers and phase != 0 return SFGS_E_UNSUPPORTED, then the s check,
+ * then the validation of the matching pinhole entry. */
+int sfgs_rasterize_forward_ortho(const sfgs_forward_args* a, const float* subpixel_offset);
+int sfgs_rasterize_backward_ortho(const sfgs_backward_args* a, const float* subpixel_offset, int deterministic);
+
 /* ---- markVisible --------------------------------------------------------- */
 int sfgs_mark_visible(int P, const float* means3D, const float* viewmatrix,
                       const float* projmatrix, unsigned char* present, void* stream);

@@ -14,6 +14,7 @@
 // Backward = zero accumulators -> tile blend adjoint -> per-Gaussian adjoint.
 // Deterministic backward = clear the written flags -> ORDERED blend adjoint (partial rows, no reductions) ->
 //            fixed-order float64 sum of each Gaussian's rows into acc (sfgs_bwd_order.cu) -> per-Gaussian adjoint.
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <atomic>
@@ -25,7 +26,7 @@ std::atomic<long long> g_sfgs_launches{0};
 
 void sfgs_launch_preprocess(const sfgs_forward_args* a, const GeomLayout& g, const ImageLayout& im,
                             const BinningLayout& b, unsigned long long capacity, float focal_x, float focal_y,
-                            const float* tan_fov, cudaStream_t st);
+                            const float* tan_fov, bool ortho, cudaStream_t st);
 void sfgs_launch_mark_visible(int P, const float* means3D, const float* viewmatrix, unsigned char* present,
                               cudaStream_t st);
 void sfgs_launch_tile_scan(const ImageLayout& im, unsigned long long capacity, cudaStream_t st);
@@ -56,7 +57,7 @@ int sfgs_launch_activations_bwd(int P, const float* opacity_raw, const float* sc
                                 float* g_rotation_raw, cudaStream_t st);
 void sfgs_launch_gauss_bwd(const sfgs_backward_args* a, const GeomLayout& g, float focal_x, float focal_y,
                            const float* acc, int g_begin, int g_end, int acc_row0, double* cam_part, int ncam,
-                           const float* tan_fov, cudaStream_t st);
+                           const float* tan_fov, bool ortho, cudaStream_t st);
 size_t sfgs_camera_scratch_bytes(int P, int ncam);
 void sfgs_launch_camera_reduce(int P, int ncam, const double* cam_part, float* dL_dcamera, cudaStream_t st);
 void sfgs_launch_camera_partial_reduce(int n, int ncam, const double* cam_part, double* dL_dcamera, cudaStream_t st);
@@ -211,6 +212,7 @@ struct FwdCall {
   bool peers_with_off = false;        // out_peers may come with offsets (the _subpixel_peers entry)
   const float* tan_fov = nullptr;     // graph: NULL or the DEVICE [2] intrinsics
   unsigned int* status = nullptr;     // graph: the DEVICE status word the frame's error flags are ORed into
+  bool ortho = false;                 // the orthographic camera (sfgs_rasterize_forward_ortho)
 };
 
 struct BwdCall {
@@ -223,6 +225,7 @@ struct BwdCall {
   float* dL_dcamera = nullptr;        // CAMERA, GRAPH: the DEVICE [ncam] camera gradients
   double* dL_dcamera_partial = nullptr;   // CAMERA_PARTIAL: the DEVICE [ncam] float64 sums of the Gaussian slice
   const float* tan_fov = nullptr;     // GRAPH: NULL or the DEVICE [2] intrinsics the per-Gaussian adjoint reads
+  bool ortho = false;                 // the orthographic camera (sfgs_rasterize_backward_ortho)
 };
 
 int rasterize_forward(const sfgs_forward_args* a, const FwdCall& c);
@@ -319,15 +322,34 @@ long long sfgs_capacity_estimate(int device, int P, int width, int height) {
   return cap_lookup(CapKey{device, P, width, height, 0, 0});
 }
 
+int sfgs_rasterize_forward_ortho(const sfgs_forward_args* a, const float* subpixel_offset) {
+  return rasterize_forward(a, {"forward_ortho", false, subpixel_offset, false, nullptr, nullptr, true});
+}
+
+int sfgs_rasterize_backward_ortho(const sfgs_backward_args* a, const float* subpixel_offset, int deterministic) {
+  return rasterize_backward(a, {"backward_ortho", BwdCall::EAGER, subpixel_offset, false, deterministic != 0, 0, nullptr,
+                                nullptr, nullptr, true});
+}
+
 }  // extern "C"
 
 namespace {
 
 // Every rejection of the forward entries, in the order that decides which one an entry reports; all before any CUDA
 // work.  Messages are "<entry>: <what>".
+// the orthographic camera's half-extents s_x, s_y (carried by tan_fovx, tan_fovy): finite and > 0
+bool ortho_extent_ok(float sx, float sy) { return std::isfinite(sx) && std::isfinite(sy) && sx > 0.f && sy > 0.f; }
+
 int check_forward(const sfgs_forward_args* a, const FwdCall& c) {
   const auto reject = [&c](int code, const char* what) { return fail_in(c.name, code, what); };
   if (!a) return reject(SFGS_E_BADARG, "null args");
+  if (c.ortho) {
+    if (a->tile_row_begin != 0 || a->tile_row_end != 0)
+      return reject(SFGS_E_UNSUPPORTED, "tile-row bands are not supported with an orthographic camera");
+    if (a->out_peers != nullptr) return reject(SFGS_E_UNSUPPORTED, "out_peers are not supported with an orthographic camera");
+    if (!ortho_extent_ok(a->tan_fovx, a->tan_fovy))
+      return reject(SFGS_E_BADARG, "the half-extents tan_fovx, tan_fovy must be finite and > 0");
+  }
   if (c.graph) {
     if (!c.status) return reject(SFGS_E_BADARG, "null status word");
     if (a->debug) return reject(SFGS_E_BADARG, "debug synchronises after every stage and cannot be captured");
@@ -408,7 +430,7 @@ int rasterize_forward(const sfgs_forward_args* a, const FwdCall& c) {
 
     if (P > 0) {
       PROF_BEGIN(ST_PREPROCESS);
-      sfgs_launch_preprocess(a, g, im, b, (unsigned long long)capacity, focal_x, focal_y, c.tan_fov, st);
+      sfgs_launch_preprocess(a, g, im, b, (unsigned long long)capacity, focal_x, focal_y, c.tan_fov, c.ortho, st);
       PROF_END();
       STAGE_CHECK("preprocess");
     }
@@ -491,6 +513,15 @@ int rasterize_forward(const sfgs_forward_args* a, const FwdCall& c) {
 int check_backward(const sfgs_backward_args* a, const BwdCall& c) {
   const auto reject = [&c](int code, const char* what) { return fail_in(c.name, code, what); };
   if (!a) return reject(SFGS_E_BADARG, "null args");
+  if (c.ortho) {
+    if (a->phase != 0)
+      return reject(SFGS_E_UNSUPPORTED, "phases 1 and 2 (the two-phase backward) are not supported with an orthographic camera");
+    if (a->acc_peers != nullptr) return reject(SFGS_E_UNSUPPORTED, "acc_peers are not supported with an orthographic camera");
+    if (a->tile_row_begin != 0 || a->tile_row_end != 0)
+      return reject(SFGS_E_UNSUPPORTED, "tile-row bands are not supported with an orthographic camera");
+    if (!ortho_extent_ok(a->tan_fovx, a->tan_fovy))
+      return reject(SFGS_E_BADARG, "the half-extents tan_fovx, tan_fovy must be finite and > 0");
+  }
   if (c.kind == BwdCall::CAMERA) {
     if (!c.dL_dcamera) return reject(SFGS_E_BADARG, "null dL_dcamera");
     if (a->phase != 0)
@@ -658,7 +689,7 @@ int rasterize_backward(const sfgs_backward_args* a, const BwdCall& c) {
   if (do_gauss) {
     PROF_BEGIN(ST_GAUSS_BWD);
     sfgs_launch_gauss_bwd(a, g, focal_x, focal_y, acc, g_begin, g_end, phase == 2 ? g_begin : 0, cam_part, ncam,
-                          c.tan_fov, st);
+                          c.tan_fov, c.ortho, st);
     if (dL_dcamera) sfgs_launch_camera_reduce(P, ncam, cam_part, dL_dcamera, st);
     // an empty slice has no spans: the reduction writes zeros
     if (dL_dcamera_partial) sfgs_launch_camera_partial_reduce(g_end - g_begin, ncam, cam_part, dL_dcamera_partial, st);

@@ -100,7 +100,11 @@ __device__ __forceinline__ float3 dnormvdv3(float3 v, float3 dv) {
 // SH view direction (minus the dnormvdv3 result).  Entries the forward does not read (viewmatrix[3,7,11,15],
 // projmatrix[2,6,10,14]) stay 0.  NCAM: the number of camera terms formed, 0 (none), GB_CAM_POSE or GB_CAM (the pose
 // terms and the focal terms).
-template <int NCAM, class SH>
+// ORTHO: the orthographic camera (see preprocess_kernel<DEV_FOV, ORTHO>).  h_x, h_y are the pixel scales of the constant
+// J = [[h_x, 0, 0], [0, h_y, 0]], which contributes no dL/dt; the projected centre [m, 1]·proj has no divide, so
+// dL/dm = proj rows 0-1 times dL/dndc; the SH view direction is the view's +z axis (view[2], view[6], view[10]) and has
+// no dL/dm term.  The depth term is the perspective one.  Only with NCAM == 0.
+template <int NCAM, bool ORTHO, class SH>
 __device__ __forceinline__ void gauss_adjoint(
     int D, float mx, float my, float mz, bool has_scales, float4 q_in, float scx, float scy, float scz,
     float scale_modifier, bool has_sh, unsigned cm, SH sh, const float* cov3D, bool norm_precomp, float4 A0,
@@ -139,8 +143,8 @@ __device__ __forceinline__ void gauss_adjoint(
     const float x_grad_mul = txtz < -limx || txtz > limx ? 0 : 1;
     const float y_grad_mul = tytz < -limy || tytz > limy ? 0 : 1;
 
-    const float a0 = h_x / tz, a2 = -(h_x * tx) / (tz * tz);
-    const float b1 = h_y / tz, b2 = -(h_y * ty) / (tz * tz);
+    const float a0 = ORTHO ? h_x : h_x / tz, a2 = ORTHO ? 0.0f : -(h_x * tx) / (tz * tz);
+    const float b1 = ORTHO ? h_y : h_y / tz, b2 = ORTHO ? 0.0f : -(h_y * ty) / (tz * tz);
     // W[c][r]
     const float Wm[3][3] = {{view[0], view[4], view[8]}, {view[1], view[5], view[9]}, {view[2], view[6], view[10]}};
     float T[3][3];   // T[c][r]
@@ -216,10 +220,12 @@ __device__ __forceinline__ void gauss_adjoint(
     const float dL_dtx = x_grad_mul * -h_x * tz2 * dL_dJ02;
     const float dL_dty = y_grad_mul * -h_y * tz2 * dL_dJ12;
     const float dL_dtz = -h_x * tz2 * dL_dJ00 - h_y * tz2 * dL_dJ11 + (2 * h_x * tx) * tz3 * dL_dJ02 + (2 * h_y * ty) * tz3 * dL_dJ12;
-    // view^T (3x3 part)
-    o_mean[0] = view[0] * dL_dtx + view[1] * dL_dty + view[2] * dL_dtz;
-    o_mean[1] = view[4] * dL_dtx + view[5] * dL_dty + view[6] * dL_dtz;
-    o_mean[2] = view[8] * dL_dtx + view[9] * dL_dty + view[10] * dL_dtz;
+    // view^T (3x3 part); a constant J (ORTHO) has no dL/dt
+    if constexpr (!ORTHO) {
+      o_mean[0] = view[0] * dL_dtx + view[1] * dL_dty + view[2] * dL_dtz;
+      o_mean[1] = view[4] * dL_dtx + view[5] * dL_dty + view[6] * dL_dtz;
+      o_mean[2] = view[8] * dL_dtx + view[9] * dL_dty + view[10] * dL_dtz;
+    }
     if constexpr (NCAM > 0) {
       // t = [m, 1]·view (columns 0..2): dL/dview[4k + r] = m_k dL/dt_r, dL/dview[12 + r] = dL/dt_r.  T = J·W with
       // W[k][r] = view[4r + k] and J = [[a0, 0, a2], [0, b1, b2]]: dL/dW[k][r] = sum_i J[i][k] dL/dT[i][r].
@@ -263,9 +269,13 @@ __device__ __forceinline__ void gauss_adjoint(
     const float mul1 = (proj[0] * mx + proj[4] * my + proj[8] * mz + proj[12]) * m_w * m_w;
     const float mul2 = (proj[1] * mx + proj[5] * my + proj[9] * mz + proj[13]) * m_w * m_w;
     const float gx = o_mean2D[0], gy = o_mean2D[1];
-    const float d0 = (proj[0] * m_w - proj[3] * mul1) * gx + (proj[1] * m_w - proj[3] * mul2) * gy;
-    const float d1 = (proj[4] * m_w - proj[7] * mul1) * gx + (proj[5] * m_w - proj[7] * mul2) * gy;
-    const float d2 = (proj[8] * m_w - proj[11] * mul1) * gx + (proj[9] * m_w - proj[11] * mul2) * gy;
+    // ORTHO: ndc = ([m, 1]·proj).xy, no divide
+    const float d0 = ORTHO ? proj[0] * gx + proj[1] * gy
+                           : (proj[0] * m_w - proj[3] * mul1) * gx + (proj[1] * m_w - proj[3] * mul2) * gy;
+    const float d1 = ORTHO ? proj[4] * gx + proj[5] * gy
+                           : (proj[4] * m_w - proj[7] * mul1) * gx + (proj[5] * m_w - proj[7] * mul2) * gy;
+    const float d2 = ORTHO ? proj[8] * gx + proj[9] * gy
+                           : (proj[8] * m_w - proj[11] * mul1) * gx + (proj[9] * m_w - proj[11] * mul2) * gy;
     o_mean[0] += d0; o_mean[1] += d1; o_mean[2] += d2;
     const float mul3 = view[2] * mx + view[6] * my + view[10] * mz + view[14];
     const float e0 = (view[2] - view[3] * mul3) * o_depth;
@@ -293,7 +303,9 @@ __device__ __forceinline__ void gauss_adjoint(
 
   // ---------------- RGB -> SH and view direction -> mean ----------------
   if (has_sh) {
-    const float ox = mx - campos[0], oy = my - campos[1], oz = mz - campos[2];
+    // ORTHO: one direction per frame, the view's +z axis
+    const float ox = ORTHO ? view[2] : mx - campos[0], oy = ORTHO ? view[6] : my - campos[1];
+    const float oz = ORTHO ? view[10] : mz - campos[2];
     const float len = sqrt(ox * ox + oy * oy + oz * oz);
     const float x = ox / len, y = oy / len, z = oz / len;
     dL_dRGB[0] = o_color[0] * ((cm & 1u) ? 0 : 1);
@@ -351,8 +363,10 @@ __device__ __forceinline__ void gauss_adjoint(
       dL_ddir.x = dRGBdx[0] * dL_dRGB[0] + dRGBdx[1] * dL_dRGB[1] + dRGBdx[2] * dL_dRGB[2];
       dL_ddir.y = dRGBdy[0] * dL_dRGB[0] + dRGBdy[1] * dL_dRGB[1] + dRGBdy[2] * dL_dRGB[2];
       dL_ddir.z = dRGBdz[0] * dL_dRGB[0] + dRGBdz[1] * dL_dRGB[1] + dRGBdz[2] * dL_dRGB[2];
-      const float3 dm = dnormvdv3(make_float3(ox, oy, oz), dL_ddir);
-      o_mean[0] += dm.x; o_mean[1] += dm.y; o_mean[2] += dm.z;
+      if constexpr (!ORTHO) {
+        const float3 dm = dnormvdv3(make_float3(ox, oy, oz), dL_ddir);
+        o_mean[0] += dm.x; o_mean[1] += dm.y; o_mean[2] += dm.z;
+      }
       if constexpr (NCAM > 0) {
         // -dnormvdv3(v, dL_ddir), evaluated again in double: reading dm here would give its final products a second
         // use, and the compiler would then no longer fuse them into the o_mean sums, changing dL_dmean3D's rounding
@@ -503,8 +517,9 @@ static_assert(sizeof(float) * (GB_CAM_STAGE + GB_CAM * GB_SLOTS) <= sizeof(GbInp
 // order.  DEV_FOV: device-resident intrinsics (the graph backward, sfgs_rasterize_backward_graph): tan_fov [2] is read
 // from device memory and the focal lengths are formed from it as the host forms them (W / (2 tan_fovx),
 // H / (2 tan_fovy)), as in preprocess_kernel<DEV_FOV>.  A trailing parameter an instantiation does not read costs
-// nothing, and new parameters go at the end of the list.
-template <int NCAM, bool DEV_FOV>
+// nothing, and new parameters go at the end of the list.  ORTHO: the orthographic camera's adjoint (gauss_adjoint); only
+// <0, false, true> is instantiated.
+template <int NCAM, bool DEV_FOV, bool ORTHO>
 __global__ void __launch_bounds__(GB_THREADS, GB_CTAS_PER_SM)
 gauss_bwd_kernel(int g_begin, int g_end, int spans_per_cta, int acc_row0, int D, int M,
                  const float* __restrict__ means3D, const int* __restrict__ radii, const float* __restrict__ shs,
@@ -518,6 +533,7 @@ gauss_bwd_kernel(int g_begin, int g_end, int spans_per_cta, int acc_row0, int D,
                  float* __restrict__ dL_dmean3D, float* __restrict__ dL_dcov3D, float* __restrict__ dL_dnorm3D,
                  float* __restrict__ dL_dsh, float* __restrict__ dL_dscale, float* __restrict__ dL_drot,
                  double* __restrict__ cam_part, const float* __restrict__ tan_fov, int W, int H) {
+  static_assert(!ORTHO || (NCAM == 0 && !DEV_FOV), "the orthographic adjoint has no camera terms and host intrinsics");
   if constexpr (DEV_FOV) {
     tan_fovx = tan_fov[0];
     tan_fovy = tan_fov[1];
@@ -639,7 +655,7 @@ gauss_bwd_kernel(int g_begin, int g_end, int spans_per_cta, int acc_row0, int D,
       const float* shk = reinterpret_cast<const float*>(&in.sh[0][k]);   // float j at word (j >> 2) * 4 * SLOTS + (j & 3)
       const float cov3D[6] = {in.cov[0][k], in.cov[1][k], in.cov[2][k], in.cov[3][k], in.cov[4][k], in.cov[5][k]};
       const unsigned cm = has_sh ? (in.clamped[k] >> (8 * (S.gidx[b][k] & 3))) & 0xffu : 0u;
-      gauss_adjoint<NCAM>(D, in.mean[0][k], in.mean[1][k], in.mean[2][k], has_scales,
+      gauss_adjoint<NCAM, ORTHO>(D, in.mean[0][k], in.mean[1][k], in.mean[2][k], has_scales,
                     has_scales ? in.rot[k] : make_float4(0.f, 0.f, 0.f, 0.f),
                     has_scales ? in.scale[0][k] : 0.f, has_scales ? in.scale[1][k] : 0.f,
                     has_scales ? in.scale[2][k] : 0.f, scale_modifier, has_sh, cm,
@@ -791,19 +807,21 @@ void sfgs_launch_camera_partial_reduce(int n, int ncam, const double* cam_part, 
 // span's camera partials, ncam = 35 (pose terms) or 37 (pose and focal terms)
 // tan_fov: NULL (the launch parameters a->tan_fovx / a->tan_fovy, focal_x, focal_y are used) or DEVICE float [2], read
 // by the kernel (DEV_FOV)
+// ortho: the orthographic adjoint (focal_x / focal_y are its pixel scales); cam_part and tan_fov are then NULL
 void sfgs_launch_gauss_bwd(const sfgs_backward_args* a, const GeomLayout& g, float focal_x, float focal_y,
                            const float* acc, int g_begin, int g_end, int acc_row0, double* cam_part, int ncam,
-                           const float* tan_fov, cudaStream_t st) {
+                           const float* tan_fov, bool ortho, cudaStream_t st) {
   if (g_end <= g_begin) return;
   const bool dev_fov = tan_fov != nullptr;
   const size_t smem = sizeof(GbShared);
   const auto kernel =
-      cam_part == nullptr ? (dev_fov ? sfgs_smem_kernel<gauss_bwd_kernel<0, true>>(smem)
-                                     : sfgs_smem_kernel<gauss_bwd_kernel<0, false>>(smem))
-      : ncam == GB_CAM    ? (dev_fov ? sfgs_smem_kernel<gauss_bwd_kernel<GB_CAM, true>>(smem)
-                                     : sfgs_smem_kernel<gauss_bwd_kernel<GB_CAM, false>>(smem))
-                          : (dev_fov ? sfgs_smem_kernel<gauss_bwd_kernel<GB_CAM_POSE, true>>(smem)
-                                     : sfgs_smem_kernel<gauss_bwd_kernel<GB_CAM_POSE, false>>(smem));
+      ortho               ? sfgs_smem_kernel<gauss_bwd_kernel<0, false, true>>(smem)
+      : cam_part == nullptr ? (dev_fov ? sfgs_smem_kernel<gauss_bwd_kernel<0, true, false>>(smem)
+                                       : sfgs_smem_kernel<gauss_bwd_kernel<0, false, false>>(smem))
+      : ncam == GB_CAM    ? (dev_fov ? sfgs_smem_kernel<gauss_bwd_kernel<GB_CAM, true, false>>(smem)
+                                     : sfgs_smem_kernel<gauss_bwd_kernel<GB_CAM, false, false>>(smem))
+                          : (dev_fov ? sfgs_smem_kernel<gauss_bwd_kernel<GB_CAM_POSE, true, false>>(smem)
+                                     : sfgs_smem_kernel<gauss_bwd_kernel<GB_CAM_POSE, false, false>>(smem));
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   { int v = 0; if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && v > 0) sms = v; }

@@ -86,25 +86,32 @@ __device__ __forceinline__ void normal_from_scale_rot(float sx, float sy, float 
 
 // EWA projection of the 3D covariance + Mip-Splatting 2D filter.
 // Mirrors computeCov2D, forward.cu:74-124. Returns (cov00+k, cov01, cov11+k, coef).
+// ORTHO: the orthographic camera's constant Jacobian J = [[h_x, 0, 0], [0, h_y, 0]] (focal_x / focal_y carry the pixel
+// scales h = W / (2 s)): no clamp and no t dependence; everything after J is the perspective code.
+template <bool ORTHO>
 __device__ __forceinline__ float4 cov2d_project(float mx, float my, float mz,
                                                 float focal_x, float focal_y,
                                                 float tan_fovx, float tan_fovy, float kernel_size,
                                                 const Sym3& V, const float* __restrict__ vm) {
-  float tx = vm[0] * mx + vm[4] * my + vm[8] * mz + vm[12];
-  float ty = vm[1] * mx + vm[5] * my + vm[9] * mz + vm[13];
-  const float tz = vm[2] * mx + vm[6] * my + vm[10] * mz + vm[14];
-  const float limx = 1.3f * tan_fovx;
-  const float limy = 1.3f * tan_fovy;
-  const float txtz = tx / tz;
-  const float tytz = ty / tz;
-  tx = min(limx, max(-limx, txtz)) * tz;
-  ty = min(limy, max(-limy, tytz)) * tz;
+  float a0, a2, b1, b2;   // J columns: (a0, 0, a2), (0, b1, b2), 0
+  if constexpr (ORTHO) {
+    a0 = focal_x; a2 = 0.0f; b1 = focal_y; b2 = 0.0f;
+  } else {
+    float tx = vm[0] * mx + vm[4] * my + vm[8] * mz + vm[12];
+    float ty = vm[1] * mx + vm[5] * my + vm[9] * mz + vm[13];
+    const float tz = vm[2] * mx + vm[6] * my + vm[10] * mz + vm[14];
+    const float limx = 1.3f * tan_fovx;
+    const float limy = 1.3f * tan_fovy;
+    const float txtz = tx / tz;
+    const float tytz = ty / tz;
+    tx = min(limx, max(-limx, txtz)) * tz;
+    ty = min(limy, max(-limy, tytz)) * tz;
 
-  // J columns: (a0, 0, a2), (0, b1, b2), 0
-  const float a0 = focal_x / tz;
-  const float a2 = -(focal_x * tx) / (tz * tz);
-  const float b1 = focal_y / tz;
-  const float b2 = -(focal_y * ty) / (tz * tz);
+    a0 = focal_x / tz;
+    a2 = -(focal_x * tx) / (tz * tz);
+    b1 = focal_y / tz;
+    b2 = -(focal_y * ty) / (tz * tz);
+  }
   // W columns: (vm0,vm4,vm8), (vm1,vm5,vm9), (vm2,vm6,vm10); T = W * J
   float T0[3], T1[3];
   T0[0] = vm[0] * a0 + vm[1] * 0.0f + vm[2] * a2;
@@ -205,7 +212,12 @@ __device__ __forceinline__ float radius_bound(float trace_sigma, float view_z, f
 // DEV_FOV: tan_fov [2] is read from device memory (the graph forward, sfgs_rasterize_forward_graph, whose camera
 // intrinsics are refilled between replays) and tan_fovx, tan_fovy, focal_x, focal_y are derived from it exactly as the
 // host derives them; without it the trailing pointer is not read and the code is that of the launch-parameter form.
-template <bool DEV_FOV>
+// ORTHO: the orthographic camera (sfgs_rasterize_forward_ortho).  tan_fovx / tan_fovy carry the half-extents s_x, s_y
+// of the view volume and focal_x / focal_y the pixel scales h = W / (2 s); the projected centre is [m, 1]·projmatrix
+// with no divide; J is constant (cov2d_project<true>), so the cull bound has no 1 / t_z^2; and the view direction of SH
+// and of the normal's sign flip is the view's +z axis in world space, (vm[2], vm[6], vm[10]), for every Gaussian, in
+// place of m - campos.  cam_pos is not read.  Only <false, true> is instantiated.
+template <bool DEV_FOV, bool ORTHO>
 __global__ void __launch_bounds__(PRE_THREADS, 3)
 preprocess_kernel(int P, int D, int M,
                   const float* __restrict__ means3D, const float* __restrict__ scales, float scale_modifier,
@@ -246,7 +258,9 @@ preprocess_kernel(int P, int D, int M,
   const float limx = 1.3f * tan_fovx, limy = 1.3f * tan_fovy;
   const float wf2 = vm[0] * vm[0] + vm[1] * vm[1] + vm[2] * vm[2] + vm[4] * vm[4] + vm[5] * vm[5] + vm[6] * vm[6] +
                     vm[8] * vm[8] + vm[9] * vm[9] + vm[10] * vm[10];
-  const float jw2 = (focal_x * focal_x * (1.f + limx * limx) + focal_y * focal_y * (1.f + limy * limy)) * wf2;
+  // ORTHO: |J|_F^2 = h_x^2 + h_y^2 with no 1 / t_z^2, which the bound below then divides by 1
+  const float jw2 = ORTHO ? (focal_x * focal_x + focal_y * focal_y) * wf2
+                          : (focal_x * focal_x * (1.f + limx * limx) + focal_y * focal_y * (1.f + limy * limy)) * wf2;
   unsigned cand_bits = 0;          // bit j: Gaussian base + j*256 + tid is a candidate
   // every load of the four Gaussians is issued before anything is computed: one DRAM round trip per thread instead of
   // eight dependent ones (the test is latency-bound; the few bytes fetched for Gaussians behind the camera are cheaper
@@ -278,9 +292,14 @@ preprocess_kernel(int P, int D, int M,
       if (view_z > 0.199f) {                                            // 0.2 with a margin: the exact test follows
         const float hx = pm[0] * px + pm[4] * py + pm[8] * pz + pm[12];
         const float hy = pm[1] * px + pm[5] * py + pm[9] * pz + pm[13];
-        const float hw = pm[3] * px + pm[7] * py + pm[11] * pz + pm[15];
-        const float p_w = 1.0f / (hw + 0.0000001f);
-        const float pix_x = ndc_to_pix(hx * p_w, W), pix_y = ndc_to_pix(hy * p_w, H);
+        float pix_x, pix_y;
+        if constexpr (ORTHO) {
+          pix_x = ndc_to_pix(hx, W); pix_y = ndc_to_pix(hy, H);
+        } else {
+          const float hw = pm[3] * px + pm[7] * py + pm[11] * pz + pm[15];
+          const float p_w = 1.0f / (hw + 0.0000001f);
+          pix_x = ndc_to_pix(hx * p_w, W); pix_y = ndc_to_pix(hy * p_w, H);
+        }
         float trace_sigma;
         if (cov3D_precomp != nullptr) {
           trace_sigma = scl4[j].x + scl4[j].y + scl4[j].z;
@@ -295,7 +314,7 @@ preprocess_kernel(int P, int D, int M,
           const float n2 = R[0][2] * R[0][2] + R[1][2] * R[1][2] + R[2][2] * R[2][2];
           trace_sigma = scale_modifier * scale_modifier * (sx * sx * n0 + sy * sy * n1 + sz * sz * n2);
         }
-        const float rb = radius_bound(fabsf(trace_sigma), view_z, jw2, kernel_size);
+        const float rb = radius_bound(fabsf(trace_sigma), ORTHO ? 1.0f : view_z, jw2, kernel_size);
         if (!(rb < 1.0e9f) || !(fabsf(pix_x) < 1.0e9f) || !(fabsf(pix_y) < 1.0e9f)) cand_j = true;   // inf / NaN: let the exact path decide
         else {
           const TileRect r = tile_rect(pix_x, pix_y, (int)rb + 1, gx, gy);
@@ -364,9 +383,12 @@ preprocess_kernel(int P, int D, int M,
       if (view_z > 0.2f) {
         const float hx = pm[0] * px + pm[4] * py + pm[8] * pz + pm[12];
         const float hy = pm[1] * px + pm[5] * py + pm[9] * pz + pm[13];
-        const float hw = pm[3] * px + pm[7] * py + pm[11] * pz + pm[15];
-        const float p_w = 1.0f / (hw + 0.0000001f);
-        const float proj_x = hx * p_w, proj_y = hy * p_w;
+        float proj_x = hx, proj_y = hy;
+        if constexpr (!ORTHO) {
+          const float hw = pm[3] * px + pm[7] * py + pm[11] * pz + pm[15];
+          const float p_w = 1.0f / (hw + 0.0000001f);
+          proj_x = hx * p_w; proj_y = hy * p_w;
+        }
 
         Sym3 V;
         if (cov3D_precomp != nullptr) {
@@ -376,7 +398,7 @@ preprocess_kernel(int P, int D, int M,
           V = cov3d_from_scale_rot(sx, sy, sz, scale_modifier, q.x, q.y, q.z, q.w);
         }
 
-        const float4 cov = cov2d_project(px, py, pz, focal_x, focal_y, tan_fovx, tan_fovy, kernel_size, V, vm);
+        const float4 cov = cov2d_project<ORTHO>(px, py, pz, focal_x, focal_y, tan_fovx, tan_fovy, kernel_size, V, vm);
         const float det = (cov.x * cov.z - cov.y * cov.y);
         if (det != 0.0f) {
           const float det_inv = 1.f / det;
@@ -420,11 +442,14 @@ preprocess_kernel(int P, int D, int M,
           float* co = cov3D_out + 6 * (size_t)idx;
           co[0] = g_V.c0; co[1] = g_V.c1; co[2] = g_V.c2; co[3] = g_V.c3; co[4] = g_V.c4; co[5] = g_V.c5;
         }
+        // the view direction the normal flip and SH read: p - cam_pos, or the orthographic view axis (as d - 0)
+#define VIEW_DIR ORTHO ? vm[2] : px, ORTHO ? vm[6] : py, ORTHO ? vm[10] : pz, ORTHO ? 0.f : cam_pos[0], \
+                 ORTHO ? 0.f : cam_pos[1], ORTHO ? 0.f : cam_pos[2]
         float n[3];
         if (norm3D_precomp != nullptr) {
           n[0] = norm3D_precomp[3 * (size_t)idx]; n[1] = norm3D_precomp[3 * (size_t)idx + 1]; n[2] = norm3D_precomp[3 * (size_t)idx + 2];
         } else {
-          normal_from_scale_rot(sx, sy, sz, q.x, q.y, q.z, q.w, px, py, pz, cam_pos[0], cam_pos[1], cam_pos[2], n);
+          normal_from_scale_rot(sx, sy, sz, q.x, q.y, q.z, q.w, VIEW_DIR, n);
         }
         float rgb[3];
         unsigned cmask = 0;
@@ -433,15 +458,15 @@ preprocess_kernel(int P, int D, int M,
             asm volatile("cp.async.wait_group 0;\n" ::: "memory");
             // coefficient j sits in word (j & 3) of float4 [j >> 2][tid] of this thread's shared-memory column
             const float* col = reinterpret_cast<const float*>(s_sh) + 4 * tid;
-            sh_to_rgb(D, [&](int j) { return col[(j >> 2) * (4 * PRE_THREADS) + (j & 3)]; }, px, py, pz, cam_pos[0],
-                      cam_pos[1], cam_pos[2], rgb, cmask);
+            sh_to_rgb(D, [&](int j) { return col[(j >> 2) * (4 * PRE_THREADS) + (j & 3)]; }, VIEW_DIR, rgb, cmask);
           } else {
             const float* shp = shs + (size_t)idx * M * 3;
-            sh_to_rgb(D, [&](int j) { return shp[j]; }, px, py, pz, cam_pos[0], cam_pos[1], cam_pos[2], rgb, cmask);
+            sh_to_rgb(D, [&](int j) { return shp[j]; }, VIEW_DIR, rgb, cmask);
           }
         } else {
           rgb[0] = colors_precomp[3 * (size_t)idx]; rgb[1] = colors_precomp[3 * (size_t)idx + 1]; rgb[2] = colors_precomp[3 * (size_t)idx + 2];
         }
+#undef VIEW_DIR
         clamped[idx] = (unsigned char)cmask;
 
         float4* o = reinterpret_cast<float4*>(rec + (size_t)idx * REC_FLOATS);
@@ -500,19 +525,22 @@ __global__ void mark_visible_kernel(int P, const float* __restrict__ means3D,
 
 void sfgs_launch_preprocess(const sfgs_forward_args* a, const GeomLayout& g, const ImageLayout& im,
                             const BinningLayout& b, unsigned long long capacity, float focal_x, float focal_y,
-                            const float* tan_fov, cudaStream_t st) {
+                            const float* tan_fov, bool ortho, cudaStream_t st) {
   const int blocks = (a->P + PRE_SPAN - 1) / PRE_SPAN;
   constexpr size_t smem = PRE_THREADS * (12 * sizeof(float4) + sizeof(uint32_t) + sizeof(int4) + sizeof(uint32_t)) +
                           PRE_SPAN * sizeof(unsigned short);
   static SfgsPerDeviceOnce attr_once;   // function attributes are per device
   if (attr_once.first_use()) {
-    cudaFuncSetAttribute(preprocess_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaFuncSetAttribute(preprocess_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(preprocess_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(preprocess_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(preprocess_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   }
   const SfgsBand band = sfgs_band(a->tile_row_begin, a->tile_row_end, im.tiles_y);
   const int band0 = band.b0, band1 = band.b1;
   SFGS_COUNT_LAUNCH();
-  const auto kernel = tan_fov != nullptr ? preprocess_kernel<true> : preprocess_kernel<false>;
+  // ortho: tan_fov is NULL (the orthographic entries take the intrinsics as launch parameters)
+  const auto kernel = ortho ? preprocess_kernel<false, true>
+                      : tan_fov != nullptr ? preprocess_kernel<true, false> : preprocess_kernel<false, false>;
   kernel<<<blocks, PRE_THREADS, smem, st>>>(
       a->P, a->D, a->M, a->means3D, a->scales, a->scale_modifier, a->rotations, a->opacities, a->shs,
       a->cov3D_precomp, a->norm3D_precomp, a->colors_precomp, a->viewmatrix, a->projmatrix, a->cam_pos,

@@ -99,6 +99,7 @@ EXPORTS = [
     "sfgs_appearance_backward_scratch_bytes", "sfgs_compute_3d_filter",
     "sfgs_densification_stats", "sfgs_densify_plan_blocks", "sfgs_densify_plan", "sfgs_densify_apply",
     "sfgs_rasterize_forward_graph", "sfgs_rasterize_backward_graph", "sfgs_capacity_estimate",
+    "sfgs_rasterize_forward_ortho", "sfgs_rasterize_backward_ortho",
 ]
 STAGE_NAMES = ["fwd_zero", "preprocess", "tile_scan", "emit_keys", "tile_sort", "render_fwd", "bwd_zero", "render_bwd",
                "gauss_bwd", "bwd_order"]
@@ -144,6 +145,10 @@ def lib() -> C.CDLL:
     L.sfgs_rasterize_backward_graph.argtypes = [C.POINTER(BackwardArgs), C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
                                                 C.c_int]
     L.sfgs_rasterize_backward_graph.restype = C.c_int
+    L.sfgs_rasterize_forward_ortho.argtypes = [C.POINTER(ForwardArgs), C.c_void_p]
+    L.sfgs_rasterize_forward_ortho.restype = C.c_int
+    L.sfgs_rasterize_backward_ortho.argtypes = [C.POINTER(BackwardArgs), C.c_void_p, C.c_int]
+    L.sfgs_rasterize_backward_ortho.restype = C.c_int
     L.sfgs_capacity_estimate.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int]
     L.sfgs_capacity_estimate.restype = C.c_longlong
     L.sfgs_mark_visible.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]

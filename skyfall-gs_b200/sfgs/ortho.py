@@ -1,0 +1,188 @@
+"""Orthographic views: render and differentiate nadir height maps of a satellite scene.
+
+The rasterizer's orthographic camera (sfgs_rasterize_forward_ortho / sfgs_rasterize_backward_ortho, include/sfgs.h)
+behind a module shaped like diff_gauss.GaussianRasterizer:
+
+    OrthoRasterizationSettings   NamedTuple; half_width / half_height (s_x, s_y) replace tanfovx / tanfovy, no campos
+    OrthoRasterizer(settings)    nn.Module; same call signature, validation and 6-tuple as GaussianRasterizer
+    projection_matrix(...)       the orthographic projection, transposed (row vectors) like getProjectionMatrix
+    nadir_camera(...)            a camera looking straight down (-z) on an axis-aligned box of a z-up scene
+    render_height_map(...)       the scene's height map (a DSM) in one rasterizer call, differentiable
+
+The view is t = [m, 1]·viewmatrix.  A Gaussian's pixel position is ndc = ([m, 1]·projmatrix).xy (no divide), its depth
+t_z, and its 2D covariance J W Sigma W^T J^T with the constant J = diag(W / (2 s_x), H / (2 s_y)).  SH colours and the
+normals' orientation use the view's +z axis, one direction for the whole frame.
+"""
+from __future__ import annotations
+
+from typing import NamedTuple, Optional
+
+import torch
+import torch.nn as nn
+
+from . import rasterizer as R
+
+
+class OrthoRasterizationSettings(NamedTuple):
+    image_height: int
+    image_width: int
+    half_width: float       # s_x: half the view volume's width, in view-space units
+    half_height: float      # s_y
+    kernel_size: float
+    bg: torch.Tensor
+    scale_modifier: float
+    viewmatrix: torch.Tensor
+    projmatrix: torch.Tensor
+    sh_degree: int
+    prefiltered: bool
+    debug: bool
+    subpixel_offset: Optional[torch.Tensor] = None   # [H,W,2] CUDA float32, or None
+
+
+def projection_matrix(s_x, s_y, znear, zfar, cx=0.0, cy=0.0):
+    """The orthographic projection of the box |x| <= s_x, |y| <= s_y, znear <= z <= zfar of view space, as the
+    transposed (row-vector) [4,4] float32 matrix, like getProjectionMatrix: projmatrix = viewmatrix @ this.
+
+    x and y map to ndc x / s_x + cx and y / s_y + cy, so (cx, cy) is the principal point's offset in ndc (0: the
+    image centre); z maps to [0, 1] (the rasterizer does not read it) and w is 1."""
+    O = torch.zeros((4, 4), dtype=torch.float64)
+    O[0, 0], O[0, 3] = 1.0 / float(s_x), float(cx)
+    O[1, 1], O[1, 3] = 1.0 / float(s_y), float(cy)
+    O[2, 2], O[2, 3] = 1.0 / (float(zfar) - float(znear)), -float(znear) / (float(zfar) - float(znear))
+    O[3, 3] = 1.0
+    return O.t().contiguous().float()
+
+
+class NadirCamera(NamedTuple):
+    image_height: int
+    image_width: int
+    half_width: float
+    half_height: float
+    viewmatrix: torch.Tensor    # [4,4] float32, row vectors (world_view_transform)
+    projmatrix: torch.Tensor    # [4,4] float32, viewmatrix @ projection_matrix
+    z_top: float                # the camera plane; a pixel's height is z_top - its depth
+    xmin: float                 # world x of the image's left edge
+    ymax: float                 # world y of the image's top edge
+    resolution: float           # world units per pixel
+
+
+def nadir_camera(xmin, xmax, ymin, ymax, resolution, z_top):
+    """An orthographic camera at height z_top looking down (-z) on the box [xmin, xmax] x [ymin, ymax] of a scene
+    whose up axis is +z (Skyfall-GS's normalised scenes).  Image columns run along +x and rows along -y (north up);
+    pixel (i, j) covers x in [xmin + i r, xmin + (i+1) r], y in [ymax - (j+1) r, ymax - j r] for r = resolution.
+    The image is round((xmax - xmin) / r) x round((ymax - ymin) / r) pixels, so the box is grown or shrunk on its right
+    and bottom edges by less than half a pixel.  View depth is z_top - z: the scene must lie at least 0.2 below z_top,
+    as for any camera (the near cull)."""
+    r = float(resolution)
+    if not r > 0.0:
+        raise ValueError(f"resolution must be > 0, got {resolution}")
+    W = max(1, int(round((float(xmax) - float(xmin)) / r)))
+    H = max(1, int(round((float(ymax) - float(ymin)) / r)))
+    s_x, s_y = 0.5 * W * r, 0.5 * H * r
+    c = (float(xmin) + s_x, float(ymax) - s_y, float(z_top))
+    # view axes in world space: x_v = +x, y_v = -y, z_v = -z (a proper rotation); t = R (m - c)
+    Rm = torch.tensor([[1.0, 0.0, 0.0], [0.0, -1.0, 0.0], [0.0, 0.0, -1.0]], dtype=torch.float64)
+    V = torch.zeros((4, 4), dtype=torch.float64)
+    V[:3, :3] = Rm.t()
+    V[3, :3] = -(Rm @ torch.tensor(c, dtype=torch.float64))
+    V[3, 3] = 1.0
+    view = V.float()
+    proj = (V @ projection_matrix(s_x, s_y, 0.01, max(2.0 * abs(float(z_top)), 1.0) + 1e4).double()).float()
+    return NadirCamera(H, W, s_x, s_y, view, proj, float(z_top), float(xmin), float(ymax), r)
+
+
+def _requires_grad(x):
+    return isinstance(x, torch.Tensor) and x.requires_grad
+
+
+class _RasterizeOrtho(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                norm3Ds_precomp, extra_attrs, rs):
+        n_extra = extra_attrs.shape[1] if extra_attrs.shape[0] != 0 else 0
+        dev = means3D.device
+        campos = torch.zeros(3, dtype=torch.float32, device=dev)      # not read by the orthographic camera
+        off = rs.subpixel_offset
+        (num_rendered, color, depth, norm, alpha, radii, extra, geom_buf, binning_buf, img_buf,
+         norm_raw) = R.rasterize_gaussians(
+            rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier, cov3Ds_precomp,
+            norm3Ds_precomp, extra_attrs, n_extra, rs.viewmatrix, rs.projmatrix, rs.half_width, rs.half_height,
+            rs.kernel_size, rs.image_height, rs.image_width, sh, rs.sh_degree, campos, rs.prefiltered, rs.debug,
+            fuse_normalize=True, subpixel_offset=off, ortho=True)
+        ctx.rs, ctx.campos, ctx.num_rendered = rs, campos, num_rendered
+        ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, norm3Ds_precomp, radii,
+                              extra_attrs, sh, geom_buf, binning_buf, img_buf, alpha, norm_raw)
+        ctx.mark_non_differentiable(radii)
+        return color, depth, norm, alpha, radii, extra
+
+    @staticmethod
+    def backward(ctx, g_color, g_depth, g_norm, g_alpha, _g_radii, g_extra):
+        rs = ctx.rs
+        (colors_precomp, means3D, scales, rotations, cov3Ds_precomp, norm3Ds_precomp, radii, extra_attrs, sh,
+         geom_buf, binning_buf, img_buf, alpha, norm_raw) = ctx.saved_tensors
+        # deterministic under torch.use_deterministic_algorithms(True), as for the perspective backward
+        grads = R.rasterize_gaussians_backward(
+            rs.bg, means3D, radii, colors_precomp, scales, rotations, extra_attrs, rs.scale_modifier, cov3Ds_precomp,
+            norm3Ds_precomp, rs.viewmatrix, rs.projmatrix, rs.half_width, rs.half_height, rs.kernel_size,
+            g_color.contiguous(), g_depth.contiguous(), g_norm.contiguous(), g_alpha.contiguous(),
+            g_extra.contiguous(), sh, rs.sh_degree, ctx.campos, geom_buf, ctx.num_rendered, binning_buf, img_buf,
+            alpha, rs.debug, norm_raw=norm_raw, subpixel_offset=rs.subpixel_offset, ortho=True)
+        (g_means2D, g_colors, g_opac, g_means3D, g_cov3D, g_norm3D, g_sh, g_scales, g_rot, g_extra_attrs) = grads
+        return (g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rot, g_cov3D, g_norm3D, g_extra_attrs, None)
+
+
+class OrthoRasterizer(nn.Module):
+    """diff_gauss.GaussianRasterizer for an orthographic camera: same call, same checks, same returned
+    (color [3,H,W], depth [1,H,W], unit normal [3,H,W], alpha [1,H,W], radii [P], extra [F,H,W] | empty).  `means2D`'s
+    .grad receives (dL/dx_ndc W/2, dL/dy_ndc H/2, sum |.|), the densification statistics.  There are no camera
+    gradients: a viewmatrix or projmatrix that requires grad raises."""
+
+    def __init__(self, raster_settings: OrthoRasterizationSettings):
+        super().__init__()
+        self.raster_settings = raster_settings
+
+    def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
+                cov3Ds_precomp=None, norm3Ds_precomp=None, extra_attrs=None):
+        rs = self.raster_settings
+        if (shs is None) == (colors_precomp is None):
+            raise Exception('Please provide excatly one of either SHs or precomputed colors!')
+        has_sr = scales is not None or rotations is not None
+        if ((scales is None or rotations is None) and cov3Ds_precomp is None) or (has_sr and cov3Ds_precomp is not None):
+            raise Exception('Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!')
+        if scales is None:
+            raise ValueError('To support norm and depth prediction, scales == None is not allowed')
+        if rotations is None:
+            raise ValueError('To support norm and depth prediction, rotations == None is not allowed')
+        if _requires_grad(rs.viewmatrix) or _requires_grad(rs.projmatrix):
+            raise ValueError("OrthoRasterizer forms no camera gradients: viewmatrix and projmatrix must not require "
+                             "grad (detach them)")
+        if rs.subpixel_offset is not None:
+            R.check_subpixel_offset(rs.subpixel_offset, int(rs.image_height), int(rs.image_width))
+
+        def _or_empty(t):
+            return torch.Tensor([]) if t is None else t
+
+        return _RasterizeOrtho.apply(means3D, means2D, _or_empty(shs), _or_empty(colors_precomp), opacities, scales,
+                                     rotations, _or_empty(cov3Ds_precomp), _or_empty(norm3Ds_precomp),
+                                     _or_empty(extra_attrs), rs)
+
+
+def render_height_map(camera: NadirCamera, means3D, opacities, scales, rotations, shs=None, colors_precomp=None,
+                      sh_degree=0, alpha_min=0.5, kernel_size=0.1, scale_modifier=1.0):
+    """The scene's height map [H, W] seen by `camera` (nadir_camera): z_top - depth / alpha where the accumulated
+    alpha is >= alpha_min, NaN elsewhere.  depth / alpha is the alpha-normalised expected view depth of the pixel.
+    Differentiable with respect to the Gaussians (e.g. an L1 against a DSM over the finite pixels)."""
+    dev = means3D.device
+    if shs is None and colors_precomp is None:
+        colors_precomp = torch.zeros((means3D.shape[0], 3), dtype=torch.float32, device=dev)
+    rs = OrthoRasterizationSettings(camera.image_height, camera.image_width, camera.half_width, camera.half_height,
+                                    kernel_size, torch.zeros(3, device=dev), scale_modifier,
+                                    camera.viewmatrix.to(dev), camera.projmatrix.to(dev), sh_degree, False, False)
+    means2D = torch.zeros_like(means3D)
+    _, depth, _, alpha, _, _ = OrthoRasterizer(rs)(means3D, means2D, opacities, shs=shs,
+                                                   colors_precomp=colors_precomp, scales=scales,
+                                                   rotations=rotations)
+    depth, alpha = depth[0], alpha[0]
+    valid = alpha >= alpha_min
+    safe = torch.where(valid, alpha, torch.ones_like(alpha))       # no 0/0 in the masked branch's gradient
+    return torch.where(valid, camera.z_top - depth / safe, torch.full_like(depth, float("nan")))

@@ -99,11 +99,19 @@ def _graph_unsupported(where, debug, tile_rows=None, peers=None, phase=0):
         raise N.SfgsError(f"{where}: {', '.join(what)} cannot be captured in a CUDA graph")
 
 
+def _ortho_unsupported(where, **opts):
+    """The options an orthographic call cannot take (truthy values of `opts`), as an error raised before any native
+    call."""
+    what = [k for k, v in opts.items() if v]
+    if what:
+        raise N.SfgsError(f"{where}: {', '.join(what)} not supported with an orthographic camera")
+
+
 def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations, scale_modifier,
                         cov3Ds_precomp, norm3Ds_precomp, extra_attrs, attr_degree, viewmatrix, projmatrix,
                         tan_fovx, tan_fovy, kernel_size, image_height, image_width, sh, degree, campos,
                         prefiltered, debug, capacity_hint=0, tile_rows=None, fuse_normalize=False, out_planes=None,
-                        out_peers=None, subpixel_offset=None, graph=False):
+                        out_peers=None, subpixel_offset=None, graph=False, *, ortho=False):
     """Same positional signature and return tuple as the reference's `_C.rasterize_gaussians`.  With
     `fuse_normalize=True` the returned normal map is already F.normalize(., dim=0) (the reference's torch post-op,
     diff_gauss/__init__.py:48) and the un-normalised blend is appended to the tuple for the backward.
@@ -117,9 +125,17 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
     `graph=True`: the capture-safe forward (sfgs_rasterize_forward_graph) for torch.cuda.graph.  `capacity_hint` (> 0)
     is the binning capacity; `tan_fovx` / `tan_fovy` may be 0-d CUDA tensors, read on the device at every replay; the
     frame's error flags go to the sticky status word of sfgs.graphs instead of raising, and the first element of the
-    tuple is -1 (num_rendered is not known on the host).  debug, tile_rows and out_peers raise."""
+    tuple is -1 (num_rendered is not known on the host).  debug, tile_rows and out_peers raise.
+
+    `ortho=True`: an orthographic view (sfgs_rasterize_forward_ortho, include/sfgs.h; sfgs.ortho builds its matrices):
+    `tan_fovx` / `tan_fovy` are the half-extents s_x, s_y of the view volume, the projected centre is
+    [m, 1]·projmatrix without a divide, and SH and normals see the view's +z axis.  Offsets combine with it; graph,
+    tile_rows and out_peers raise SfgsError."""
     if means3D.ndim != 2 or means3D.shape[1] != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")
+    if ortho:
+        _ortho_unsupported("rasterize_gaussians(ortho=True)", graph=graph, tile_rows=tile_rows is not None,
+                           out_peers=out_peers is not None)
     if graph:
         _graph_unsupported("rasterize_gaussians(graph=True)", debug, tile_rows,
                            "out_peers" if out_peers is not None else None)
@@ -205,6 +221,9 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
                                                    graphs.status_word(dev).data_ptr()),
                     "sfgs_rasterize_forward_graph")
             rendered = -1
+        elif ortho:
+            off = _ptr(subpixel_offset, keep) if subpixel_offset is not None else None
+            rendered = N.check(L.sfgs_rasterize_forward_ortho(C.byref(a), off), "sfgs_rasterize_forward_ortho")
         elif subpixel_offset is not None:
             entry = "sfgs_rasterize_forward_subpixel" + ("_peers" if out_peers is not None else "")
             rendered = N.check(getattr(L, entry)(C.byref(a), _ptr(subpixel_offset, keep)), entry)
@@ -251,7 +270,7 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
                                  dL_dout_extra, sh, degree, campos, geomBuffer, R, binningBuffer, imageBuffer,
                                  out_alpha, debug, tile_rows=None, norm_raw=None, phase=0, acc=None,
                                  gauss_range=None, acc_peers=None, peer_slice=0, subpixel_offset=None,
-                                 camera_grad=False, intrinsics_grad=False, graph=False):
+                                 camera_grad=False, intrinsics_grad=False, graph=False, *, ortho=False):
     """Same positional signature and return tuple as the reference's `_C.rasterize_gaussians_backward`.  With
     `norm_raw` (the extra tensor a `fuse_normalize=True` forward returned) `dL_dout_norm` is taken w.r.t. the unit
     normal map and the adjoint of F.normalize is applied inside the blend-adjoint kernel.
@@ -287,7 +306,15 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     `graph=True`: the capture-safe backward (sfgs_rasterize_backward_graph) of a `graph=True` forward; `R` is the
     capacity that forward was given, and `tan_fovx` / `tan_fovy` may be 0-d CUDA tensors.  Every option of the
     one-call backward is taken (offsets, deterministic mode, camera and focal gradients); phases 1 and 2, acc_peers,
-    tile_rows and debug raise."""
+    tile_rows and debug raise.
+
+    `ortho=True`: the backward of an `ortho=True` forward (sfgs_rasterize_backward_ortho), with the same settings and
+    offsets; the deterministic mode is taken as above.  graph, tile_rows, acc_peers, phases 1 and 2 and camera or
+    focal gradients raise SfgsError."""
+    if ortho:
+        _ortho_unsupported("rasterize_gaussians_backward(ortho=True)", graph=graph, tile_rows=tile_rows is not None,
+                           acc_peers=acc_peers is not None, **{f"phase={int(phase)}": int(phase) != 0},
+                           camera_grad=camera_grad, intrinsics_grad=intrinsics_grad)
     if intrinsics_grad and not camera_grad:
         raise ValueError("intrinsics_grad=True needs camera_grad=True")
     if graph:
@@ -399,6 +426,9 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
                                                     tan_fov.data_ptr() if tan_fov is not None else None,
                                                     dL_dcamera.data_ptr() if ncam else None, ncam),
                     "sfgs_rasterize_backward_graph")
+        elif ortho:
+            off = _ptr(subpixel_offset, keep) if subpixel_offset is not None else None
+            N.check(L.sfgs_rasterize_backward_ortho(C.byref(a), off, int(deterministic)), "sfgs_rasterize_backward_ortho")
         elif camera_grad and phase == 2:
             ncam = 37 if intrinsics_grad else 35
             dL_dcamera = torch.empty((ncam,), dtype=torch.float64, device=dev)
