@@ -108,25 +108,41 @@ def forward(means3D, scales, rotations, opacities, shs, sh_degree, viewmatrix, p
     return o
 
 
-def backward(fwd, dL_color, dL_depth, dL_norm, dL_alpha, dL_extra=None):
-    """Backward of `forward` for the given pixel cotangents. Returns the 10 gradient arrays of the reference."""
+def blend_backward(fwd, dL_color, dL_depth, dL_norm, dL_alpha, dL_extra=None):
+    """The blend adjoint of `forward` for the given pixel cotangents: the screen-space sums means2D [P,3], conic [P,4],
+    opacity [P], colors [P,3], depths [P], norm3D [P,3] and extra [P,ED] the per-Gaussian stage starts from."""
     L = lib()
     I = fwd["_inputs"]
     P = I["means3D"].shape[0]
-    W, H, M, ED = I["W"], I["H"], I["M"], I["ED"]
+    W, H, ED = I["W"], I["H"], I["ED"]
     dL_color, dL_depth, dL_norm, dL_alpha, dL_extra = _f(dL_color), _f(dL_depth), _f(dL_norm), _f(dL_alpha), _f(dL_extra)
     colors = I["colors_precomp"] if I["colors_precomp"] is not None else fwd["rgb"]
     norms = I["norm3D_precomp"] if I["norm3D_precomp"] is not None else fwd["norm3D"]
-    cov3D = I["cov3D_precomp"] if I["cov3D_precomp"] is not None else fwd["cov3D"]
     z = lambda *s: np.zeros(s, np.float32)  # noqa: E731
-    g = dict(means2D=z(P, 3), conic=z(P, 4), opacity=z(P), colors=z(P, 3), depths=z(P), means3D=z(P, 3), cov3D=z(P, 6),
-             norm3D=z(P, 3), sh=z(P, M, 3), scales=z(P, 3), rot=z(P, 4), extra=z(P, max(ED, 0)))
+    g = dict(means2D=z(P, 3), conic=z(P, 4), opacity=z(P), colors=z(P, 3), depths=z(P), norm3D=z(P, 3),
+             extra=z(P, max(ED, 0)))
     plist = np.ascontiguousarray(fwd["point_list"])
     L.oracle_render_backward(C.c_int(W), C.c_int(H), C.c_int(ED), _p(fwd["ranges"]), _p(plist), _p(I["bg"]),
                              _p(fwd["means2D"]), _p(fwd["conic_opacity"]), _p(colors), _p(fwd["depths"]), _p(norms),
                              _p(I["extras"]), _p(fwd["alpha"]), _p(fwd["n_contrib"]), _p(dL_color), _p(dL_depth),
                              _p(dL_norm), _p(dL_alpha), _p(dL_extra), _p(g["means2D"]), _p(g["conic"]),
                              _p(g["opacity"]), _p(g["colors"]), _p(g["depths"]), _p(g["norm3D"]), _p(g["extra"]))
+    return g
+
+
+def backward(fwd, dL_color, dL_depth, dL_norm, dL_alpha, dL_extra=None):
+    """Backward of `forward` for the given pixel cotangents. Returns the 10 gradient arrays of the reference."""
+    L = lib()
+    I = fwd["_inputs"]
+    P = I["means3D"].shape[0]
+    W, H, M = I["W"], I["H"], I["M"]
+    norms = I["norm3D_precomp"] if I["norm3D_precomp"] is not None else fwd["norm3D"]
+    cov3D = I["cov3D_precomp"] if I["cov3D_precomp"] is not None else fwd["cov3D"]
+    s = blend_backward(fwd, dL_color, dL_depth, dL_norm, dL_alpha, dL_extra)
+    z = lambda *s: np.zeros(s, np.float32)  # noqa: E731
+    g = dict(means2D=s["means2D"], conic=s["conic"], opacity=s["opacity"], colors=s["colors"], depths=s["depths"],
+             means3D=z(P, 3), cov3D=z(P, 6), norm3D=s["norm3D"], sh=z(P, M, 3), scales=z(P, 3), rot=z(P, 4),
+             extra=s["extra"])
     L.oracle_gauss_backward(C.c_int(P), C.c_int(I["sh_degree"]), C.c_int(M), _p(I["means3D"]), _p(fwd["radii"]),
                             _p(I["shs"]), _p(fwd["clamped"]), _p(I["scales"]), _p(I["rotations"]),
                             C.c_float(I["scale_modifier"]), _p(cov3D), _p(norms),

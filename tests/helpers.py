@@ -1,10 +1,12 @@
 """Shared helpers for the parity tests (test infrastructure)."""
 from __future__ import annotations
 
+import contextlib
 import hashlib
 import os
 
 import numpy as np
+import pytest
 import torch
 
 from sfgs import synthetic as S
@@ -17,8 +19,30 @@ def to_torch(scene: S.Scene, cam: S.Camera, device):
                 projmatrix=t(cam.projmatrix), campos=t(cam.campos))
 
 
+FWD_KEYS = ("num_rendered", "color", "depth", "norm", "alpha", "radii", "extra", "geom", "binning", "img")
+BWD_KEYS = ("means2D", "colors", "opacity", "means3D", "cov3D", "norm3D", "sh", "scales", "rot", "extra",
+            "view", "proj", "campos", "tanx", "tany")
+
+
+class deterministic:
+    """torch.use_deterministic_algorithms(on, warn_only=...) for a block; the previous setting is restored."""
+
+    def __init__(self, on=True, warn_only=False):
+        self.on, self.warn_only = on, warn_only
+
+    def __enter__(self):
+        self.prev = (torch.are_deterministic_algorithms_enabled(), torch.is_deterministic_algorithms_warn_only_enabled())
+        torch.use_deterministic_algorithms(self.on, warn_only=self.warn_only)
+
+    def __exit__(self, *exc):
+        torch.use_deterministic_algorithms(self.prev[0], warn_only=self.prev[1])
+
+
 def run_ours_forward(d, cam, sh_degree, bg, kernel_size=0.1, scale_modifier=1.0, colors=None, debug=False,
-                     extras=None):
+                     extras=None, **kw):
+    """One rasterizer forward as a dict (FWD_KEYS).  cam needs width, height, tanfovx and tanfovy (the half-extents
+    s_x, s_y with ortho=True); d the Gaussians and viewmatrix, projmatrix, campos.  kw: the forward's options
+    (subpixel_offset, tile_rows, ortho, out_planes, out_peers, ...)."""
     from sfgs import rasterizer as R
     e = torch.empty(0, device=d["means3D"].device)
     sh = e if colors is not None else d["shs"]
@@ -26,28 +50,105 @@ def run_ours_forward(d, cam, sh_degree, bg, kernel_size=0.1, scale_modifier=1.0,
     ex, ED = (extras, int(extras.shape[1])) if extras is not None else (e, 0)
     out = R.rasterize_gaussians(bg, d["means3D"], col, d["opacities"], d["scales"], d["rotations"], scale_modifier,
                                 e, e, ex, ED, d["viewmatrix"], d["projmatrix"], cam.tanfovx, cam.tanfovy, kernel_size,
-                                cam.height, cam.width, sh, sh_degree, d["campos"], False, debug)
-    keys = ("num_rendered", "color", "depth", "norm", "alpha", "radii", "extra", "geom", "binning", "img")
-    return dict(zip(keys, out))
+                                cam.height, cam.width, sh, sh_degree, d["campos"], False, debug, **kw)
+    return dict(zip(FWD_KEYS, out))
 
 
 def run_ours_backward(d, cam, sh_degree, bg, fwd, cot, kernel_size=0.1, scale_modifier=1.0, colors=None, debug=False,
-                      extras=None, dL_extra=None, **kw):
+                      extras=None, dL_extra=None, det=None, **kw):
+    """One rasterizer backward as a dict (BWD_KEYS: the ten gradients, then view, proj, campos with camera_grad=True
+    and tanx, tany with intrinsics_grad=True).  A phase-1 call returns the [P,16] blend-adjoint sums and a phase-2
+    call with camera_grad=True the native tuple (its camera partial last).  det: run under
+    torch.use_deterministic_algorithms(det) (None: the current setting).  kw: the backward's options (phase, acc,
+    gauss_range, tile_rows, subpixel_offset, camera_grad, intrinsics_grad, ortho, ...)."""
     from sfgs import rasterizer as R
     e = torch.empty(0, device=d["means3D"].device)
     sh = e if colors is not None else d["shs"]
     col = colors if colors is not None else e
     ex = extras if extras is not None else e
     dex = dL_extra if dL_extra is not None else e
-    out = R.rasterize_gaussians_backward(bg, d["means3D"], fwd["radii"], col, d["scales"], d["rotations"], ex,
-                                         scale_modifier, e, e, d["viewmatrix"], d["projmatrix"], cam.tanfovx,
-                                         cam.tanfovy, kernel_size, cot[0], cot[1], cot[2], cot[3], dex, sh, sh_degree,
-                                         d["campos"], fwd["geom"], fwd["num_rendered"], fwd["binning"], fwd["img"],
-                                         fwd["alpha"], debug, **kw)
-    if kw.get("phase") == 1:
-        return out                      # the [P,16] blend-adjoint sums
-    keys = ("means2D", "colors", "opacity", "means3D", "cov3D", "norm3D", "sh", "scales", "rot", "extra")
-    return dict(zip(keys, out))
+    with deterministic(det) if det is not None else contextlib.nullcontext():
+        out = R.rasterize_gaussians_backward(bg, d["means3D"], fwd["radii"], col, d["scales"], d["rotations"], ex,
+                                             scale_modifier, e, e, d["viewmatrix"], d["projmatrix"], cam.tanfovx,
+                                             cam.tanfovy, kernel_size, cot[0], cot[1], cot[2], cot[3], dex, sh,
+                                             sh_degree, d["campos"], fwd["geom"], fwd["num_rendered"], fwd["binning"],
+                                             fwd["img"], fwd["alpha"], debug, **kw)
+    if kw.get("phase") == 1 or (kw.get("phase") == 2 and kw.get("camera_grad")):
+        return out
+    return dict(zip(BWD_KEYS, out))
+
+
+def bits(t):
+    """A tensor to compare bit for bit: floating point as its int32 words, anything else as it is."""
+    return t.contiguous().view(torch.int32) if t.dtype.is_floating_point else t
+
+
+def uniform_offsets(H, W, dev, seed):
+    """Subpixel offsets U(-0.5, 0.5) [H,W,2] of a seeded device generator."""
+    g = torch.Generator(device=dev).manual_seed(seed)
+    return torch.rand((H, W, 2), generator=g, device=dev) - 0.5
+
+
+def restatement_inputs(f, d, cam, D, bg, cot, colors=None, off=None, det=True):
+    """chain_f64.chain's inputs for the forward f: the phase-1 blend-adjoint sums of a backward (deterministic by
+    default: the same `acc` bits the deterministic gradient calls use) and the forward's internals (cov3D, combined
+    opacity, clamp flags and blended normals)."""
+    acc = run_ours_backward(d, cam, D, bg, f, cot, colors=colors, det=det, phase=1, subpixel_offset=off)
+    P = d["means3D"].shape[0]
+    I = our_internals(f, P, cam.height, cam.width)
+    clamped = torch.stack([(I["clamped"].int() >> ch) & 1 for ch in range(3)], 1) != 0
+    return dict(acc=acc, radii=f["radii"], means3D=d["means3D"], cov3D=I["cov3D"], combined_opacity=I["rec"][:, 5],
+                clamped=clamped, shs=None if colors is not None else d["shs"], D=D, viewmatrix=d["viewmatrix"],
+                projmatrix=d["projmatrix"], campos=d["campos"], W=cam.width, H=cam.height, tan_fovx=cam.tanfovx,
+                tan_fovy=cam.tanfovy, kernel_size=0.1, norm_rec=I["norm3D"])
+
+
+# ----------------------------------------------------------------------------- cached frames
+_CACHE = {}
+
+
+def cached(slot, key, make):
+    """make()'s value for `key`, kept until another key is asked for in the same slot: one 1M-Gaussian frame (or one
+    result computed on it) per slot at a time.  The previous value is dropped before make() runs."""
+    if _CACHE.get(slot, (None,))[0] != key:
+        _CACHE.pop(slot, None)
+        _CACHE[slot] = (key, make())
+    return _CACHE[slot][1]
+
+
+@pytest.fixture(scope="module", autouse=True)
+def release_cached_frames():
+    """The frames and results cached between a module's tests are freed when it is done (import it by name)."""
+    yield
+    _CACHE.clear()
+    if torch.cuda.is_available():
+        torch.cuda.empty_cache()
+
+
+def _make_frame(name):
+    D = 1 if name.startswith("m4") or name == "precomp" else 3
+    if name == "clamp":
+        scene = S.city_scene(200_000, seed=4, sh_degree=3, extent=128.0)
+        scene.scales *= 8.0         # ~1700 rasterized Gaussians beyond the clamp bound in y
+        cam = S.jax004_camera(640, 360)
+    else:
+        scene = S.city_scene(1_000_000, seed=0, sh_degree=D)
+        cam = S.orbit_camera(width=1920, height=1080) if name == "orbit" else S.jax004_camera(1920, 1080)
+    colors = None
+    if name == "precomp":
+        colors = np.random.default_rng(5).uniform(0, 1, size=(scene.P, 3)).astype(np.float32)
+    return scene, cam, D, colors
+
+
+def frame(name, dev):
+    """The benched frames (1M Gaussians, 1920x1080: JAX_004 and the whole-scene orbit) at SH degree 3, the JAX_004
+    frame at SH degree 1 (M = 4) with SH or with precomputed colours, and 'clamp': the JAX_004 frame of a small city
+    whose Gaussians extend beyond the frustum clamp bound.  Returns scene, cam, D, the device tensors and the
+    colours."""
+    scene, cam, D, colors = cached("frame", name, lambda: _make_frame(name))
+    d = to_torch(scene, cam, dev)
+    col = torch.from_numpy(colors).to(dev) if colors is not None else None
+    return scene, cam, D, d, col
 
 
 def run_ref_forward(d, cam, sh_degree, bg, kernel_size=0.1, scale_modifier=1.0, colors=None):

@@ -9,10 +9,7 @@ dtype), what sfgs_rasterize_forward_ortho's preprocess computes per Gaussian (in
   - the SH colour along the view's +z axis normalize(viewmatrix[0:3, 2]) (+0.5, clamped at 0), one direction per frame;
   - the normal: the shortest scale axis of the rotation, flipped so that it does not point along the view axis.
 `render` blends the restated records with the CPU oracle's blend (tests/subpixel_oracle.c, which includes the
-unchanged oracle), with or without subpixel offsets.  `chain` is the per-Gaussian adjoint's chain for given blend-adjoint
-sums: the autograd gradient of  sum_g <acc_g, outputs_g>, with the conic inverse and the Mip coefficient entering
-through the kernel's own local derivatives (as in camera_chain_f64.py) and the normal's adjoint sign taken by the
-kernel's rule.
+unchanged oracle), with or without subpixel offsets.  The per-Gaussian adjoint's chain is chain_f64.chain(ortho=True).
 """
 from __future__ import annotations
 
@@ -21,41 +18,15 @@ import ctypes as C
 import numpy as np
 import torch
 
-from camera_chain_f64 import eval_sh
+from chain_f64 import axis_index, cov3d, eval_sh, quat_to_rot, sym6_to_mat, view_axis  # noqa: F401
 
 TILE = 16
-
-
-def quat_to_rot(q):
-    """The library's rotation of an un-normalised quaternion (r, x, y, z): R[a][b] with Sigma = R diag(s^2) R^T."""
-    r, x, y, z = q[:, 0], q[:, 1], q[:, 2], q[:, 3]
-    return torch.stack([
-        torch.stack([1 - 2 * (y * y + z * z), 2 * (x * y - r * z), 2 * (x * z + r * y)], -1),
-        torch.stack([2 * (x * y + r * z), 1 - 2 * (x * x + z * z), 2 * (y * z - r * x)], -1),
-        torch.stack([2 * (x * z - r * y), 2 * (y * z + r * x), 1 - 2 * (x * x + y * y)], -1)], -2)
-
-
-def sym6_to_mat(c):
-    return torch.stack([c[:, [0, 1, 2]], c[:, [1, 3, 4]], c[:, [2, 4, 5]]], 1)
 
 
 def pixel_scales(W, H, s_x, s_y):
     """The library's float32 h_x = W / (2 s_x), h_y = H / (2 s_y)."""
     f32 = np.float32
     return float(f32(W) / (f32(2.0) * f32(s_x))), float(f32(H) / (f32(2.0) * f32(s_y)))
-
-
-def view_axis(viewmatrix, dtype=torch.float64):
-    """The world-space unit vector of the view's +z axis (the SH and normal view direction)."""
-    V = torch.as_tensor(viewmatrix).reshape(4, 4).to(dtype)
-    d = V[:3, 2]
-    return d / torch.sqrt((d * d).sum())
-
-
-def _axis_index(scales):
-    """Index of the shortest-axis rule of the normal: z if sx > sz and sy > sz, else y if sx > sy and sz > sy, else x."""
-    sx, sy, sz = scales[:, 0], scales[:, 1], scales[:, 2]
-    return torch.where((sx > sz) & (sy > sz), 2, torch.where((sx > sy) & (sz > sy), 1, 0))
 
 
 def project(means3D, scales, rotations, viewmatrix, projmatrix, W, H, s_x, s_y, kernel_size, scale_modifier=1.0,
@@ -71,9 +42,7 @@ def project(means3D, scales, rotations, viewmatrix, projmatrix, W, H, s_x, s_y, 
     pix = torch.stack([((ndc[:, 0] + 1.0) * W - 1.0) * 0.5, ((ndc[:, 1] + 1.0) * H - 1.0) * 0.5], 1)
     Rm = quat_to_rot(rotations)
     if cov3D is None:
-        s = scale_modifier * scales
-        Sig = Rm @ torch.diag_embed(s * s) @ Rm.transpose(1, 2)
-        cov3D = torch.stack([Sig[:, 0, 0], Sig[:, 0, 1], Sig[:, 0, 2], Sig[:, 1, 1], Sig[:, 1, 2], Sig[:, 2, 2]], 1)
+        cov3D = cov3d(scale_modifier * scales, Rm)
     h_x, h_y = pixel_scales(W, H, s_x, s_y)
     T0, T1 = h_x * V[:3, 0], h_y * V[:3, 1]        # rows of T = J W, W[r][k] = viewmatrix[k][r]
     S = sym6_to_mat(cov3D)
@@ -121,7 +90,7 @@ def preprocess(means3D, scales, rotations, opacities, viewmatrix, projmatrix, W,
         v = eval_sh(int(D), f(shs), d.expand(m.shape[0], 3)) + 0.5
         clamped = v < 0
         rgb = torch.where(clamped, torch.zeros_like(v), v)
-    ax = _axis_index(sc)
+    ax = axis_index(sc)
     n = g["R"][torch.arange(m.shape[0]), :, ax]              # R e_axis
     n = torch.where(((n @ d) > 0)[:, None], -n, n)
     z = lambda x: torch.where(vis.reshape(-1, *([1] * (x.ndim - 1))), x, torch.zeros_like(x))  # noqa: E731
@@ -168,83 +137,6 @@ def render(pre, W, H, bg, subpixel_offset=None):
         C.c_int(W), C.c_int(H), C.c_int(0), p(np.ascontiguousarray(ranges)), p(np.ascontiguousarray(plist)),
         p(means2D), p(rgb), p(nrm), p(dep), None, p(co), p(f32(bg)), p(out["color"]), p(out["depth"]), p(out["norm"]),
         p(out["alpha"]), None, p(n_contrib), p(off))
-    return out
-
-
-def chain(acc, visible, means3D, scales, rotations, opacities, viewmatrix, projmatrix, W, H, s_x, s_y, kernel_size,
-          D=0, shs=None, clamped=None, norm_rec=None, dtype=torch.float64):
-    """The per-Gaussian adjoint of an orthographic frame for blend-adjoint sums acc [P,16] (the library's acc rows:
-    colour 3, depth, normal 3, mean2D 3, conic xx xy yy, opacity, 0, 0), by autograd in `dtype`.
-
-    visible [P] bool (radii > 0); clamped [P,3] bool and norm_rec [P,3] (the forward's clamp flags and blended normals,
-    which fix the adjoint's control flow).  Returns the ten gradients of sfgs_rasterize_backward_ortho (extra is empty)
-    as CPU tensors: means2D, colors, opacity [P,1], means3D, cov3D, norm3D, sh, scales, rot; rows of culled Gaussians
-    are 0."""
-    f = lambda a: torch.as_tensor(a).detach().cpu().to(dtype)  # noqa: E731
-    vis = torch.as_tensor(visible).cpu().bool()
-    idx = torch.nonzero(vis).flatten()
-    P = int(vis.numel())
-    A = f(acc)[idx]
-    m = f(means3D)[idx].clone().requires_grad_(True)
-    sc = f(scales)[idx].clone().requires_grad_(True)
-    q = f(rotations)[idx].clone().requires_grad_(True)
-    g = project(m, sc, q, viewmatrix, projmatrix, W, H, s_x, s_y, kernel_size)
-    cov = g["cov3D"]
-    cov.retain_grad()
-    ks = float(np.float32(kernel_size))
-    c00, c01, c11 = g["c00"], g["c01"], g["c11"]
-    L = A[:, 7] * g["ndc"][:, 0] + A[:, 8] * g["ndc"][:, 1] + A[:, 3] * g["t"][:, 2]
-    with torch.no_grad():
-        # the kernel's dL/d(c00, c01, c11): the conic inverse with its 1e-7 guard, plus the Mip coefficient's share
-        dLcx, dLcy, dLcz, o_opac = A[:, 10], A[:, 11], A[:, 12], A[:, 13]
-        a, b, c = c00 + ks, c01, c11 + ks
-        denom = a * c - b * b
-        d2i = 1.0 / (denom * denom + 1e-7)
-        dL_da = d2i * (-c * c * dLcx + 2 * b * c * dLcy + (denom - a * c) * dLcz)
-        dL_dc = d2i * (-a * a * dLcz + 2 * a * b * dLcy + (denom - a * c) * dLcx)
-        dL_db = d2i * 2 * (b * c * dLcx - (denom + 2 * b * b) * dLcy + a * b * dLcz)
-        det0 = (c00 * c11 - c01 * c01).clamp_min(1e-6)
-        det1 = (a * c - b * b).clamp_min(1e-6)
-        coef = torch.sqrt(det0 / (det1 + 1e-6) + 1e-6)
-        ok = ((det0 > 1e-6) & (det1 > 1e-6)).to(dtype)
-        dsq = o_opac * f(opacities).reshape(-1)[idx] * 0.5 / (coef + 1e-6)
-        dd0, dd1 = dsq / (det1 + 1e-6), dsq * det0 * (-1.0 / (det1 * det1 + 1e-6))
-        dL_da = dL_da + ok * (dd0 * c11 + dd1 * (c11 + ks))
-        dL_db = dL_db + ok * (dd0 * (-2 * c01) + dd1 * (-2 * c01))
-        dL_dc = dL_dc + ok * (dd0 * c00 + dd1 * (c00 + ks))
-        g_opac = (o_opac * coef * ok)[:, None]
-    L = L + dL_da * c00 + dL_db * c01 + dL_dc * c11
-    # the normal R e_axis: the adjoint takes its sign from (R^T e_axis) . n_rec, the rule of computeNorm3D's backward
-    ax = _axis_index(sc.detach())
-    ar = torch.arange(idx.numel())
-    n = g["R"][ar, :, ax]
-    with torch.no_grad():
-        rt = g["R"].transpose(1, 2)[ar, :, ax]
-        sgn = torch.where((rt * f(norm_rec)[idx]).sum(1) < 0, -1.0, 1.0).to(dtype)
-    L = L + (A[:, 4:7] * n * sgn[:, None]).sum(1)
-    shv = None
-    if shs is not None:
-        shv = f(shs)[idx].clone().requires_grad_(True)
-        d = view_axis(viewmatrix, dtype).expand(idx.numel(), 3)
-        rgb = eval_sh(int(D), shv, d)
-        keep = (~torch.as_tensor(clamped).cpu().bool()[idx]).to(dtype)
-        L = L + (keep * A[:, 0:3] * rgb).sum(1)
-    L.sum().backward()
-    z = lambda *s: torch.zeros(s, dtype=dtype)  # noqa: E731
-    out = dict(means2D=z(P, 3), colors=z(P, 3), opacity=z(P, 1), means3D=z(P, 3), cov3D=z(P, 6), norm3D=z(P, 3),
-               scales=z(P, 3), rot=z(P, 4))
-    out["means2D"][idx] = A[:, 7:10]
-    out["colors"][idx] = A[:, 0:3]
-    out["opacity"][idx] = g_opac
-    out["means3D"][idx] = m.grad
-    out["cov3D"][idx] = cov.grad
-    out["norm3D"][idx] = A[:, 4:7]
-    out["scales"][idx] = sc.grad
-    out["rot"][idx] = q.grad
-    if shs is not None:
-        M = int(torch.as_tensor(shs).shape[1])
-        out["sh"] = z(P, M, 3)
-        out["sh"][idx] = shv.grad
     return out
 
 

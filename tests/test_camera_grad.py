@@ -1,5 +1,5 @@
 """Camera gradients (sfgs_rasterize_backward_camera): dL/dviewmatrix, dL/dprojmatrix and dL/dcampos, the adjoint of the
-chain dL_dmean3D differentiates.  The oracle is tests/camera_chain_f64.py: for given blend-adjoint sums it restates
+chain dL_dmean3D differentiates.  The oracle is tests/chain_f64.py: for given blend-adjoint sums it restates
 that chain in torch, and its gradient with respect to means3D must reproduce the library's dL_dmean3D.
 
 CPU: the C ABI's argument checks, the autograd layer's native call sequence (the reference's own render() on a
@@ -13,9 +13,10 @@ import numpy as np
 import pytest
 import torch
 
-import camera_chain_f64 as CC
+import chain_f64 as CH
 import golden_cases as G
 import helpers as Hh
+from helpers import release_cached_frames  # noqa: F401
 from sfgs import synthetic as S
 
 SFGS_E_BADARG, SFGS_E_UNSUPPORTED = -2, -4
@@ -182,24 +183,11 @@ def _oracle_case(name):
                   cam.viewmatrix, cam.projmatrix, cam.campos, cam.width, cam.height, cam.tanfovx, cam.tanfovy, bg,
                   kernel_size=kw["kernel_size"], scale_modifier=kw["scale_modifier"], colors_precomp=colors)
     g = O.backward(o, *kw["cot"])
-    # the blend adjoint's sums alone (O.backward's per-Gaussian stage rewrites the opacity row)
-    L = O.lib()
-    P, W, H = scene.P, cam.width, cam.height
-    f = lambda a: np.ascontiguousarray(a, np.float32)  # noqa: E731
-    s = dict(means2D=np.zeros((P, 3), np.float32), conic=np.zeros((P, 4), np.float32), opacity=np.zeros(P, np.float32),
-             colors=np.zeros((P, 3), np.float32), depths=np.zeros(P, np.float32), norm3D=np.zeros((P, 3), np.float32))
-    cot = [f(c) for c in kw["cot"]]
-    cols = f(colors) if colors is not None else o["rgb"]
-    p = O._p
-    L.oracle_render_backward(C.c_int(W), C.c_int(H), C.c_int(0), p(o["ranges"]), p(np.ascontiguousarray(o["point_list"])),
-                             p(f(bg)), p(o["means2D"]), p(o["conic_opacity"]), p(cols), p(o["depths"]), p(o["norm3D"]),
-                             None, p(o["alpha"]), p(o["n_contrib"]), p(cot[0]), p(cot[1]), p(cot[2]), p(cot[3]), None,
-                             p(s["means2D"]), p(s["conic"]), p(s["opacity"]), p(s["colors"]), p(s["depths"]),
-                             p(s["norm3D"]), None)
-    acc = CC.acc_from_screen_grads(s["means2D"], s["colors"], s["depths"], s["norm3D"], s["conic"], s["opacity"])
-    r = CC.camera_chain(acc, o["radii"], scene.means3D, o["cov3D"], o["conic_opacity"][:, 3], o["clamped"] != 0,
-                        None if colors is not None else scene.shs, kw["sh_degree"], cam.viewmatrix, cam.projmatrix,
-                        cam.campos, W, H, cam.tanfovx, cam.tanfovy, kw["kernel_size"])
+    s = O.blend_backward(o, *kw["cot"])
+    acc = CH.acc_from_screen_grads(s["means2D"], s["colors"], s["depths"], s["norm3D"], s["conic"], s["opacity"])
+    r = CH.chain(acc, o["radii"], scene.means3D, o["conic_opacity"][:, 3], o["clamped"] != 0,
+                 None if colors is not None else scene.shs, kw["sh_degree"], cam.viewmatrix, cam.projmatrix, cam.campos,
+                 cam.width, cam.height, cam.tanfovx, cam.tanfovy, kw["kernel_size"], cov3D=o["cov3D"])
     return scene, cam, g, r
 
 
@@ -216,89 +204,16 @@ def test_restatement_reproduces_the_oracle_mean_gradient(name):
 @pytest.mark.parametrize("name", G.CASES)
 def test_translation_identity_of_the_restatement(name):
     scene, cam, g, r = _oracle_case(name)
-    res, scale = CC.translation_residual(r, cam.viewmatrix, cam.projmatrix)
+    res, scale = CH.translation_residual(r, cam.viewmatrix, cam.projmatrix)
     assert (res.abs() <= 1e-12 * scale + 1e-300).all(), (name, res, scale)
 
 
 # ----------------------------------------------------------------------------- GPU helpers
-_FRAMES = {}
-_ACC = {}
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _release_cached_frames():
-    """The 1M-Gaussian frames and results cached between this module's tests are freed when it is done."""
-    yield
-    _FRAMES.clear()
-    _ACC.clear()
-    if torch.cuda.is_available():
-        torch.cuda.empty_cache()
-
-
-def _frame(name, dev):
-    """The benched frames (1M Gaussians, 1920x1080: JAX_004 and the whole-scene orbit) at SH degree 3, and the JAX_004
-    frame at SH degree 1 (M = 4) with SH or with precomputed colours."""
-    if name not in _FRAMES:
-        D = 1 if name.startswith("m4") or name == "precomp" else 3
-        scene = S.city_scene(1_000_000, seed=0, sh_degree=D)
-        cam = S.orbit_camera(width=1920, height=1080) if name == "orbit" else S.jax004_camera(1920, 1080)
-        colors = None
-        if name == "precomp":
-            colors = np.random.default_rng(5).uniform(0, 1, size=(scene.P, 3)).astype(np.float32)
-        _FRAMES.clear()             # one 1M frame on the device at a time
-        _FRAMES[name] = (scene, cam, D, colors)
-    scene, cam, D, colors = _FRAMES[name]
-    d = Hh.to_torch(scene, cam, dev)
-    col = torch.from_numpy(colors).to(dev) if colors is not None else None
-    return scene, cam, D, d, col
-
-
-def _fwd(d, cam, D, bg, colors=None, off=None):
-    from sfgs import rasterizer as R
-    e = torch.empty(0, device=d["means3D"].device)
-    out = R.rasterize_gaussians(bg, d["means3D"], colors if colors is not None else e, d["opacities"], d["scales"],
-                                d["rotations"], 1.0, e, e, e, 0, d["viewmatrix"], d["projmatrix"], cam.tanfovx,
-                                cam.tanfovy, 0.1, cam.height, cam.width, e if colors is not None else d["shs"], D,
-                                d["campos"], False, False, subpixel_offset=off)
-    return dict(zip(("num_rendered", "color", "depth", "norm", "alpha", "radii", "extra", "geom", "binning", "img"),
-                    out))
-
-
-def _bwd(d, cam, D, bg, f, cot, colors=None, off=None, det=False, camera=False, **kw):
-    """One backward; with camera=True also 'view', 'proj', 'campos'.  det: under torch.use_deterministic_algorithms."""
-    from sfgs import rasterizer as R
-    e = torch.empty(0, device=d["means3D"].device)
-    prev = torch.are_deterministic_algorithms_enabled()
-    torch.use_deterministic_algorithms(det)
-    try:
-        out = R.rasterize_gaussians_backward(
-            bg, d["means3D"], f["radii"], colors if colors is not None else e, d["scales"], d["rotations"], e, 1.0, e,
-            e, d["viewmatrix"], d["projmatrix"], cam.tanfovx, cam.tanfovy, 0.1, cot[0], cot[1], cot[2], cot[3], e,
-            e if colors is not None else d["shs"], D, d["campos"], f["geom"], f["num_rendered"], f["binning"],
-            f["img"], f["alpha"], False, subpixel_offset=off, camera_grad=camera, **kw)
-    finally:
-        torch.use_deterministic_algorithms(prev)
-    if kw.get("phase") == 1:
-        return out
-    keys = ("means2D", "colors", "opacity", "means3D", "cov3D", "norm3D", "sh", "scales", "rot", "extra", "view", "proj",
-            "campos")
-    return dict(zip(keys, out))
-
-
-def _bits(t):
-    return t.contiguous().view(torch.int32)
-
-
-def _uniform(H, W, dev, seed):
-    g = torch.Generator(device=dev).manual_seed(seed)
-    return torch.rand((H, W, 2), generator=g, device=dev) - 0.5
-
-
 def _setup(name, dev, jitter, seed=6):
-    scene, cam, D, d, colors = _frame(name, dev)
+    scene, cam, D, d, colors = Hh.frame(name, dev)
     bg = torch.tensor([0.1, 0.2, 0.3], device=dev)
-    off = _uniform(cam.height, cam.width, dev, 23) if jitter else None
-    f = _fwd(d, cam, D, bg, colors, off)
+    off = Hh.uniform_offsets(cam.height, cam.width, dev, 23) if jitter else None
+    f = Hh.run_ours_forward(d, cam, D, bg, colors=colors, subpixel_offset=off)
     cot = [torch.from_numpy(c).to(dev) for c in S.cotangents(cam.width, cam.height, seed=seed)]
     return scene, cam, D, d, colors, bg, off, f, cot
 
@@ -317,12 +232,12 @@ def test_other_outputs_unchanged(cuda_device, name):
     for jitter in (False, True):
         scene, cam, D, d, colors, bg, off, f, cot = _setup(name, dev, jitter)
         keys = [k for k in GRAD_KEYS if not (colors is not None and k == "sh")]
-        a = _bwd(d, cam, D, bg, f, cot, colors, off, det=True)
-        b = _bwd(d, cam, D, bg, f, cot, colors, off, det=True, camera=True)
+        a = Hh.run_ours_backward(d, cam, D, bg, f, cot, colors=colors, subpixel_offset=off, det=True)
+        b = Hh.run_ours_backward(d, cam, D, bg, f, cot, colors=colors, subpixel_offset=off, det=True, camera_grad=True)
         for k in keys:
-            assert torch.equal(_bits(a[k]), _bits(b[k])), (name, jitter, "deterministic", k)
-        g1, g2 = (_bwd(d, cam, D, bg, f, cot, colors, off) for _ in range(2))
-        gc = _bwd(d, cam, D, bg, f, cot, colors, off, camera=True)
+            assert torch.equal(Hh.bits(a[k]), Hh.bits(b[k])), (name, jitter, "deterministic", k)
+        g1, g2 = (Hh.run_ours_backward(d, cam, D, bg, f, cot, colors=colors, subpixel_offset=off) for _ in range(2))
+        gc = Hh.run_ours_backward(d, cam, D, bg, f, cot, colors=colors, subpixel_offset=off, camera_grad=True)
         for k in [k for k in keys if k in ("means2D", "colors", "opacity", "norm3D", "sh")]:
             spread = (g1[k].double() - g2[k].double()).abs().max().item()
             err = (gc[k].double() - g1[k].double()).abs().max().item()
@@ -331,25 +246,18 @@ def test_other_outputs_unchanged(cuda_device, name):
         assert all(torch.isfinite(gc[k]).all() for k in ("view", "proj", "campos"))
 
 
-
 def _accuracy_case(case, dev):
     """GPU camera gradients of a deterministic call and the restatement (float64 and float32) from the phase-1 sums of
     a deterministic run: the same `acc` bits the camera call uses."""
-    if case in _ACC:
-        return _ACC[case]
-    name = {"d3": "jax004", "d1": "m4", "precomp": "precomp"}[case.split("_")[0]]
-    scene, cam, D, d, colors, bg, off, f, cot = _setup(name, dev, case.endswith("jitter"))
-    g = _bwd(d, cam, D, bg, f, cot, colors, off, det=True, camera=True)
-    acc = _bwd(d, cam, D, bg, f, cot, colors, off, det=True, phase=1)
-    I = Hh.our_internals(f, scene.P, cam.height, cam.width)
-    clamped = torch.stack([(I["clamped"].int() >> ch) & 1 for ch in range(3)], 1) != 0
-    args = (acc, f["radii"], d["means3D"], I["cov3D"], I["rec"][:, 5], clamped, None if colors is not None else d["shs"],
-            D, d["viewmatrix"], d["projmatrix"], d["campos"], cam.width, cam.height, cam.tanfovx, cam.tanfovy, 0.1)
-    r64 = CC.camera_chain(*args, dtype=torch.float64)
-    r32 = CC.camera_chain(*args, dtype=torch.float32)
-    _ACC.clear()
-    _ACC[case] = (cam, d, g, r64, r32, colors)
-    return _ACC[case]
+    def make():
+        name = {"d3": "jax004", "d1": "m4", "precomp": "precomp"}[case.split("_")[0]]
+        scene, cam, D, d, colors, bg, off, f, cot = _setup(name, dev, case.endswith("jitter"))
+        g = Hh.run_ours_backward(d, cam, D, bg, f, cot, colors=colors, subpixel_offset=off, det=True, camera_grad=True)
+        a = Hh.restatement_inputs(f, d, cam, D, bg, cot, colors, off)
+        r64 = CH.chain(**a, dtype=torch.float64)
+        r32 = CH.chain(**a, dtype=torch.float32)
+        return cam, d, g, r64, r32, colors
+    return Hh.cached("case", case, make)
 
 
 def _flat(r):
@@ -381,7 +289,7 @@ def test_translation_identity_at_1080p(cuda_device):
     cam, d, g, r64, _, _ = _accuracy_case("d3", cuda_device)
     gg = dict(means3D=g["means3D"].double(), view=g["view"].double(), proj=g["proj"].double(),
               campos=g["campos"].double())
-    res, _ = CC.translation_residual(gg, d["viewmatrix"].double(), d["projmatrix"].double())
+    res, _ = CH.translation_residual(gg, d["viewmatrix"].double(), d["projmatrix"].double())
     Vm, Pm = d["viewmatrix"].double().reshape(4, 4), d["projmatrix"].double().reshape(4, 4)
     a = r64["abs"].double()
     scale = (g["means3D"].double().abs().sum(0) + a[32:35] + (Vm[:3].abs() * a[12:16]).sum(1)
@@ -394,10 +302,11 @@ def test_deterministic_camera_gradients_are_reproducible(cuda_device):
     dev = cuda_device
     for jitter in (False, True):
         scene, cam, D, d, colors, bg, off, f, cot = _setup("jax004", dev, jitter)
-        runs = [_bwd(d, cam, D, bg, f, cot, colors, off, det=True, camera=True) for _ in range(3)]
+        runs = [Hh.run_ours_backward(d, cam, D, bg, f, cot, colors=colors, subpixel_offset=off, det=True,
+                                     camera_grad=True) for _ in range(3)]
         for k in ("view", "proj", "campos"):
             for r in runs[1:]:
-                assert torch.equal(_bits(runs[0][k]), _bits(r[k])), (jitter, k)
+                assert torch.equal(Hh.bits(runs[0][k]), Hh.bits(r[k])), (jitter, k)
 
 
 def _so3(w):

@@ -11,24 +11,11 @@ import torch
 
 import helpers as Hh
 from golden_cases import build_case
+from helpers import deterministic
 from sfgs import synthetic as S
 
 SFGS_E_UNSUPPORTED = -4
 GRAD_KEYS = ("means2D", "colors", "opacity", "means3D", "cov3D", "norm3D", "sh", "scales", "rot", "extra")
-
-
-class deterministic:
-    """torch.use_deterministic_algorithms(on, warn_only=...) for a block; the previous setting is restored."""
-
-    def __init__(self, on=True, warn_only=False):
-        self.on, self.warn_only = on, warn_only
-
-    def __enter__(self):
-        self.prev = (torch.are_deterministic_algorithms_enabled(), torch.is_deterministic_algorithms_warn_only_enabled())
-        torch.use_deterministic_algorithms(self.on, warn_only=self.warn_only)
-
-    def __exit__(self, *exc):
-        torch.use_deterministic_algorithms(self.prev[0], warn_only=self.prev[1])
 
 
 # ----------------------------------------------------------------------------- CPU
@@ -146,19 +133,13 @@ def _setup(scene, cam, dev, bg=(0.0, 0.0, 0.0), cot_seed=1, **kw):
     return d, bg_t, sh_degree, f, cot
 
 
-def _det_backward(d, cam, sh_degree, bg, f, cot, **kw):
-    with deterministic(True):
-        return Hh.run_ours_backward(d, cam, sh_degree, bg, f, cot, **kw)
-
-
-def _bits(out):
-    if isinstance(out, torch.Tensor):
-        return [out.contiguous().view(torch.int32).cpu()]
-    return [out[k].contiguous().view(torch.int32).cpu() for k in GRAD_KEYS]
+def _run_bits(out):
+    """The bits of a phase-1 call's sums, or of a backward's gradients, on the host."""
+    return [Hh.bits(t).cpu() for t in ([out] if isinstance(out, torch.Tensor) else [out[k] for k in GRAD_KEYS])]
 
 
 def _assert_three_runs_identical(d, cam, sh_degree, bg, f, cot, **kw):
-    runs = [_bits(_det_backward(d, cam, sh_degree, bg, f, cot, **kw)) for _ in range(3)]
+    runs = [_run_bits(Hh.run_ours_backward(d, cam, sh_degree, bg, f, cot, det=True, **kw)) for _ in range(3)]
     for r in runs[1:]:
         for a, b, k in zip(runs[0], r, GRAD_KEYS):
             assert torch.equal(a, b), f"{k} differs between deterministic runs"
@@ -179,19 +160,14 @@ def test_bit_reproducible(cuda_device, case):
         P = 1_000_000 if case.startswith("configs1") else 5_000_000
         scene, cam, bg = S.city_scene(P, seed=0), S.jax004_camera(1920, 1080), (0.0, 0.0, 0.0)
     if case == "banded":
-        from sfgs import rasterizer as R
         d = Hh.to_torch(scene, cam, dev)
         bg_t = torch.tensor(bg, device=dev)
-        e = torch.empty(0, device=dev)
         band = (3, 15)
-        f = R.rasterize_gaussians(bg_t, d["means3D"], e, d["opacities"], d["scales"], d["rotations"], 1.0, e, e, e, 0,
-                                  d["viewmatrix"], d["projmatrix"], cam.tanfovx, cam.tanfovy, 0.1, cam.height,
-                                  cam.width, d["shs"], 3, d["campos"], False, False, tile_rows=band)
-        f = dict(zip(("num_rendered", "color", "depth", "norm", "alpha", "radii", "extra", "geom", "binning", "img"), f))
+        f = Hh.run_ours_forward(d, cam, 3, bg_t, tile_rows=band)
         cot = [torch.from_numpy(c).to(dev) for c in S.cotangents(cam.width, cam.height, seed=2)]
         _assert_three_runs_identical(d, cam, 3, bg_t, f, cot, tile_rows=band)
         # the band's deterministic gradients match its default ones up to the sums' order
-        g_det = _det_backward(d, cam, 3, bg_t, f, cot, tile_rows=band)
+        g_det = Hh.run_ours_backward(d, cam, 3, bg_t, f, cot, tile_rows=band, det=True)
         g_def = Hh.run_ours_backward(d, cam, 3, bg_t, f, cot, tile_rows=band)
         for k in GRAD_KEYS[:-1]:
             assert (g_det[k] - g_def[k]).abs().max().item() <= 1e-5 + 2e-4 * g_def[k].abs().max().item(), k
@@ -233,7 +209,7 @@ def test_accurate_against_float64(cuda_device, tag):
     d, bg_t, sh, f, cot = _setup(scene, cam, dev, bg=bg, cot_seed=cs)
     P, H, W = scene.P, cam.height, cam.width
     oi = Hh.our_internals(f, P, H, W)
-    gb = _det_backward(d, cam, sh, bg_t, f, cot)
+    gb = Hh.run_ours_backward(d, cam, sh, bg_t, f, cot, det=True)
     if F.live:
         from oracle import ref_cuda
         ref = Hh.run_ref_forward(d, cam, sh, bg_t)
@@ -253,10 +229,11 @@ def test_two_phase_equals_single_call(cuda_device):
     dev = cuda_device
     scene, cam = S.blob_scene(5000, seed=91), S.simple_camera(256, 144)
     d, bg_t, sh, f, cot = _setup(scene, cam, dev, bg=(0.3, 0.2, 0.1), cot_seed=4)
-    one = _det_backward(d, cam, sh, bg_t, f, cot)
-    acc = _det_backward(d, cam, sh, bg_t, f, cot, phase=1)
-    assert torch.equal(acc.view(torch.int32), _det_backward(d, cam, sh, bg_t, f, cot, phase=1).view(torch.int32))
-    two = _det_backward(d, cam, sh, bg_t, f, cot, phase=2, acc=acc, gauss_range=(0, scene.P))
+    one = Hh.run_ours_backward(d, cam, sh, bg_t, f, cot, det=True)
+    acc = Hh.run_ours_backward(d, cam, sh, bg_t, f, cot, det=True, phase=1)
+    assert torch.equal(acc.view(torch.int32),
+                       Hh.run_ours_backward(d, cam, sh, bg_t, f, cot, det=True, phase=1).view(torch.int32))
+    two = Hh.run_ours_backward(d, cam, sh, bg_t, f, cot, det=True, phase=2, acc=acc, gauss_range=(0, scene.P))
     for k in GRAD_KEYS[:-1]:
         assert torch.equal(one[k].view(torch.int32), two[k].view(torch.int32)), k
 

@@ -15,6 +15,7 @@ import torch
 
 import helpers as Hh
 from golden_cases import CASES, build_case
+from helpers import bits
 from sfgs import synthetic as S
 
 pytestmark = pytest.mark.gpu
@@ -30,10 +31,6 @@ def ref_available():
 def ref_internals(ref, P, H, W):
     from oracle import ref_cuda
     return ref_cuda.internals(ref, P, H, W) if ref is not None else None
-
-
-def bits(t):
-    return t.contiguous().view(torch.int32) if t.dtype.is_floating_point else t
 
 
 def run_pair(scene, cam, dev, bg=(0.1, 0.2, 0.3), colors=None, live=True, **kw):

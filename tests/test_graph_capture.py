@@ -11,6 +11,7 @@ import numpy as np
 import pytest
 import torch
 
+from helpers import deterministic
 from sfgs import graphs, native
 from sfgs import synthetic as S
 
@@ -123,18 +124,6 @@ def test_capacity_sources():
 
 
 # ----------------------------------------------------------------------------- GPU helpers
-class deterministic:
-    def __init__(self, on=True):
-        self.on = on
-
-    def __enter__(self):
-        self.prev = torch.are_deterministic_algorithms_enabled()
-        torch.use_deterministic_algorithms(self.on)
-
-    def __exit__(self, *exc):
-        torch.use_deterministic_algorithms(self.prev)
-
-
 def _t(x, dev):
     return torch.from_numpy(np.ascontiguousarray(x)).to(dev)
 

@@ -1,5 +1,5 @@
 """Focal-length gradients (sfgs_rasterize_backward_camera_intrinsics): dL/dtan_fovx and dL/dtan_fovy, after the 35
-camera gradients.  The oracle is tests/intrinsics_chain_f64.py, the camera restatement with tan_fov as leaves.
+camera gradients.  The oracle is tests/chain_f64.py, the camera restatement with tan_fov as leaves (focal=True).
 
 CPU: the restatement against the camera restatement (bit for bit) and against finite differences (including clamped
 Gaussians), the C ABI's argument checks, and the autograd layer's native calls.
@@ -11,10 +11,10 @@ import numpy as np
 import pytest
 import torch
 
-import camera_chain_f64 as CC
+import chain_f64 as CH
 import golden_cases as G
 import helpers as Hh
-import intrinsics_chain_f64 as IC
+from helpers import release_cached_frames  # noqa: F401
 from sfgs import synthetic as S
 
 SFGS_E_BADARG, SFGS_E_UNSUPPORTED = -2, -4
@@ -31,32 +31,20 @@ def _oracle_args(name):
     o = O.forward(scene.means3D, scene.scales, scene.rotations, scene.opacities, scene.shs, kw["sh_degree"],
                   cam.viewmatrix, cam.projmatrix, cam.campos, cam.width, cam.height, cam.tanfovx, cam.tanfovy, bg,
                   kernel_size=kw["kernel_size"], scale_modifier=kw["scale_modifier"], colors_precomp=colors)
-    L = O.lib()
-    P, W, H = scene.P, cam.width, cam.height
-    f = lambda a: np.ascontiguousarray(a, np.float32)  # noqa: E731
-    s = dict(means2D=np.zeros((P, 3), np.float32), conic=np.zeros((P, 4), np.float32), opacity=np.zeros(P, np.float32),
-             colors=np.zeros((P, 3), np.float32), depths=np.zeros(P, np.float32), norm3D=np.zeros((P, 3), np.float32))
-    cot = [f(c) for c in kw["cot"]]
-    cols = f(colors) if colors is not None else o["rgb"]
-    p = O._p
-    L.oracle_render_backward(C.c_int(W), C.c_int(H), C.c_int(0), p(o["ranges"]), p(np.ascontiguousarray(o["point_list"])),
-                             p(f(bg)), p(o["means2D"]), p(o["conic_opacity"]), p(cols), p(o["depths"]), p(o["norm3D"]),
-                             None, p(o["alpha"]), p(o["n_contrib"]), p(cot[0]), p(cot[1]), p(cot[2]), p(cot[3]), None,
-                             p(s["means2D"]), p(s["conic"]), p(s["opacity"]), p(s["colors"]), p(s["depths"]),
-                             p(s["norm3D"]), None)
-    acc = CC.acc_from_screen_grads(s["means2D"], s["colors"], s["depths"], s["norm3D"], s["conic"], s["opacity"])
+    s = O.blend_backward(o, *kw["cot"])
+    acc = CH.acc_from_screen_grads(s["means2D"], s["colors"], s["depths"], s["norm3D"], s["conic"], s["opacity"])
     return dict(acc=acc, radii=o["radii"], means3D=scene.means3D, cov3D=o["cov3D"],
                 combined_opacity=o["conic_opacity"][:, 3], clamped=o["clamped"] != 0,
                 shs=None if colors is not None else scene.shs, D=kw["sh_degree"], viewmatrix=cam.viewmatrix,
-                projmatrix=cam.projmatrix, campos=cam.campos, W=W, H=H, tan_fovx=cam.tanfovx, tan_fovy=cam.tanfovy,
-                kernel_size=kw["kernel_size"])
+                projmatrix=cam.projmatrix, campos=cam.campos, W=cam.width, H=cam.height, tan_fovx=cam.tanfovx,
+                tan_fovy=cam.tanfovy, kernel_size=kw["kernel_size"])
 
 
 @pytest.mark.parametrize("name", G.CASES)
 def test_restatement_extends_the_camera_restatement_bit_for_bit(name):
     a = _oracle_args(name)
-    r = IC.intrinsics_chain(**a)
-    c = CC.camera_chain(**a)
+    r = CH.chain(**a, focal=True)
+    c = CH.chain(**a)
     for k in ("means3D", "view", "proj", "campos"):
         assert torch.equal(r[k], c[k]), (name, k)
     assert torch.equal(r["abs"][:35], c["abs"]), name
@@ -68,7 +56,7 @@ def _away_from_kinks(a, scale):
     from the clamp bound 1.3 tan_fov."""
     for k in range(200):
         s = scale * (1.0 + 1.7e-3 * k)
-        r = IC.intrinsics_chain(**dict(a, tan_fovx=a["tan_fovx"] * s, tan_fovy=a["tan_fovy"] * s), exact=True)
+        r = CH.chain(**dict(a, tan_fovx=a["tan_fovx"] * s, tan_fovy=a["tan_fovy"] * s), focal=True, exact=True)
         if (torch.cat([r["txtz_lim"], r["tytz_lim"]]) - 1).abs().min() > 1e-3:
             return s, r
     raise AssertionError("no tan_fov scale away from the clamp kinks")
@@ -92,7 +80,7 @@ def test_restatement_matches_finite_differences(name, scale):
         for sgn in (1.0, -1.0):
             kw = dict(a, tan_fovx=tx0, tan_fovy=ty0)
             kw[which] = t0 + sgn * h
-            Lg.append(IC.intrinsics_chain(**kw, exact=True, coef=r["coef"])["Lg"])
+            Lg.append(CH.chain(**kw, focal=True, exact=True, coef=r["coef"])["Lg"])
         fd = float((Lg[0] - Lg[1]).sum()) / (2 * h)
         ad = float(r[key])
         scale_abs = float(r["abs"][35 if key == "tanx" else 36])
@@ -101,8 +89,8 @@ def test_restatement_matches_finite_differences(name, scale):
         if scale < 1.0:
             # the clamp term matters: without it the gradient misses the finite differences by far more than the
             # tolerance above
-            held = IC.intrinsics_chain(**dict(a, tan_fovx=tx0, tan_fovy=ty0), exact=True, coef=r["coef"],
-                                       hold_bound=True)
+            held = CH.chain(**dict(a, tan_fovx=tx0, tan_fovy=ty0), focal=True, exact=True, coef=r["coef"],
+                            hold_bound=True)
             clamp_term.append(abs(fd - float(held[key])) / scale_abs)
     if scale < 1.0:
         assert max(clamp_term) > 1e-5, (name, clamp_term)
@@ -244,86 +232,11 @@ def test_autograd_layer_calls_the_intrinsics_entry_for_focal_leaves(monkeypatch,
 
 
 # ----------------------------------------------------------------------------- GPU helpers
-_FRAMES = {}
-_ACC = {}
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _release_cached_frames():
-    """The 1M-Gaussian frames and results cached between this module's tests are freed when it is done."""
-    yield
-    _FRAMES.clear()
-    _ACC.clear()
-    if torch.cuda.is_available():
-        torch.cuda.empty_cache()
-
-
-def _frame(name, dev):
-    """The benched frames (1M Gaussians, 1920x1080: JAX_004 and the whole-scene orbit) at SH degree 3, the JAX_004
-    frame at SH degree 1 (M = 4) with SH or with precomputed colours, and 'clamp': the JAX_004 frame of a small city
-    whose Gaussians extend beyond the frustum clamp bound."""
-    if name not in _FRAMES:
-        D = 1 if name.startswith("m4") or name == "precomp" else 3
-        if name == "clamp":
-            scene = S.city_scene(200_000, seed=4, sh_degree=3, extent=128.0)
-            scene.scales *= 8.0         # ~1700 rasterized Gaussians beyond the clamp bound in y
-            cam = S.jax004_camera(640, 360)
-        else:
-            scene = S.city_scene(1_000_000, seed=0, sh_degree=D)
-            cam = S.orbit_camera(width=1920, height=1080) if name == "orbit" else S.jax004_camera(1920, 1080)
-        colors = None
-        if name == "precomp":
-            colors = np.random.default_rng(5).uniform(0, 1, size=(scene.P, 3)).astype(np.float32)
-        _FRAMES.clear()             # one 1M frame on the device at a time
-        _FRAMES[name] = (scene, cam, D, colors)
-    scene, cam, D, colors = _FRAMES[name]
-    d = Hh.to_torch(scene, cam, dev)
-    col = torch.from_numpy(colors).to(dev) if colors is not None else None
-    return scene, cam, D, d, col
-
-
-def _fwd(d, cam, D, bg, colors=None, off=None):
-    from sfgs import rasterizer as R
-    e = torch.empty(0, device=d["means3D"].device)
-    out = R.rasterize_gaussians(bg, d["means3D"], colors if colors is not None else e, d["opacities"], d["scales"],
-                                d["rotations"], 1.0, e, e, e, 0, d["viewmatrix"], d["projmatrix"], cam.tanfovx,
-                                cam.tanfovy, 0.1, cam.height, cam.width, e if colors is not None else d["shs"], D,
-                                d["campos"], False, False, subpixel_offset=off)
-    return dict(zip(("num_rendered", "color", "depth", "norm", "alpha", "radii", "extra", "geom", "binning", "img"),
-                    out))
-
-
-def _bwd(d, cam, D, bg, f, cot, colors=None, off=None, det=False, camera=False, intrinsics=False, **kw):
-    """One backward; with camera=True also 'view', 'proj', 'campos', with intrinsics=True also 'tanx', 'tany'."""
-    from sfgs import rasterizer as R
-    e = torch.empty(0, device=d["means3D"].device)
-    prev = torch.are_deterministic_algorithms_enabled()
-    torch.use_deterministic_algorithms(det)
-    try:
-        out = R.rasterize_gaussians_backward(
-            bg, d["means3D"], f["radii"], colors if colors is not None else e, d["scales"], d["rotations"], e, 1.0, e,
-            e, d["viewmatrix"], d["projmatrix"], cam.tanfovx, cam.tanfovy, 0.1, cot[0], cot[1], cot[2], cot[3], e,
-            e if colors is not None else d["shs"], D, d["campos"], f["geom"], f["num_rendered"], f["binning"],
-            f["img"], f["alpha"], False, subpixel_offset=off, camera_grad=camera, intrinsics_grad=intrinsics, **kw)
-    finally:
-        torch.use_deterministic_algorithms(prev)
-    if kw.get("phase") == 1:
-        return out
-    return dict(zip(GRAD_KEYS + CAM_KEYS + ("tanx", "tany"), out))
-
-
-def _bits(t):
-    return t.contiguous().view(torch.int32)
-
-
 def _setup(name, dev, jitter, seed=6):
-    scene, cam, D, d, colors = _frame(name, dev)
+    scene, cam, D, d, colors = Hh.frame(name, dev)
     bg = torch.tensor([0.1, 0.2, 0.3], device=dev)
-    off = None
-    if jitter:
-        g = torch.Generator(device=dev).manual_seed(23)
-        off = torch.rand((cam.height, cam.width, 2), generator=g, device=dev) - 0.5
-    f = _fwd(d, cam, D, bg, colors, off)
+    off = Hh.uniform_offsets(cam.height, cam.width, dev, 23) if jitter else None
+    f = Hh.run_ours_forward(d, cam, D, bg, colors=colors, subpixel_offset=off)
     cot = [torch.from_numpy(c).to(dev) for c in S.cotangents(cam.width, cam.height, seed=seed)]
     return scene, cam, D, d, colors, bg, off, f, cot
 
@@ -337,36 +250,33 @@ def test_other_outputs_and_camera_terms_unchanged(cuda_device, name):
     dev = cuda_device
     for jitter in (False, True):
         scene, cam, D, d, colors, bg, off, f, cot = _setup(name, dev, jitter)
-        a = _bwd(d, cam, D, bg, f, cot, colors, off, det=True, camera=True)
-        b = _bwd(d, cam, D, bg, f, cot, colors, off, det=True, camera=True, intrinsics=True)
+        a = Hh.run_ours_backward(d, cam, D, bg, f, cot, colors=colors, subpixel_offset=off, det=True, camera_grad=True)
+        b = Hh.run_ours_backward(d, cam, D, bg, f, cot, colors=colors, subpixel_offset=off, det=True, camera_grad=True,
+                                 intrinsics_grad=True)
         for k in GRAD_KEYS + CAM_KEYS:
             assert a[k].shape == b[k].shape, (name, jitter, k)
-            assert torch.equal(_bits(a[k]), _bits(b[k])), (name, jitter, k)
+            assert torch.equal(Hh.bits(a[k]), Hh.bits(b[k])), (name, jitter, k)
         assert b["tanx"].shape == () and b["tany"].shape == ()
         assert bool(torch.isfinite(b["tanx"])) and bool(torch.isfinite(b["tany"]))
         # the default call forms the same focal terms from the same kernel
-        gc = _bwd(d, cam, D, bg, f, cot, colors, off, camera=True, intrinsics=True)
+        gc = Hh.run_ours_backward(d, cam, D, bg, f, cot, colors=colors, subpixel_offset=off, camera_grad=True,
+                                  intrinsics_grad=True)
         assert bool(torch.isfinite(gc["tanx"])) and bool(torch.isfinite(gc["tany"]))
 
 
 def _accuracy_case(case, dev):
     """GPU focal gradients of a deterministic call and the restatement (float64 and float32) evaluated on the phase-1
     sums of a deterministic run: the same `acc` bits the call uses."""
-    if case in _ACC:
-        return _ACC[case]
-    name = {"d3": "jax004", "d1": "m4", "precomp": "precomp", "clamp": "clamp"}[case.split("_")[0]]
-    scene, cam, D, d, colors, bg, off, f, cot = _setup(name, dev, case.endswith("jitter"))
-    g = _bwd(d, cam, D, bg, f, cot, colors, off, det=True, camera=True, intrinsics=True)
-    acc = _bwd(d, cam, D, bg, f, cot, colors, off, det=True, phase=1)
-    I = Hh.our_internals(f, scene.P, cam.height, cam.width)
-    clamped = torch.stack([(I["clamped"].int() >> ch) & 1 for ch in range(3)], 1) != 0
-    args = (acc, f["radii"], d["means3D"], I["cov3D"], I["rec"][:, 5], clamped, None if colors is not None else d["shs"],
-            D, d["viewmatrix"], d["projmatrix"], d["campos"], cam.width, cam.height, cam.tanfovx, cam.tanfovy, 0.1)
-    r64 = IC.intrinsics_chain(*args, dtype=torch.float64)
-    r32 = IC.intrinsics_chain(*args, dtype=torch.float32)
-    _ACC.clear()
-    _ACC[case] = (g, r64, r32)
-    return _ACC[case]
+    def make():
+        name = {"d3": "jax004", "d1": "m4", "precomp": "precomp", "clamp": "clamp"}[case.split("_")[0]]
+        scene, cam, D, d, colors, bg, off, f, cot = _setup(name, dev, case.endswith("jitter"))
+        g = Hh.run_ours_backward(d, cam, D, bg, f, cot, colors=colors, subpixel_offset=off, det=True, camera_grad=True,
+                                 intrinsics_grad=True)
+        a = Hh.restatement_inputs(f, d, cam, D, bg, cot, colors, off)
+        r64 = CH.chain(**a, focal=True, dtype=torch.float64)
+        r32 = CH.chain(**a, focal=True, dtype=torch.float32)
+        return g, r64, r32
+    return Hh.cached("case", case, make)
 
 
 @pytest.mark.gpu
@@ -392,10 +302,11 @@ def test_deterministic_focal_gradients_are_reproducible(cuda_device):
     dev = cuda_device
     for jitter in (False, True):
         scene, cam, D, d, colors, bg, off, f, cot = _setup("jax004", dev, jitter)
-        runs = [_bwd(d, cam, D, bg, f, cot, colors, off, det=True, camera=True, intrinsics=True) for _ in range(3)]
+        runs = [Hh.run_ours_backward(d, cam, D, bg, f, cot, colors=colors, subpixel_offset=off, det=True,
+                                     camera_grad=True, intrinsics_grad=True) for _ in range(3)]
         for k in CAM_KEYS + ("tanx", "tany"):
             for r in runs[1:]:
-                assert torch.equal(_bits(runs[0][k]), _bits(r[k])), (jitter, k)
+                assert torch.equal(Hh.bits(runs[0][k]), Hh.bits(r[k])), (jitter, k)
 
 
 def _projection(tanx, tany, cx, cy, W, H, znear=0.01, zfar=100.0):

@@ -1,7 +1,8 @@
 """Orthographic views (sfgs_rasterize_forward_ortho / sfgs_rasterize_backward_ortho, sfgs.ortho).
 
 The reference rasterizer has no orthographic camera; the oracle is tests/ortho_chain_f64.py, a float64 restatement of
-the orthographic preprocess and per-Gaussian adjoint, blended by the unchanged CPU oracle's blend.
+the orthographic preprocess blended by the unchanged CPU oracle's blend, and tests/chain_f64.py's per-Gaussian adjoint
+(ortho=True).
 
 CPU: the restatement against float64 central differences, projection_matrix, nadir_camera, the C ABI's and the Python
 layer's rejections and their order, and the native calls OrthoRasterizer makes.
@@ -10,11 +11,13 @@ restatement's autograd and an end-to-end finite-difference check, the determinis
 and a height-map fit."""
 import ctypes as C
 import math
+import types
 
 import numpy as np
 import pytest
 import torch
 
+import chain_f64 as CH
 import helpers as Hh
 import ortho_chain_f64 as OC
 from sfgs import synthetic as S
@@ -48,32 +51,31 @@ def scene_tensors(P, seed, D, M, dev, spread=2.0, scale=0.12, colors=False):
     return d
 
 
-def forward(d, view, proj, W, H, s_x, s_y, bg, ks=0.1, off=None):
-    from sfgs import rasterizer as R
+def _frame(d, view, proj, W, H, s_x, s_y):
+    """The harness's Gaussians with the matrices, and its camera (the half-extents in place of tan_fov)."""
     dev = d["means3D"].device
-    e = torch.empty(0, device=dev)
-    sh = d["shs"] if d.get("shs") is not None else e
-    col = d.get("colors") if d.get("colors") is not None else e
-    out = R.rasterize_gaussians(bg, d["means3D"], col, d["opacities"], d["scales"], d["rotations"], 1.0, e, e, e, 0,
-                                view.to(dev), proj.to(dev), s_x, s_y, ks, H, W, sh, d["D"],
-                                torch.zeros(3, device=dev), False, False, subpixel_offset=off, ortho=True)
-    keys = ("num_rendered", "color", "depth", "norm", "alpha", "radii", "extra", "geom", "binning", "img")
-    return dict(zip(keys, out))
+    cam = types.SimpleNamespace(width=W, height=H, tanfovx=s_x, tanfovy=s_y)
+    return dict(d, viewmatrix=view.to(dev), projmatrix=proj.to(dev), campos=torch.zeros(3, device=dev)), cam
+
+
+def forward(d, view, proj, W, H, s_x, s_y, bg, ks=0.1, off=None):
+    dd, cam = _frame(d, view, proj, W, H, s_x, s_y)
+    return Hh.run_ours_forward(dd, cam, d["D"], bg, kernel_size=ks, colors=d.get("colors"), subpixel_offset=off,
+                               ortho=True)
 
 
 def backward(d, view, proj, W, H, s_x, s_y, bg, fwd, cot, ks=0.1, off=None, **kw):
-    from sfgs import rasterizer as R
-    dev = d["means3D"].device
-    e = torch.empty(0, device=dev)
-    sh = d["shs"] if d.get("shs") is not None else e
-    col = d.get("colors") if d.get("colors") is not None else e
-    out = R.rasterize_gaussians_backward(bg, d["means3D"], fwd["radii"], col, d["scales"], d["rotations"], e, 1.0, e,
-                                         e, view.to(dev), proj.to(dev), s_x, s_y, ks, cot[0], cot[1], cot[2], cot[3],
-                                         e, sh, d["D"], torch.zeros(3, device=dev), fwd["geom"], fwd["num_rendered"],
-                                         fwd["binning"], fwd["img"], fwd["alpha"], False, subpixel_offset=off, **kw)
-    if kw.get("phase") == 1:
-        return out
-    return dict(zip(GRAD_KEYS + ("extra",), out))
+    dd, cam = _frame(d, view, proj, W, H, s_x, s_y)
+    return Hh.run_ours_backward(dd, cam, d["D"], bg, fwd, cot, kernel_size=ks, colors=d.get("colors"),
+                                subpixel_offset=off, **kw)
+
+
+def restatement(d, view, proj, W, H, s_x, s_y, bg, fwd, cot, off=None):
+    """chain_f64.chain(ortho=True) on this frame's phase-1 sums (the blend adjoint reads only the forward's records, so
+    the pinhole phase-1 call gives them), with scales and rotations as leaves."""
+    dd, cam = _frame(d, view, proj, W, H, s_x, s_y)
+    a = Hh.restatement_inputs(fwd, dd, cam, d["D"], bg, cot, d.get("colors"), off, det=None)
+    return CH.chain(**dict(a, cov3D=None), scales=d["scales"], rotations=d["rotations"], ortho=True)
 
 
 def restated(d, view, proj, W, H, s_x, s_y, ks=0.1):
@@ -120,8 +122,8 @@ def test_restatement_chain_matches_central_differences():
     vis = torch.ones(P, dtype=torch.bool)
     clamped = torch.zeros(P, 3, dtype=torch.bool)
     pre = OC.preprocess(m, sc, q, torch.ones(P, 1), view, proj, W, H, s_x, s_y, 0.1, D=3, shs=sh)
-    g = OC.chain(acc, vis, m, sc, q, torch.ones(P, 1), view, proj, W, H, s_x, s_y, 0.1, D=3, shs=sh, clamped=clamped,
-                 norm_rec=pre["norm3D"] + 0 * m)
+    g = CH.chain(acc, vis, m, torch.ones(P), clamped, sh, 3, view, proj, None, W, H, s_x, s_y, 0.1, scales=sc,
+                 rotations=q, norm_rec=pre["norm3D"] + 0 * m, ortho=True)
     d = OC.view_axis(view)
 
     def L(m_, sh_):
@@ -414,7 +416,7 @@ def _grad_check(ours, ref, what):
     for k in GRAD_KEYS:
         if k not in ref:
             continue
-        a, b = ours[k].detach().double().cpu().reshape(ref[k].shape), ref[k].double()
+        a, b = ours[k].detach().double().cpu().reshape(ref[k].shape), ref[k].double().cpu()
         atol = 1e-4 * float(b.abs().max()) + 1e-7
         err = float(((a - b).abs() - 1e-3 * b.abs()).max())
         assert err <= atol, (what, k, err, atol)
@@ -427,12 +429,7 @@ def _gradient_case(dev, seed, colors=False):
         d["shs"] = None
     fwd = forward(d, view, proj, W, H, s_x, s_y, bg)
     cot = [torch.from_numpy(c).to(dev) for c in S.cotangents(W, H, seed=seed + 3)]
-    # the blend adjoint reads only the forward's records, so the pinhole phase-1 call gives this frame's sums
-    acc = backward(d, view, proj, W, H, s_x, s_y, bg, fwd, cot, phase=1)
-    I = Hh.our_internals(fwd, 400, H, W)
-    cl = torch.stack([(I["clamped"].long() >> k) & 1 for k in range(3)], 1).bool()
-    ref = OC.chain(acc, fwd["radii"] > 0, d["means3D"], d["scales"], d["rotations"], d["opacities"], view, proj, W, H,
-                   s_x, s_y, 0.1, D=d["D"], shs=d.get("shs"), clamped=cl, norm_rec=I["norm3D"])
+    ref = restatement(d, view, proj, W, H, s_x, s_y, bg, fwd, cot)
     return d, view, proj, W, H, s_x, s_y, bg, fwd, cot, ref
 
 
@@ -495,22 +492,13 @@ def test_end_to_end_finite_differences(cuda_device):
 def test_deterministic_backward(cuda_device):
     d, view, proj, W, H, s_x, s_y, bg, fwd, cot, ref = _gradient_case(cuda_device, 4)
     default = backward(d, view, proj, W, H, s_x, s_y, bg, fwd, cot, ortho=True)
-    with _det():
+    with Hh.deterministic():
         g1 = backward(d, view, proj, W, H, s_x, s_y, bg, fwd, cot, ortho=True)
         g2 = backward(d, view, proj, W, H, s_x, s_y, bg, fwd, cot, ortho=True)
     for k in GRAD_KEYS:
         assert torch.equal(g1[k].view(torch.int32), g2[k].view(torch.int32)), k
     _grad_check(default, ref, "default")
     _grad_check(g1, ref, "deterministic")
-
-
-class _det:
-    def __enter__(self):
-        self.was = torch.are_deterministic_algorithms_enabled()
-        torch.use_deterministic_algorithms(True)
-
-    def __exit__(self, *a):
-        torch.use_deterministic_algorithms(self.was)
 
 
 @pytest.mark.gpu
@@ -543,11 +531,7 @@ def test_fractional_offsets_against_restatement(cuda_device):
     _image_close(fwd, ref, "offsets")
     # the backward takes the same offsets: its gradients match the restatement's chain for the offset frame's sums
     cot = [torch.from_numpy(c).to(dev) for c in S.cotangents(W, H, seed=9)]
-    acc = backward(d, view, proj, W, H, s_x, s_y, bg, fwd, cot, off=off, phase=1)
-    I = Hh.our_internals(fwd, 400, H, W)
-    cl = torch.stack([(I["clamped"].long() >> k) & 1 for k in range(3)], 1).bool()
-    ref_g = OC.chain(acc, fwd["radii"] > 0, d["means3D"], d["scales"], d["rotations"], d["opacities"], view, proj, W,
-                     H, s_x, s_y, 0.1, D=3, shs=d["shs"], clamped=cl, norm_rec=I["norm3D"])
+    ref_g = restatement(d, view, proj, W, H, s_x, s_y, bg, fwd, cot, off)
     _grad_check(backward(d, view, proj, W, H, s_x, s_y, bg, fwd, cot, off=off, ortho=True), ref_g, "offsets")
 
 

@@ -217,25 +217,6 @@ def test_reference_render_forwards_offsets_only_when_opted_in(reference_stack, m
 
 
 # ----------------------------------------------------------------------------- GPU helpers
-def _forward(d, cam, sh, bg, off=None, **kw):
-    from sfgs import rasterizer as R
-    e = torch.empty(0, device=d["means3D"].device)
-    out = R.rasterize_gaussians(bg, d["means3D"], e, d["opacities"], d["scales"], d["rotations"], 1.0, e, e, e, 0,
-                                d["viewmatrix"], d["projmatrix"], cam.tanfovx, cam.tanfovy, 0.1, cam.height, cam.width,
-                                d["shs"], sh, d["campos"], False, False, subpixel_offset=off, **kw)
-    return dict(zip(("num_rendered", "color", "depth", "norm", "alpha", "radii", "extra", "geom", "binning", "img"),
-                    out))
-
-
-def _backward(d, cam, sh, bg, f, cot, off=None, det=False, **kw):
-    prev = torch.are_deterministic_algorithms_enabled()
-    torch.use_deterministic_algorithms(det)
-    try:
-        return Hh.run_ours_backward(d, cam, sh, bg, f, cot, subpixel_offset=off, **kw)
-    finally:
-        torch.use_deterministic_algorithms(prev)
-
-
 def inst_masks(f, W, H):
     """The reach mask of every sorted instance (BinningLayout: point_list, then inst_mask)."""
     hdr = f["img"][:32].view(torch.int32).cpu().numpy().astype(np.uint32)
@@ -243,10 +224,6 @@ def inst_masks(f, W, H):
     base = (f["binning"].data_ptr() + 255) & ~255
     off = base - f["binning"].data_ptr() + ((cap * 4 + 255) & ~255)
     return f["binning"][off:off + f["num_rendered"]].clone()
-
-
-def _bits(t):
-    return t.contiguous().view(torch.int32) if t.dtype == torch.float32 else t
 
 
 def _close(a, b, k, extra=0.0):
@@ -265,11 +242,6 @@ def _scene(name, dev):
     return scene, cam, Hh.to_torch(scene, cam, dev)
 
 
-def _uniform(H, W, dev, seed):
-    g = torch.Generator(device=dev).manual_seed(seed)
-    return torch.rand((H, W, 2), generator=g, device=dev) - 0.5
-
-
 # ----------------------------------------------------------------------------- GPU tests
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", ["blob", "city"])
@@ -279,9 +251,9 @@ def test_zero_offsets_equal_the_default_call(cuda_device, name):
     bg = torch.tensor([0.3, 0.1, 0.2], device=dev)
     H, W = cam.height, cam.width
     zero = torch.zeros((H, W, 2), device=dev)
-    f0, f1 = _forward(d, cam, 3, bg), _forward(d, cam, 3, bg, zero)
+    f0, f1 = Hh.run_ours_forward(d, cam, 3, bg), Hh.run_ours_forward(d, cam, 3, bg, subpixel_offset=zero)
     for k in ("color", "depth", "norm", "alpha", "radii"):
-        assert torch.equal(_bits(f0[k]), _bits(f1[k])), k
+        assert torch.equal(Hh.bits(f0[k]), Hh.bits(f1[k])), k
     i0, i1 = Hh.our_internals(f0, scene.P, H, W), Hh.our_internals(f1, scene.P, H, W)
     for k in ("n_contrib", "point_list", "ranges", "keys"):
         assert torch.equal(i0[k], i1[k]), k
@@ -289,10 +261,11 @@ def test_zero_offsets_equal_the_default_call(cuda_device, name):
     cot = [torch.from_numpy(c).to(dev) for c in S.cotangents(W, H, seed=6)]
     # the ill-conditioned covariance / rotation gradients of the 1080p frame differ between two calls of the default
     # backward itself (unordered reductions) by about the bound: that spread is allowed on top of it
-    ga, gb = _backward(d, cam, 3, bg, f0, cot), _backward(d, cam, 3, bg, f0, cot)
+    ga, gb = Hh.run_ours_backward(d, cam, 3, bg, f0, cot), Hh.run_ours_backward(d, cam, 3, bg, f0, cot)
     spread = {k: (ga[k].double() - gb[k].double()).abs().max().item() for k in GRAD_KEYS}
     for det in (False, True):
-        g0, g1 = _backward(d, cam, 3, bg, f0, cot, det=det), _backward(d, cam, 3, bg, f1, cot, zero, det=det)
+        g0 = Hh.run_ours_backward(d, cam, 3, bg, f0, cot, det=det)
+        g1 = Hh.run_ours_backward(d, cam, 3, bg, f1, cot, subpixel_offset=zero, det=det)
         for k in GRAD_KEYS:
             _close(g1[k], g0[k], (k, det), extra=2.0 * spread[k])
 
@@ -303,7 +276,7 @@ def _shift_case(dev, name, ox, oy, det_grads=True):
     H, W = cam.height, cam.width
     off = torch.empty((H, W, 2), device=dev)
     off[..., 0], off[..., 1] = float(ox), float(oy)
-    f0, f1 = _forward(d, cam, 3, bg), _forward(d, cam, 3, bg, off)
+    f0, f1 = Hh.run_ours_forward(d, cam, 3, bg), Hh.run_ours_forward(d, cam, 3, bg, subpixel_offset=off)
     assert torch.equal(f0["radii"], f1["radii"])
     y, x = torch.meshgrid(torch.arange(H, device=dev), torch.arange(W, device=dev), indexing="ij")
     sx, sy = x + ox, y + oy
@@ -313,7 +286,7 @@ def _shift_case(dev, name, ox, oy, det_grads=True):
     for k in ("color", "depth", "norm", "alpha"):
         a = f1[k].reshape(f1[k].shape[0], -1)[:, ok.flatten()]
         b = f0[k].reshape(f0[k].shape[0], -1)[:, src]
-        assert torch.equal(_bits(a), _bits(b)), (k, ox, oy)
+        assert torch.equal(Hh.bits(a), Hh.bits(b)), (k, ox, oy)
     n0 = Hh.our_internals(f0, scene.P, H, W)["n_contrib"]
     n1 = Hh.our_internals(f1, scene.P, H, W)["n_contrib"]
     assert torch.equal(n1[ok.flatten()], n0[src]), (ox, oy)
@@ -325,8 +298,8 @@ def _shift_case(dev, name, ox, oy, det_grads=True):
     cot0 = [torch.zeros_like(c) for c in cot]
     for c0, c1 in zip(cot0, cot1):
         c0.view(c0.shape[0], -1)[:, src] = c1.view(c1.shape[0], -1)[:, ok.flatten()]
-    g1 = _backward(d, cam, 3, bg, f1, cot1, off, det=True)
-    g0 = _backward(d, cam, 3, bg, f0, cot0, det=True)
+    g1 = Hh.run_ours_backward(d, cam, 3, bg, f1, cot1, subpixel_offset=off, det=True)
+    g0 = Hh.run_ours_backward(d, cam, 3, bg, f0, cot0, det=True)
     for k in GRAD_KEYS:
         _close(g1[k], g0[k], (k, ox, oy))
 
@@ -368,8 +341,8 @@ def test_fractional_offsets_against_cpu_oracle(cuda_device, case):
     bg = np.array([0.3, 0.1, 0.2], np.float32)
     bg_t = torch.from_numpy(bg).to(dev)
     d = Hh.to_torch(scene, cam, dev)
-    off = _uniform(cam.height, cam.width, dev, 17)
-    f = _forward(d, cam, deg, bg_t, off)
+    off = Hh.uniform_offsets(cam.height, cam.width, dev, 17)
+    f = Hh.run_ours_forward(d, cam, deg, bg_t, subpixel_offset=off)
     o = SO.cpu_forward(scene.means3D, scene.scales, scene.rotations, scene.opacities, scene.shs, deg, cam.viewmatrix,
                        cam.projmatrix, cam.campos, cam.width, cam.height, cam.tanfovx, cam.tanfovy, bg,
                        subpixel_offset=off.cpu().numpy())
@@ -380,7 +353,7 @@ def test_fractional_offsets_against_cpu_oracle(cuda_device, case):
     for k in ("color", "depth", "norm", "alpha"):
         assert np.abs(f[k].cpu().numpy() - o[k]).max() <= 5e-5, k
     cot = S.cotangents(cam.width, cam.height, seed=6)
-    gb = _backward(d, cam, deg, bg_t, f, [torch.from_numpy(c).to(dev) for c in cot], off)
+    gb = Hh.run_ours_backward(d, cam, deg, bg_t, f, [torch.from_numpy(c).to(dev) for c in cot], subpixel_offset=off)
     og = SO.cpu_backward(o, *cot)
     for k in ("means2D", "opacity", "means3D", "sh", "scales", "rot"):
         a, b = gb[k].cpu().numpy().astype(np.float64), og[k].astype(np.float64)
@@ -398,9 +371,9 @@ def test_fractional_offsets_adjudicated_in_float64(cuda_device):
     H, W = cam.height, cam.width
     cot = [torch.from_numpy(c).to(dev) for c in S.cotangents(W, H, seed=4)]
     rep = {}
-    for tag, off in (("plain", None), ("jitter", _uniform(H, W, dev, 23))):
-        f = _forward(d, cam, 3, bg, off)
-        runs = [_backward(d, cam, 3, bg, f, cot, off) for _ in range(3)]
+    for tag, off in (("plain", None), ("jitter", Hh.uniform_offsets(H, W, dev, 23))):
+        f = Hh.run_ours_forward(d, cam, 3, bg, subpixel_offset=off)
+        runs = [Hh.run_ours_backward(d, cam, 3, bg, f, cot, subpixel_offset=off) for _ in range(3)]
         I = Hh.our_internals(f, scene.P, H, W)
         args = (I, d["means3D"], f["radii"], d["shs"], d["scales"], d["rotations"], 1.0, d["viewmatrix"],
                 d["projmatrix"], d["campos"], cam.tanfovx, cam.tanfovy, 0.1, 3, bg, f["alpha"], cot)
@@ -418,13 +391,13 @@ def test_deterministic_backward_with_offsets(cuda_device):
     dev = cuda_device
     scene, cam, d = _scene("banded", dev)
     bg = torch.tensor([0.3, 0.1, 0.2], device=dev)
-    off = _uniform(cam.height, cam.width, dev, 5)
-    f = _forward(d, cam, 3, bg, off)
+    off = Hh.uniform_offsets(cam.height, cam.width, dev, 5)
+    f = Hh.run_ours_forward(d, cam, 3, bg, subpixel_offset=off)
     cot = [torch.from_numpy(c).to(dev) for c in S.cotangents(cam.width, cam.height, seed=3)]
-    a, b = (_backward(d, cam, 3, bg, f, cot, off, det=True) for _ in range(2))
-    g = _backward(d, cam, 3, bg, f, cot, off)
+    a, b = (Hh.run_ours_backward(d, cam, 3, bg, f, cot, subpixel_offset=off, det=True) for _ in range(2))
+    g = Hh.run_ours_backward(d, cam, 3, bg, f, cot, subpixel_offset=off)
     for k in GRAD_KEYS:
-        assert torch.equal(_bits(a[k]), _bits(b[k])), k
+        assert torch.equal(Hh.bits(a[k]), Hh.bits(b[k])), k
         _close(a[k], g[k], k)
 
 
@@ -435,18 +408,18 @@ def test_two_phase_backward_with_offsets(cuda_device, det):
     scene, cam = S.blob_scene(5000, seed=91), S.simple_camera(256, 144)
     d = Hh.to_torch(scene, cam, dev)
     bg = torch.tensor([0.3, 0.2, 0.1], device=dev)
-    off = _uniform(cam.height, cam.width, dev, 9)
+    off = Hh.uniform_offsets(cam.height, cam.width, dev, 9)
     cot = [torch.from_numpy(c).to(dev) for c in S.cotangents(cam.width, cam.height, seed=4)]
-    f = _forward(d, cam, 3, bg, off)
-    one = _backward(d, cam, 3, bg, f, cot, off, det=det)
-    acc = _backward(d, cam, 3, bg, f, cot, off, det=det, phase=1)
+    f = Hh.run_ours_forward(d, cam, 3, bg, subpixel_offset=off)
+    one = Hh.run_ours_backward(d, cam, 3, bg, f, cot, subpixel_offset=off, det=det)
+    acc = Hh.run_ours_backward(d, cam, 3, bg, f, cot, subpixel_offset=off, det=det, phase=1)
     cut = 2173
-    parts = [_backward(d, cam, 3, bg, f, cot, off, det=det, phase=2, acc=acc[a:b].clone(), gauss_range=(a, b))
-             for a, b in ((0, cut), (cut, scene.P))]
+    parts = [Hh.run_ours_backward(d, cam, 3, bg, f, cot, subpixel_offset=off, det=det, phase=2, acc=acc[a:b].clone(),
+                                  gauss_range=(a, b)) for a, b in ((0, cut), (cut, scene.P))]
     for k in GRAD_KEYS:
         got = torch.cat([parts[0][k][:cut], parts[1][k][cut:]], 0)
         if det:
-            assert torch.equal(_bits(got), _bits(one[k])), k
+            assert torch.equal(Hh.bits(got), Hh.bits(one[k])), k
         else:
             _close(got, one[k], k)
 
@@ -457,14 +430,14 @@ def test_non_finite_offset_is_rejected(cuda_device):
     dev = cuda_device
     scene, cam, d = _scene("blob", dev)
     bg = torch.zeros(3, device=dev)
-    f0 = _forward(d, cam, 3, bg)
+    f0 = Hh.run_ours_forward(d, cam, 3, bg)
     for bad in (float("nan"), float("inf")):
         off = torch.zeros((cam.height, cam.width, 2), device=dev)
         off[17, 33, 1] = bad
         with pytest.raises(SfgsError, match="NaN or Inf"):
-            _forward(d, cam, 3, bg, off)
-    f1 = _forward(d, cam, 3, bg, torch.zeros((cam.height, cam.width, 2), device=dev))
-    assert torch.equal(_bits(f0["color"]), _bits(f1["color"]))
+            Hh.run_ours_forward(d, cam, 3, bg, subpixel_offset=off)
+    f1 = Hh.run_ours_forward(d, cam, 3, bg, subpixel_offset=torch.zeros((cam.height, cam.width, 2), device=dev))
+    assert torch.equal(Hh.bits(f0["color"]), Hh.bits(f1["color"]))
 
 
 @pytest.mark.gpu
@@ -475,7 +448,7 @@ def test_autograd_layer(cuda_device, monkeypatch):
     scene, cam, d = _scene("blob", dev)
     H, W = cam.height, cam.width
     bg = torch.tensor([0.3, 0.1, 0.2], device=dev)
-    off = _uniform(H, W, dev, 31)
+    off = Hh.uniform_offsets(H, W, dev, 31)
     cot = [torch.from_numpy(c).to(dev) for c in S.cotangents(W, H, seed=2)]
 
     def run(o):
@@ -499,20 +472,19 @@ def test_autograd_layer(cuda_device, monkeypatch):
                                 d["viewmatrix"], d["projmatrix"], cam.tanfovx, cam.tanfovy, 0.1, H, W, d["shs"], 3,
                                 d["campos"], False, False, fuse_normalize=True, subpixel_offset=off)
     for a, b in zip(out_j[:4], nat[1:5]):
-        assert torch.equal(_bits(a), _bits(b))
+        assert torch.equal(Hh.bits(a), Hh.bits(b))
     out_p, g_p = run(torch.zeros(1, device=dev))      # a placeholder: the default result
     monkeypatch.setattr(diff_gauss, "SUBPIXEL_OFFSET", False)
     out_d, g_d = run(off)                             # switch off: offsets ignored
     out_0, g_0 = run(torch.zeros((H, W, 2), device=dev))
     for a, b, c in zip(out_p[:4], out_d[:4], out_0[:4]):
-        assert torch.equal(_bits(a), _bits(c)) and torch.equal(_bits(b), _bits(c))
-    assert not torch.equal(_bits(out_j[0]), _bits(out_d[0]))
+        assert torch.equal(Hh.bits(a), Hh.bits(c)) and torch.equal(Hh.bits(b), Hh.bits(c))
+    assert not torch.equal(Hh.bits(out_j[0]), Hh.bits(out_d[0]))
     for k in g_0:
         _close(g_p[k], g_0[k], k)
         _close(g_d[k], g_0[k], k)
     # the jittered gradients equal the native _subpixel backward's
-    f = dict(zip(("num_rendered", "color", "depth", "norm", "alpha", "radii", "extra", "geom", "binning", "img"),
-                 nat[:10]))
+    f = dict(zip(Hh.FWD_KEYS, nat[:10]))
     gn = Hh.run_ours_backward(d, cam, 3, bg, f, cot, subpixel_offset=off, norm_raw=nat[10])
     for k, kn in (("means3D", "means3D"), ("shs", "sh"), ("opacities", "opacity"), ("scales", "scales"),
                   ("rotations", "rot"), ("means2D", "means2D")):

@@ -17,8 +17,9 @@ import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
+import chain_f64 as CH
 import helpers as Hh
-import intrinsics_chain_f64 as IC
+from helpers import release_cached_frames  # noqa: F401
 from sfgs import multigpu as MG
 from sfgs import synthetic as S
 
@@ -117,7 +118,7 @@ def _free_port():
     return p
 
 
-def _worker(rank, world, port, out):
+def _worker(rank, world, port, out, received):
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
     dist.init_process_group("gloo", rank=rank, world_size=world)
     try:
@@ -145,18 +146,23 @@ def _worker(rank, world, port, out):
         res["rs_ok"] = mine.shape == (4, 16) and torch.equal(mine, full[rank * 4:(rank + 1) * 4])
         res["rs"] = mine
         out.put((rank, res))
+        # the result tensors travel as file descriptors this process serves: it must outlive their unpickling
+        received.wait(timeout=120)
     finally:
         dist.destroy_process_group()
 
 
 def test_camera_sum_and_ordered_reduce_scatter_world2_gloo():
     ctx = mp.get_context("spawn")
-    q = ctx.Queue()
+    q, received = ctx.Queue(), ctx.Event()
     port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, 2, port, q)) for r in range(2)]
+    procs = [ctx.Process(target=_worker, args=(r, 2, port, q, received)) for r in range(2)]
     for p in procs:
         p.start()
-    res = dict(q.get(timeout=120) for _ in procs)
+    try:
+        res = dict(q.get(timeout=120) for _ in procs)
+    finally:
+        received.set()
     for p in procs:
         p.join(timeout=60)
     assert sorted(res) == [0, 1]
@@ -170,37 +176,6 @@ def test_camera_sum_and_ordered_reduce_scatter_world2_gloo():
 def _city(dev, D=3, P=120_000, extent=120.0, seed=9):
     scene, cam = S.city_scene(P, seed=seed, sh_degree=D, extent=extent), S.jax004_camera(640, 360)
     return scene, cam, Hh.to_torch(scene, cam, dev)
-
-
-def _offsets(cam, dev, seed=23):
-    g = torch.Generator(device=dev).manual_seed(seed)
-    return torch.rand((cam.height, cam.width, 2), generator=g, device=dev) - 0.5
-
-
-def _fwd(d, cam, D, bg, off=None, band=None, colors=None, **kw):
-    from sfgs import rasterizer as R
-    e = torch.empty(0, device=d["means3D"].device)
-    out = R.rasterize_gaussians(bg, d["means3D"], colors if colors is not None else e, d["opacities"], d["scales"],
-                                d["rotations"], 1.0, e, e, e, 0, d["viewmatrix"], d["projmatrix"], cam.tanfovx,
-                                cam.tanfovy, 0.1, cam.height, cam.width, e if colors is not None else d["shs"], D,
-                                d["campos"], False, False, tile_rows=band, subpixel_offset=off, **kw)
-    return dict(zip(("num_rendered", "color", "depth", "norm", "alpha", "radii", "extra", "geom", "binning", "img"),
-                    out))
-
-
-def _bwd(d, cam, D, bg, f, cot, off=None, band=None, colors=None, det=False, **kw):
-    from sfgs import rasterizer as R
-    e = torch.empty(0, device=d["means3D"].device)
-    prev = torch.are_deterministic_algorithms_enabled()
-    torch.use_deterministic_algorithms(det)
-    try:
-        return R.rasterize_gaussians_backward(
-            bg, d["means3D"], f["radii"], colors if colors is not None else e, d["scales"], d["rotations"], e, 1.0, e,
-            e, d["viewmatrix"], d["projmatrix"], cam.tanfovx, cam.tanfovy, 0.1, cot[0], cot[1], cot[2], cot[3], e,
-            e if colors is not None else d["shs"], D, d["campos"], f["geom"], f["num_rendered"], f["binning"],
-            f["img"], f["alpha"], False, tile_rows=band, subpixel_offset=off, **kw)
-    finally:
-        torch.use_deterministic_algorithms(prev)
 
 
 def _planes(f):
@@ -221,11 +196,11 @@ def test_bands_with_offsets_reassemble_the_frame(cuda_device):
     scene, cam, d = _city(dev)
     H, W = cam.height, cam.width
     bg = torch.tensor([0.1, 0.0, 0.2], device=dev)
-    off = _offsets(cam, dev)
-    full = _fwd(d, cam, 3, bg, off)
+    off = Hh.uniform_offsets(cam.height, cam.width, dev, 23)
+    full = Hh.run_ours_forward(d, cam, 3, bg, subpixel_offset=off)
     full_nc = Hh.our_internals(full, scene.P, H, W)["n_contrib"].view(H, W)
     want = _planes(full)
-    assert not torch.equal(want, _planes(_fwd(d, cam, 3, bg)))          # the offsets move the samples
+    assert not torch.equal(want, _planes(Hh.run_ours_forward(d, cam, 3, bg)))          # the offsets move the samples
     cuts = _cuts(full, scene, cam, 3)
     one = torch.full((8 * H * W,), float("nan"), device=dev)
     two = torch.full((2, 8 * H * W), float("nan"), device=dev)
@@ -233,12 +208,14 @@ def test_bands_with_offsets_reassemble_the_frame(cuda_device):
     for g in range(3):
         band = (cuts[g], cuts[g + 1])
         y0, y1 = MG.band_pixel_rows(cuts, g, H)
-        f = _fwd(d, cam, 3, bg, off, band)
+        f = Hh.run_ours_forward(d, cam, 3, bg, subpixel_offset=off, tile_rows=band)
         total_R += f["num_rendered"]
         assert torch.equal(_planes(f)[:, y0:y1], want[:, y0:y1]), g
         assert torch.equal(f["radii"], full["radii"])
-        for fp in (_fwd(d, cam, 3, bg, off, band, out_planes=one, out_peers=[one.data_ptr()]),
-                   _fwd(d, cam, 3, bg, off, band, out_planes=two[0], out_peers=[two[0].data_ptr(), two[1].data_ptr()]),
+        for fp in (Hh.run_ours_forward(d, cam, 3, bg, subpixel_offset=off, tile_rows=band, out_planes=one,
+                                       out_peers=[one.data_ptr()]),
+                   Hh.run_ours_forward(d, cam, 3, bg, subpixel_offset=off, tile_rows=band, out_planes=two[0],
+                                       out_peers=[two[0].data_ptr(), two[1].data_ptr()]),
                    f):
             nc = Hh.our_internals(fp, scene.P, H, W)["n_contrib"].view(H, W)
             assert torch.equal(nc[y0:y1], full_nc[y0:y1]), g
@@ -255,11 +232,11 @@ def test_phase1_band_and_peer_sums_with_offsets(cuda_device):
     dev = cuda_device
     scene, cam, d = _city(dev)
     bg = torch.tensor([0.1, 0.0, 0.2], device=dev)
-    off = _offsets(cam, dev)
+    off = Hh.uniform_offsets(cam.height, cam.width, dev, 23)
     cot = [torch.from_numpy(c).to(dev) for c in S.cotangents(cam.width, cam.height, seed=2)]
     P = scene.P
-    full = _fwd(d, cam, 3, bg, off)
-    ref = _bwd(d, cam, 3, bg, full, cot, off, phase=1)
+    full = Hh.run_ours_forward(d, cam, 3, bg, subpixel_offset=off)
+    ref = Hh.run_ours_backward(d, cam, 3, bg, full, cot, subpixel_offset=off, phase=1)
     tol = 1e-5 + 2e-4 * ref.abs().max().item()
     cuts = _cuts(full, scene, cam, 3)
     half = (P + 1) // 2
@@ -268,59 +245,47 @@ def test_phase1_band_and_peer_sums_with_offsets(cuda_device):
     total = torch.zeros((P, 16), device=dev)
     for g in range(3):
         band = (cuts[g], cuts[g + 1])
-        f = _fwd(d, cam, 3, bg, off, band)
-        total += _bwd(d, cam, 3, bg, f, cot, off, band, phase=1)
-        assert _bwd(d, cam, 3, bg, f, cot, off, band, phase=1, acc_peers=[acc_p.data_ptr()], peer_slice=P) is None
-        _bwd(d, cam, 3, bg, f, cot, off, band, phase=1, acc_peers=[acc_q.data_ptr(), acc_q[half:].data_ptr()],
-             peer_slice=half)
+        f = Hh.run_ours_forward(d, cam, 3, bg, subpixel_offset=off, tile_rows=band)
+        total += Hh.run_ours_backward(d, cam, 3, bg, f, cot, subpixel_offset=off, tile_rows=band, phase=1)
+        assert Hh.run_ours_backward(d, cam, 3, bg, f, cot, subpixel_offset=off, tile_rows=band, phase=1,
+                                    acc_peers=[acc_p.data_ptr()], peer_slice=P) is None
+        Hh.run_ours_backward(d, cam, 3, bg, f, cot, subpixel_offset=off, tile_rows=band, phase=1,
+                             acc_peers=[acc_q.data_ptr(), acc_q[half:].data_ptr()], peer_slice=half)
     torch.cuda.synchronize(dev)
     for name, got in (("bands", total), ("one peer", acc_p), ("two peers", acc_q[:P])):
         assert (got - ref).abs().max().item() <= tol, name
     # the offsets matter here: the sums without them differ by far more
-    plain = _bwd(d, cam, 3, bg, _fwd(d, cam, 3, bg), cot, phase=1)
+    plain = Hh.run_ours_backward(d, cam, 3, bg, Hh.run_ours_forward(d, cam, 3, bg), cot, phase=1)
     assert (plain - ref).abs().max().item() > 10 * tol
-
-
-_FRAMES = {}
 
 
 def _camera_case(name, jitter, dev):
     """One-call deterministic camera + focal gradients, the deterministic phase-1 sums, and the float64 / float32
     restatements on those sums, for a 200k-Gaussian city frame at 640x360."""
-    key = (name, jitter)
-    if key in _FRAMES:
-        return _FRAMES[key]
-    D = 3 if name == "d3" else 1
-    scene, cam, d = _city(dev, D=D, P=200_000, extent=128.0, seed=4)
-    colors = None
-    if name == "precomp":
-        colors = torch.from_numpy(np.random.default_rng(5).uniform(0, 1, size=(scene.P, 3)).astype(np.float32)).to(dev)
-    bg = torch.tensor([0.1, 0.2, 0.3], device=dev)
-    off = _offsets(cam, dev) if jitter else None
-    f = _fwd(d, cam, D, bg, off, colors=colors)
-    cot = [torch.from_numpy(c).to(dev) for c in S.cotangents(cam.width, cam.height, seed=6)]
-    one = _bwd(d, cam, D, bg, f, cot, off, colors=colors, det=True, camera_grad=True, intrinsics_grad=True)
-    one = torch.cat([one[10].reshape(16), one[11].reshape(16), one[12], one[13].reshape(1), one[14].reshape(1)])
-    acc = _bwd(d, cam, D, bg, f, cot, off, colors=colors, det=True, phase=1)
-    I = Hh.our_internals(f, scene.P, cam.height, cam.width)
-    clamped = torch.stack([(I["clamped"].int() >> ch) & 1 for ch in range(3)], 1) != 0
-    args = (acc, f["radii"], d["means3D"], I["cov3D"], I["rec"][:, 5], clamped, None if colors is not None else d["shs"],
-            D, d["viewmatrix"], d["projmatrix"], d["campos"], cam.width, cam.height, cam.tanfovx, cam.tanfovy, 0.1)
-    flat = lambda r: torch.cat([r["view"].reshape(16), r["proj"].reshape(16), r["campos"].reshape(3),  # noqa: E731
-                                r["tanx"].reshape(1), r["tany"].reshape(1)]).double()
-    r64, r32 = IC.intrinsics_chain(*args, dtype=torch.float64), IC.intrinsics_chain(*args, dtype=torch.float32)
-    _FRAMES.clear()
-    _FRAMES[key] = (scene, cam, d, D, colors, bg, off, f, cot, acc, one.double(), flat(r64), flat(r32),
-                    r64["abs"].double())
-    return _FRAMES[key]
+    def make():
+        D = 3 if name == "d3" else 1
+        scene, cam, d = _city(dev, D=D, P=200_000, extent=128.0, seed=4)
+        colors = None
+        if name == "precomp":
+            colors = np.random.default_rng(5).uniform(0, 1, size=(scene.P, 3)).astype(np.float32)
+            colors = torch.from_numpy(colors).to(dev)
+        bg = torch.tensor([0.1, 0.2, 0.3], device=dev)
+        off = Hh.uniform_offsets(cam.height, cam.width, dev, 23) if jitter else None
+        f = Hh.run_ours_forward(d, cam, D, bg, subpixel_offset=off, colors=colors)
+        cot = [torch.from_numpy(c).to(dev) for c in S.cotangents(cam.width, cam.height, seed=6)]
+        one = Hh.run_ours_backward(d, cam, D, bg, f, cot, subpixel_offset=off, colors=colors, det=True,
+                                   camera_grad=True, intrinsics_grad=True)
+        one = torch.cat([one["view"].reshape(16), one["proj"].reshape(16), one["campos"], one["tanx"].reshape(1),
+                         one["tany"].reshape(1)])
+        a = Hh.restatement_inputs(f, d, cam, D, bg, cot, colors, off)
 
-
-@pytest.fixture(scope="module", autouse=True)
-def _release_cached_frames():
-    yield
-    _FRAMES.clear()
-    if torch.cuda.is_available():
-        torch.cuda.empty_cache()
+        def flat(r):
+            return torch.cat([r["view"].reshape(16), r["proj"].reshape(16), r["campos"].reshape(3),
+                              r["tanx"].reshape(1), r["tany"].reshape(1)]).double()
+        r64, r32 = CH.chain(**a, focal=True, dtype=torch.float64), CH.chain(**a, focal=True, dtype=torch.float32)
+        return (scene, cam, d, D, colors, bg, off, f, cot, a["acc"], one.double(), flat(r64), flat(r32),
+                r64["abs"].double())
+    return Hh.cached("case", (name, jitter), make)
 
 
 @pytest.mark.gpu
@@ -341,19 +306,18 @@ def test_camera_partials_of_two_slices(cuda_device, name, jitter):
         partials = []
         for a, b in ((0, cut), (cut, P)):
             kw = dict(phase=2, gauss_range=(a, b), colors=colors, det=True)
-            runs = [_bwd(d, cam, D, bg, f, cot, off, acc=acc[a:b].clone(), camera_grad=True,
-                         intrinsics_grad=ncam == 37, **kw) for _ in range(3)]
+            runs = [Hh.run_ours_backward(d, cam, D, bg, f, cot, subpixel_offset=off, acc=acc[a:b].clone(),
+                                         camera_grad=True, intrinsics_grad=ncam == 37, **kw) for _ in range(3)]
             assert len(runs[0]) == 11
             part = runs[0][10]
             assert part.dtype == torch.float64 and part.shape == (ncam,)
             for r in runs[1:]:
                 assert torch.equal(r[10].view(torch.int64), part.view(torch.int64)), (ncam, a)
-            plain = _bwd(d, cam, D, bg, f, cot, off, acc=acc[a:b].clone(), **kw)
-            for k, x, y in zip(GRAD_KEYS, runs[0][:9], plain[:9]):
+            plain = Hh.run_ours_backward(d, cam, D, bg, f, cot, subpixel_offset=off, acc=acc[a:b].clone(), **kw)
+            for k, x in zip(GRAD_KEYS, runs[0][:9]):
                 if colors is not None and k == "sh":
                     continue
-                assert torch.equal(x[a:b].contiguous().view(torch.int32), y[a:b].contiguous().view(torch.int32)), \
-                    (ncam, a, k)
+                assert torch.equal(Hh.bits(x[a:b]), Hh.bits(plain[k][a:b])), (ncam, a, k)
             partials.append(part)
         got = (partials[0] + partials[1]).float().double()
         err = (got - f64[:ncam]).abs()
@@ -371,6 +335,6 @@ def test_empty_slice_writes_zero_partials(cuda_device):
     dev = cuda_device
     scene, cam, d, D, colors, bg, off, f, cot, acc, *_ = _camera_case("d3", True, dev)
     for ncam in (35, 37):
-        r = _bwd(d, cam, D, bg, f, cot, off, phase=2, gauss_range=(5, 5), acc=acc[5:6].clone(), camera_grad=True,
-                 intrinsics_grad=ncam == 37)
+        r = Hh.run_ours_backward(d, cam, D, bg, f, cot, subpixel_offset=off, phase=2, gauss_range=(5, 5),
+                                 acc=acc[5:6].clone(), camera_grad=True, intrinsics_grad=ncam == 37)
         assert torch.equal(r[10], torch.zeros(ncam, dtype=torch.float64, device=dev))

@@ -16,9 +16,9 @@ import pytest
 import torch
 
 import helpers as Hh
+from helpers import bits, deterministic
 from sfgs import synthetic as S
-from test_deterministic import deterministic
-from test_gpu_parity import bits, check_images, check_indexing, ref_internals
+from test_gpu_parity import check_images, check_indexing, ref_internals
 
 pytestmark = pytest.mark.gpu
 GRAD_KEYS = ("means2D", "colors", "opacity", "means3D", "cov3D", "norm3D", "sh", "scales", "rot")
