@@ -383,6 +383,46 @@ int sfgs_rasterize_backward_depth_quantile(const sfgs_backward_args* a, const fl
                                            int deterministic, const uint32_t* depth_q_pos,
                                            const float* dL_dpix_depth_q, float* dL_dcamera, int ncam);
 
+/* ---- Depth distortion --------------------------------------------------------------------------------------------
+ * The one-call forward that also writes the spread of splat depths along each pixel's ray, the distortion loss of
+ * Mip-NeRF 360 / 2DGS, and the backward that differentiates it.  It is small where the pixel's opacity gathers at one
+ * depth and large where it spreads over semi-transparent layers (floaters in front of a surface).
+ *   - Per pixel, over the forward's APPLIED records in front-to-back order (not skipped by power > 0 or
+ *     alpha < 1/255, not stopped by T (1 - alpha) < 1e-4: the pairs that enter out_depth), with w_i = alpha_i T_i in
+ *     the forward's own float values and m_i the record's depth word (view-space t_z, the value out_depth blends; for
+ *     the orthographic camera too):
+ *         A  = sum w_i  (= out_alpha),   mu = sum w_i m_i / A,   M2 = sum w_i (m_i - mu)^2
+ *         R  = sum_{i<j} w_i w_j (m_i - m_j)^2 = A M2
+ *         dR/dw_i = A (m_i - mu)^2 + M2,   dR/dm_i = 2 A w_i (m_i - mu)
+ *   - The depth is the raw view depth, with no near/far remap: R has units of depth^2, and a caller's loss weight
+ *     absorbs the scene's scale (e.g. divide by the squared scene extent).
+ *   - R is accumulated about the first applied record's depth m0 (A sum w (m - m0)^2 - (sum w (m - m0))^2), so its
+ *     rounding is relative to A sum w (m - m0)^2 and does not grow with the depth itself.
+ *   - out_distortion [1,H,W]: R, or 0 where no record is applied.  out_distortion_state [2,H,W]: (mu, M2) per pixel
+ *     (0 where no record is applied).  Opaque to the caller; the backward takes it back, like norm_raw.
+ *   - Gradient, with c = dL_dpix_distortion[p]: the per-(pixel, record) dL/dw of the blend adjoint gains
+ *     c (A (m_i - mu)^2 + M2), which the recursion carries to every alpha, and the record's depth term gains
+ *     c 2 A w_i (m_i - mu), formed per pair as a difference; through them dL_dmean3D, dL_dopacity, the conic terms and
+ *     the camera terms.  A is out_alpha (accum_alphas).
+ *   - Every other output is bit-identical to the matching entry without the option, and with dL_dpix_distortion = 0
+ *     so is every gradient of the deterministic backward (up to the sign of a zero).
+ * ortho, subpixel_offset, deterministic, ncam and dL_dcamera as for the depth quantile's entries.  Phase 1 over the
+ * whole frame is accepted (acc then holds the distortion's terms too).
+ * Before any CUDA work, in this order:
+ *   forward:  a NULL args (SFGS_E_BADARG); a NULL out_distortion or out_distortion_state (SFGS_E_BADARG); ED > 0, a
+ *             tile-row band, out_peers (SFGS_E_UNSUPPORTED); then the checks of sfgs_rasterize_forward_ortho
+ *             (ortho != 0), sfgs_rasterize_forward_subpixel (offsets) or sfgs_rasterize_forward.
+ *   backward: a NULL args (SFGS_E_BADARG); a NULL distortion_state or dL_dpix_distortion, ncam not 0, 35 or 37
+ *             (SFGS_E_BADARG); ED > 0, a tile-row band, acc_peers, phase 2, ncam > 0 with phase 1, ncam > 0 with
+ *             ortho (SFGS_E_UNSUPPORTED); then the checks of the matching entry (ortho, camera[_intrinsics],
+ *             deterministic, subpixel).
+ * Not available under graph capture, with tile-row sharding, with extra_attrs or together with the depth quantile. */
+int sfgs_rasterize_forward_distortion(const sfgs_forward_args* a, const float* subpixel_offset, int ortho,
+                                      float* out_distortion, float* out_distortion_state);
+int sfgs_rasterize_backward_distortion(const sfgs_backward_args* a, const float* subpixel_offset, int ortho,
+                                       int deterministic, const float* distortion_state,
+                                       const float* dL_dpix_distortion, float* dL_dcamera, int ncam);
+
 /* ---- markVisible --------------------------------------------------------- */
 int sfgs_mark_visible(int P, const float* means3D, const float* viewmatrix,
                       const float* projmatrix, unsigned char* present, void* stream);

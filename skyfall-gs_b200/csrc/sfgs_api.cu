@@ -38,10 +38,10 @@ void sfgs_launch_tile_sort(const GeomLayout& g, const ImageLayout& im, const Bin
 void sfgs_launch_offset_bound(const ImageLayout& im, int W, int H, const float* off, cudaStream_t st);
 void sfgs_launch_render_fwd(const sfgs_forward_args* a, const GeomLayout& g, const ImageLayout& im,
                             const BinningLayout& b, const float* off, float t, float* out_depth_q,
-                            uint32_t* out_depth_q_pos, cudaStream_t st);
+                            uint32_t* out_depth_q_pos, float* out_dist, float* out_dist_state, cudaStream_t st);
 void sfgs_launch_render_bwd(const sfgs_backward_args* a, const GeomLayout& g, const ImageLayout& im,
                             const BinningLayout& b, float* acc, float* part, unsigned char* written, const float* off,
-                            bool guarded, cudaStream_t st);
+                            bool guarded, const float* dist_state, const float* dL_dpix_dist, cudaStream_t st);
 void sfgs_launch_depth_q_adjoint(const sfgs_backward_args* a, const ImageLayout& im, const BinningLayout& b,
                                  const uint32_t* depth_q_pos, const float* dL_dpix_depth_q, float* acc, float* part,
                                  cudaStream_t st);
@@ -221,6 +221,9 @@ struct FwdCall {
   float quantile = 0.f;               // ... at level q: the record crossing T = 1 - q gives depth_q [H,W] ...
   float* out_depth_q = nullptr;
   uint32_t* out_depth_q_pos = nullptr;   // ... and its 1-based list position [H,W]
+  bool dist = false;                  // the depth distortion (sfgs_rasterize_forward_distortion): R [H,W] ...
+  float* out_distortion = nullptr;
+  float* out_distortion_state = nullptr;   // ... and the state (mu, M2) [2,H,W] its adjoint reads
 };
 
 struct BwdCall {
@@ -237,6 +240,9 @@ struct BwdCall {
   bool depth_q = false;               // the depth quantile's adjoint (sfgs_rasterize_backward_depth_quantile) ...
   const uint32_t* depth_q_pos = nullptr;      // ... from the forward's positions [H,W] ...
   const float* dL_dpix_depth_q = nullptr;     // ... and the cotangent of depth_q [H,W]
+  bool dist = false;                  // the depth distortion's adjoint (sfgs_rasterize_backward_distortion) ...
+  const float* distortion_state = nullptr;    // ... from the forward's state [2,H,W] ...
+  const float* dL_dpix_distortion = nullptr;  // ... and the cotangent of R [H,W]
 };
 
 int rasterize_forward(const sfgs_forward_args* a, const FwdCall& c);
@@ -366,6 +372,29 @@ int sfgs_rasterize_backward_depth_quantile(const sfgs_backward_args* a, const fl
   return rasterize_backward(a, c);
 }
 
+int sfgs_rasterize_forward_distortion(const sfgs_forward_args* a, const float* subpixel_offset, int ortho,
+                                      float* out_distortion, float* out_distortion_state) {
+  FwdCall c{"forward_distortion", false, subpixel_offset};
+  c.ortho = ortho != 0;
+  c.dist = true;
+  c.out_distortion = out_distortion;
+  c.out_distortion_state = out_distortion_state;
+  return rasterize_forward(a, c);
+}
+
+int sfgs_rasterize_backward_distortion(const sfgs_backward_args* a, const float* subpixel_offset, int ortho,
+                                       int deterministic, const float* distortion_state,
+                                       const float* dL_dpix_distortion, float* dL_dcamera, int ncam) {
+  // ncam > 0: the checks and the stages of sfgs_rasterize_backward_camera[_intrinsics] (a bad ncam is rejected first)
+  BwdCall c{"backward_distortion", ncam > 0 ? BwdCall::CAMERA : BwdCall::EAGER, subpixel_offset, false,
+            deterministic != 0, ncam, ncam > 0 ? dL_dcamera : nullptr};
+  c.ortho = ortho != 0;
+  c.dist = true;
+  c.distortion_state = distortion_state;
+  c.dL_dpix_distortion = dL_dpix_distortion;
+  return rasterize_backward(a, c);
+}
+
 }  // extern "C"
 
 namespace {
@@ -387,6 +416,15 @@ int check_forward(const sfgs_forward_args* a, const FwdCall& c) {
     if (a->tile_row_begin != 0 || a->tile_row_end != 0)
       return reject(SFGS_E_UNSUPPORTED, "tile-row bands are not supported with the depth quantile");
     if (a->out_peers != nullptr) return reject(SFGS_E_UNSUPPORTED, "out_peers are not supported with the depth quantile");
+  }
+  if (c.dist) {
+    if (!c.out_distortion || !c.out_distortion_state)
+      return reject(SFGS_E_BADARG, "null out_distortion or out_distortion_state");
+    if (a->ED > 0) return reject(SFGS_E_UNSUPPORTED, "extra_attrs are not supported with the depth distortion");
+    if (a->tile_row_begin != 0 || a->tile_row_end != 0)
+      return reject(SFGS_E_UNSUPPORTED, "tile-row bands are not supported with the depth distortion");
+    if (a->out_peers != nullptr)
+      return reject(SFGS_E_UNSUPPORTED, "out_peers are not supported with the depth distortion");
   }
   if (c.ortho) {
     if (a->tile_row_begin != 0 || a->tile_row_end != 0)
@@ -498,7 +536,7 @@ int rasterize_forward(const sfgs_forward_args* a, const FwdCall& c) {
     PROF_BEGIN(ST_RENDER_FWD);
     // t = 1 - q in float32: the transmittance the selected record crosses
     sfgs_launch_render_fwd(a, g, im, b, off, 1.0f - c.quantile, c.depth_q ? c.out_depth_q : nullptr, c.out_depth_q_pos,
-                           st);
+                           c.dist ? c.out_distortion : nullptr, c.out_distortion_state, st);
     PROF_END();
     STAGE_CHECK("render_fwd");
     return SFGS_OK;
@@ -568,6 +606,21 @@ int check_backward(const sfgs_backward_args* a, const BwdCall& c) {
       return reject(SFGS_E_UNSUPPORTED, "tile-row bands are not supported with the depth quantile");
     if (a->acc_peers != nullptr) return reject(SFGS_E_UNSUPPORTED, "acc_peers are not supported with the depth quantile");
     if (a->phase == 2) return reject(SFGS_E_UNSUPPORTED, "phase 2 is not supported with the depth quantile");
+    if (c.ncam > 0 && a->phase == 1)
+      return reject(SFGS_E_UNSUPPORTED, "camera gradients are formed by the one-call backward (phase 0) only");
+    if (c.ncam > 0 && c.ortho)
+      return reject(SFGS_E_UNSUPPORTED, "the orthographic camera has no camera gradients");
+  }
+  if (c.dist) {
+    if (!c.distortion_state || !c.dL_dpix_distortion)
+      return reject(SFGS_E_BADARG, "null distortion_state or dL_dpix_distortion");
+    if (c.ncam != 0 && c.ncam != 35 && c.ncam != 37) return reject(SFGS_E_BADARG, "ncam must be 0, 35 or 37");
+    if (a->ED > 0) return reject(SFGS_E_UNSUPPORTED, "extra_attrs are not supported with the depth distortion");
+    if (a->tile_row_begin != 0 || a->tile_row_end != 0)
+      return reject(SFGS_E_UNSUPPORTED, "tile-row bands are not supported with the depth distortion");
+    if (a->acc_peers != nullptr)
+      return reject(SFGS_E_UNSUPPORTED, "acc_peers are not supported with the depth distortion");
+    if (a->phase == 2) return reject(SFGS_E_UNSUPPORTED, "phase 2 is not supported with the depth distortion");
     if (c.ncam > 0 && a->phase == 1)
       return reject(SFGS_E_UNSUPPORTED, "camera gradients are formed by the one-call backward (phase 0) only");
     if (c.ncam > 0 && c.ortho)
@@ -718,7 +771,8 @@ int rasterize_backward(const sfgs_backward_args* a, const BwdCall& c) {
     PROF_END();
     if (R > 0) {   // graph: R is the capacity (> 0), so the adjoint always runs
       PROF_BEGIN(ST_RENDER_BWD);
-      sfgs_launch_render_bwd(a, g, im, b, acc, order.part, order.written, off, graph, st);
+      sfgs_launch_render_bwd(a, g, im, b, acc, order.part, order.written, off, graph,
+                             c.dist ? c.distortion_state : nullptr, c.dL_dpix_distortion, st);
       if (c.depth_q) sfgs_launch_depth_q_adjoint(a, im, b, c.depth_q_pos, c.dL_dpix_depth_q, acc, order.part, st);
       PROF_END();
       STAGE_CHECK("render_bwd");
@@ -742,7 +796,8 @@ int rasterize_backward(const sfgs_backward_args* a, const BwdCall& c) {
     PROF_END();
     if (a->R > 0 || graph) {
       PROF_BEGIN(ST_RENDER_BWD);
-      sfgs_launch_render_bwd(a, g, im, b, acc, nullptr, nullptr, off, graph, st);
+      sfgs_launch_render_bwd(a, g, im, b, acc, nullptr, nullptr, off, graph, c.dist ? c.distortion_state : nullptr,
+                             c.dL_dpix_distortion, st);
       if (c.depth_q) sfgs_launch_depth_q_adjoint(a, im, b, c.depth_q_pos, c.dL_dpix_depth_q, acc, nullptr, st);
       PROF_END();
       STAGE_CHECK("render_bwd");

@@ -72,6 +72,11 @@ struct WarpSmem {
 struct WarpSmemJitter : WarpSmem {
   float2 pos[32];               // 256 B   per-pixel sample positions (JITTER)
 };
+// DIST: the pixel rows widened by the depth distortion's per-pixel constants
+template <class Base>
+struct WarpSmemDist : Base {
+  float2 dist[32];              // 256 B   (2 c A, mu) per pixel
+};
 
 // HAS_EXTRA: also the adjoint of the ED channels of `extras` [P,ED] (extra_attrs; Skyfall-GS never passes them):
 // phase 1 keeps the reference's per-pixel recursion of the extras and adds one global atomicAdd per (pixel, Gaussian,
@@ -82,7 +87,12 @@ struct WarpSmemJitter : WarpSmem {
 // JITTER: subpixel offsets — pixel (x, y) samples the splats at (x, y) + off[W y + x] ([H,W,2] floats, the buffer the
 // forward used).  Phase 1 only moves the pixel; phase 2 sums h against each pixel's sample position about the half's
 // centre (read from the warp's table `pos`), with the same centred origin.
-template <bool PEER, bool HAS_EXTRA, bool ORDERED, bool JITTER>
+// DIST: the depth distortion's adjoint (sfgs_rasterize_backward_distortion).  With c = dL/dR, A = the pixel's alpha and
+// the forward's state (mu, M2): dR/dw_i = A (m_i - mu)^2 + M2 joins g, the record's dL/dw, so the recursion carries
+// it to every alpha -- the M2 term is the same for every record and joins the alpha cotangent, the other is formed per
+// slot from (2 c A, mu) in the warp's table `dist`; dR/dm_i = 2 A w_i (m_i - mu) joins the depth word (3) of phase 2,
+// formed per (pixel, slot) as the difference m_i - mu.  With c = 0 every sum is what it is without the option.
+template <bool PEER, bool HAS_EXTRA, bool ORDERED, bool JITTER, bool DIST>
 __device__ __forceinline__ void
 render_bwd_warp(const uint2* __restrict__ ranges, const char* __restrict__ binning_base,
                 const uint32_t* __restrict__ hdr, int W, int H, int band0,
@@ -93,8 +103,10 @@ render_bwd_warp(const uint2* __restrict__ ranges, const char* __restrict__ binni
                 const float* __restrict__ norm_raw, float* __restrict__ acc /* [P,16] zero-initialised */,
                 const PeerTable peers, const float* __restrict__ extras,
                 const float* __restrict__ dL_dpixel_extras, float* __restrict__ dL_dextras, int ED,
-                float* __restrict__ part, unsigned char* __restrict__ written, const float2* __restrict__ off) {
-  using Smem = std::conditional_t<JITTER, WarpSmemJitter, WarpSmem>;
+                float* __restrict__ part, unsigned char* __restrict__ written, const float2* __restrict__ off,
+                const float* __restrict__ dist_state, const float* __restrict__ dL_dpix_dist) {
+  using SmemBase = std::conditional_t<JITTER, WarpSmemJitter, WarpSmem>;
+  using Smem = std::conditional_t<DIST, WarpSmemDist<SmemBase>, SmemBase>;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   Smem& S = reinterpret_cast<Smem*>(smem_raw)[wid];
@@ -146,6 +158,15 @@ render_bwd_warp(const uint2* __restrict__ ranges, const char* __restrict__ binni
       dLn0 = r0; dLn1 = r1; dLn2 = r2;
     }
   }
+  if constexpr (DIST) {
+    float2 q = make_float2(0.f, 0.f);
+    if (inside) {
+      const float c = dL_dpix_dist[pix_id];
+      dLa = fmaf(c, dist_state[HW + pix_id], dLa);
+      q = make_float2(2.f * c * accum_alphas[pix_id], dist_state[pix_id]);
+    }
+    S.dist[lane] = q;
+  }
   // background term of dL/dalpha: (-T_final / (1 - alpha)) * <bg, dL/dcolour>
   const float tb = -T_final * (bg_color[0] * dLc0 + bg_color[1] * dLc1 + bg_color[2] * dLc2);
   {
@@ -179,6 +200,7 @@ render_bwd_warp(const uint2* __restrict__ ranges, const char* __restrict__ binni
   // reference keeps A, g_last and last_alpha and forms this only at the next record); last_alpha is kept for the
   // extras' recursion only
   float C = 0.f, last_alpha = 0.f;
+  float dcA = 0.f, dmu = 0.f;                  // DIST: c A and mu, read from the warp's table at each chunk
   const SfgsExpConsts ek = sfgs_exp_consts(hdr[HDR_ZERO]);
   BlendWalk<true, ORDERED ? GID_INSTANCE : GID_GAUSSIAN> walk(S.st, inst_mask, point_list, rec, range, used, wid,
                                                                lane);
@@ -198,6 +220,15 @@ render_bwd_warp(const uint2* __restrict__ ranges, const char* __restrict__ binni
     const uint32_t gid = S.st.gid[buf][slot];
     const float2* whp = &S.wh[chalf * 16][ck];
     const float4* pix = reinterpret_cast<const float4*>(&S.pix[chalf * 16][0]);
+    // DIST: each pixel's depth cotangent for this record, dL/d depth + 2 c A (m - mu)
+    const auto dLd_of = [&](const int i, const float dLd_i) {
+      if constexpr (DIST) {
+        const float2 q = S.dist[chalf * 16 + i];
+        return fmaf(q.x, rb.z - q.y, dLd_i);
+      } else {
+        return dLd_i;
+      }
+    };
     const float DX = ra.x - pix[1].w, DY = ra.y - pix[3].w;
     // abs-gradient term |h| (|u| + |v|), u = (W/2)(con.x dx + con.y dy), v = (H/2)(con.y dx + con.z dy): affine in
     // the pixel offset, so each is one FFMA from its row's base.  au .. bv are the conic scaled by d(ndc)/d(pixel)
@@ -222,7 +253,8 @@ render_bwd_warp(const uint2* __restrict__ ranges, const char* __restrict__ binni
         const float x = q.x - hcx, y = q.y - hcy;
         const float2 wh = whp[i * (BLEND_CH + 1)];
         const float4 p0 = pix[2 * i], p1 = pix[2 * i + 1];
-        s0 = fmaf(wh.x, p0.x, s0); s1 = fmaf(wh.x, p0.y, s1); s2 = fmaf(wh.x, p0.z, s2); s3 = fmaf(wh.x, p0.w, s3);
+        s0 = fmaf(wh.x, p0.x, s0); s1 = fmaf(wh.x, p0.y, s1); s2 = fmaf(wh.x, p0.z, s2);
+        s3 = fmaf(wh.x, dLd_of(i, p0.w), s3);
         s4 = fmaf(wh.x, p1.x, s4); s5 = fmaf(wh.x, p1.y, s5); s6 = fmaf(wh.x, p1.z, s6);
         const float hx = wh.y * x, hy = wh.y * y;
         sh += wh.y;
@@ -243,7 +275,8 @@ render_bwd_warp(const uint2* __restrict__ ranges, const char* __restrict__ binni
         const int r = i >> 3;
         const float2 wh = whp[i * (BLEND_CH + 1)];
         const float4 p0 = pix[2 * i], p1 = pix[2 * i + 1];
-        s0 = fmaf(wh.x, p0.x, s0); s1 = fmaf(wh.x, p0.y, s1); s2 = fmaf(wh.x, p0.z, s2); s3 = fmaf(wh.x, p0.w, s3);
+        s0 = fmaf(wh.x, p0.x, s0); s1 = fmaf(wh.x, p0.y, s1); s2 = fmaf(wh.x, p0.z, s2);
+        s3 = fmaf(wh.x, dLd_of(i, p0.w), s3);
         s4 = fmaf(wh.x, p1.x, s4); s5 = fmaf(wh.x, p1.y, s5); s6 = fmaf(wh.x, p1.z, s6);
         h1[r] += wh.y;
         hx[r] = fmaf(wh.y, x, hx[r]);
@@ -323,6 +356,10 @@ render_bwd_warp(const uint2* __restrict__ ranges, const char* __restrict__ binni
     g += rc.z * dLc2; g2 += rd.y * dLn2;
     g += rb.z * dLd;  g2 += dLa;
     g += g2;
+    if constexpr (DIST) {
+      const float dm = rb.z - dmu;
+      g = fmaf(dcA * dm, dm, g);
+    }
     float dL_dalpha_T = g - C;                  // dL/dalpha / T
     if constexpr (HAS_EXTRA) {
       const uint32_t gid = S.st.gid[buf][k];
@@ -350,6 +387,11 @@ render_bwd_warp(const uint2* __restrict__ ranges, const char* __restrict__ binni
       pixfx = q.x;
       pixfy = q.y;
     }
+    if constexpr (DIST) {
+      const float2 q = S.dist[lane];
+      dcA = 0.5f * q.x;
+      dmu = q.y;
+    }
     if (n == BLEND_CH) {                            // every chunk of a warp but its last: no per-slot bound test
       // slot k+1's parameters are read before slot k's hand-over store (the compiler cannot move a shared-memory
       // load above that store on its own), so their latency overlaps slot k's arithmetic
@@ -372,8 +414,10 @@ render_bwd_warp(const uint2* __restrict__ ranges, const char* __restrict__ binni
 // nothing, and new parameters go at the end of the list.  GUARDED (the graph backward, sfgs_rasterize_backward_graph):
 // launched whatever the frame's instance count, so it first checks the forward's overflow flag -- after an overflow the
 // ranges run past the binning capacity and nothing may read point_list or write partial rows.
-template <bool PEER, bool HAS_EXTRA, bool ORDERED, bool JITTER, bool GUARDED>
-__global__ void __launch_bounds__(BLEND_THREADS, 3)
+// DIST (the depth distortion) is instantiated only without peers, extras and GUARDED, at two CTAs per SM: at the 80
+// registers of three its instantiations spilled (8 to 20 bytes).
+template <bool PEER, bool HAS_EXTRA, bool ORDERED, bool JITTER, bool GUARDED, bool DIST>
+__global__ void __launch_bounds__(BLEND_THREADS, DIST ? 2 : 3)
 render_bwd_kernel(const uint2* __restrict__ ranges, const char* __restrict__ binning_base,
                   const uint32_t* __restrict__ hdr, int W, int H, int band0,
                   const float* __restrict__ bg_color, const float* __restrict__ rec,
@@ -383,18 +427,26 @@ render_bwd_kernel(const uint2* __restrict__ ranges, const char* __restrict__ bin
                   const float* __restrict__ norm_raw, float* __restrict__ acc /* [P,16] zero-initialised */,
                   const PeerTable peers, const float* __restrict__ extras,
                   const float* __restrict__ dL_dpixel_extras, float* __restrict__ dL_dextras, int ED,
-                  float* __restrict__ part, unsigned char* __restrict__ written, const float2* __restrict__ off) {
+                  float* __restrict__ part, unsigned char* __restrict__ written, const float2* __restrict__ off,
+                  const float* __restrict__ dist_state, const float* __restrict__ dL_dpix_dist) {
   if (GUARDED && hdr[HDR_OVERFLOW]) return;
-  render_bwd_warp<PEER, HAS_EXTRA, ORDERED, JITTER>(ranges, binning_base, hdr, W, H, band0, bg_color, rec, accum_alphas,
-                                                    n_contrib, dL_dpixels, dL_dpixel_depths, dL_dpixel_norms,
-                                                    dL_dpixel_alphas, norm_raw, acc, peers, extras, dL_dpixel_extras,
-                                                    dL_dextras, ED, part, written, off);
+  render_bwd_warp<PEER, HAS_EXTRA, ORDERED, JITTER, DIST>(ranges, binning_base, hdr, W, H, band0, bg_color, rec,
+                                                          accum_alphas, n_contrib, dL_dpixels, dL_dpixel_depths,
+                                                          dL_dpixel_norms, dL_dpixel_alphas, norm_raw, acc, peers,
+                                                          extras, dL_dpixel_extras, dL_dextras, ED, part, written, off,
+                                                          dist_state, dL_dpix_dist);
 }
 
-template <bool PEER, bool HAS_EXTRA, bool ORDERED, bool JITTER, bool GUARDED>
+template <bool JITTER, bool DIST>
+constexpr size_t render_bwd_smem() {
+  using Base = std::conditional_t<JITTER, WarpSmemJitter, WarpSmem>;
+  return BLEND_WARPS * sizeof(std::conditional_t<DIST, WarpSmemDist<Base>, Base>);
+}
+
+template <bool PEER, bool HAS_EXTRA, bool ORDERED, bool JITTER, bool GUARDED, bool DIST = false>
 auto render_bwd_instance() {
-  return sfgs_smem_kernel<render_bwd_kernel<PEER, HAS_EXTRA, ORDERED, JITTER, GUARDED>>(
-      BLEND_WARPS * (JITTER ? sizeof(WarpSmemJitter) : sizeof(WarpSmem)));
+  return sfgs_smem_kernel<render_bwd_kernel<PEER, HAS_EXTRA, ORDERED, JITTER, GUARDED, DIST>>(
+      render_bwd_smem<JITTER, DIST>());
 }
 
 // The adjoint of the depth quantile (sfgs_rasterize_backward_depth_quantile): dL/d depth_j += dL/d depth_q[p] for the
@@ -451,10 +503,11 @@ void sfgs_launch_depth_q_adjoint(const sfgs_backward_args* a, const ImageLayout&
 }
 
 // guarded: the graph backward's blend adjoint.  The entry points' checks leave these combinations: peers only in the
-// eager non-deterministic backward; extra_attrs only without offsets and without the ordered form (part != nullptr).
+// eager non-deterministic backward; extra_attrs only without offsets and without the ordered form (part != nullptr);
+// the depth distortion (dist_state != nullptr) only eager, without peers and extra_attrs.
 void sfgs_launch_render_bwd(const sfgs_backward_args* a, const GeomLayout& g, const ImageLayout& im,
                             const BinningLayout& b, float* acc, float* part, unsigned char* written, const float* off,
-                            bool guarded, cudaStream_t st) {
+                            bool guarded, const float* dist_state, const float* dL_dpix_dist, cudaStream_t st) {
   dim3 grid;
   int band0;
   if (!blend_grid(a->tile_row_begin, a->tile_row_end, im, grid, band0)) return;
@@ -464,10 +517,14 @@ void sfgs_launch_render_bwd(const sfgs_backward_args* a, const GeomLayout& g, co
     for (int r = 0; r < a->n_peers && r < 8; r++) pt.p[r] = a->acc_peers[r];
     pt.per = a->peer_slice;
   }
-  const bool ordered = part != nullptr, extra = a->ED > 0;
-  // render_bwd_instance<PEER, HAS_EXTRA, ORDERED, JITTER, GUARDED>
+  const bool ordered = part != nullptr, extra = a->ED > 0, dist = dist_state != nullptr;
+  // render_bwd_instance<PEER, HAS_EXTRA, ORDERED, JITTER, GUARDED[, DIST]>
   const auto kernel =
-      guarded ? (off != nullptr ? (ordered ? render_bwd_instance<false, false, true, true, true>()
+      dist ? (off != nullptr ? (ordered ? render_bwd_instance<false, false, true, true, false, true>()
+                                        : render_bwd_instance<false, false, false, true, false, true>())
+              : ordered      ? render_bwd_instance<false, false, true, false, false, true>()
+                             : render_bwd_instance<false, false, false, false, false, true>())
+      : guarded ? (off != nullptr ? (ordered ? render_bwd_instance<false, false, true, true, true>()
                                            : render_bwd_instance<false, false, false, true, true>())
                  : ordered      ? render_bwd_instance<false, false, true, false, true>()
                  : extra        ? render_bwd_instance<false, true, false, false, true>()
@@ -479,11 +536,12 @@ void sfgs_launch_render_bwd(const sfgs_backward_args* a, const GeomLayout& g, co
       : extra   ? render_bwd_instance<false, true, false, false, false>()
       : peer    ? render_bwd_instance<true, false, false, false, false>()
                 : render_bwd_instance<false, false, false, false, false>();
-  const size_t smem = BLEND_WARPS * (off != nullptr ? sizeof(WarpSmemJitter) : sizeof(WarpSmem));
+  const size_t smem = off != nullptr ? (dist ? render_bwd_smem<true, true>() : render_bwd_smem<true, false>())
+                                      : (dist ? render_bwd_smem<false, true>() : render_bwd_smem<false, false>());
   SFGS_COUNT_LAUNCH();
   kernel<<<grid, BLEND_THREADS, smem, st>>>(im.ranges, (const char*)b.point_list, im.hdr, a->width, a->height, band0,
                                           a->background, g.rec, a->accum_alphas, im.n_contrib, a->dL_dpix,
                                           a->dL_dpix_depth, a->dL_dpix_norm, a->dL_dpix_alpha, a->norm_raw, acc, pt,
                                           a->extra_attrs, a->dL_dpix_extra, a->dL_dextra, a->ED, part, written,
-                                          reinterpret_cast<const float2*>(off));
+                                          reinterpret_cast<const float2*>(off), dist_state, dL_dpix_dist);
 }

@@ -37,7 +37,13 @@ using PeersArg = std::conditional_t<HAS_EXTRA, const OutPeers, const OutPeers&>;
 // list position; a pixel without one gets 0 and 0.  T strictly decreases over the applied records, so at most one
 // record is selected.  The branch-free slot body keeps only the position (one compare and one select); the epilogue
 // reads the selected record's depth word, so out_depth_q is that word bit for bit.
-template <bool HAS_EXTRA, bool JITTER, bool QDEPTH>
+// DIST: the depth distortion (sfgs_rasterize_forward_distortion).  Over the applied records, with w = alpha T and m the
+// depth word, the slot body accumulates A = sum w, S1 = sum w (m - m0) and S2 = sum w (m - m0)^2 about the first
+// applied record's depth m0 (a record is the first applied one iff T is still exactly 1: an applied record has
+// alpha >= 1/255).  The epilogue writes R = A S2 - S1^2 = sum_{i<j} w_i w_j (m_i - m_j)^2, whose rounding is relative
+// to A S2 and does not grow with the depth itself (the unshifted A sum w m^2 - (sum w m)^2 cancels at depths of
+// hundreds), and the state (mu, M2) = (m0 + S1 / A, R / A) the adjoint reads.
+template <bool HAS_EXTRA, bool JITTER, bool QDEPTH, bool DIST>
 __device__ __forceinline__ void
 render_fwd_warp(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list,
                 const unsigned char* __restrict__ inst_mask, const uint32_t* __restrict__ hdr, int W, int H,
@@ -46,7 +52,8 @@ render_fwd_warp(const uint2* __restrict__ ranges, const uint32_t* __restrict__ p
                 float* __restrict__ out_norm_raw, float* __restrict__ out_alpha, uint32_t* __restrict__ n_contrib,
                 PeersArg<HAS_EXTRA> peers, const float* __restrict__ extras, int ED, float* __restrict__ out_extra,
                 const float2* __restrict__ off, float t, float* __restrict__ out_depth_q,
-                uint32_t* __restrict__ out_depth_q_pos) {
+                uint32_t* __restrict__ out_depth_q_pos, float* __restrict__ out_dist,
+                float* __restrict__ out_dist_state) {
   if (hdr[HDR_OVERFLOW]) return;
   __shared__ BlendStage<HAS_EXTRA> s_warp[BLEND_WARPS];   // extra_attrs: the slot's gid word is the Gaussian id
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
@@ -68,6 +75,7 @@ render_fwd_warp(const uint2* __restrict__ ranges, const uint32_t* __restrict__ p
   float T_done = 0.0f;
   uint32_t last_contributor = 0;
   uint32_t Pq = 0;                  // QDEPTH: the selected record's list position
+  float m0 = 0.f, A = 0.f, S1 = 0.f, S2 = 0.f;   // DIST: the reference depth and the shifted sums
   float C0 = 0.f, C1 = 0.f, C2 = 0.f, Dp = 0.f, N0 = 0.f, N1 = 0.f, N2 = 0.f;
   float E[HAS_EXTRA ? SFGS_MAX_EXTRA : 1];
   if constexpr (HAS_EXTRA)
@@ -96,6 +104,14 @@ render_fwd_warp(const uint2* __restrict__ ranges, const uint32_t* __restrict__ p
     // image reaches hundreds of units, where 1e-5 absolute is below one ulp, so it keeps the reference's exact
     // association (depth * alpha) * T and stays bit-identical
     const float w = alpha * Ta;
+    if constexpr (DIST) {
+      m0 = apply && T == 1.0f ? c.z : m0;
+      const float dm = c.z - m0;
+      const float wd = w * dm;
+      A += w;
+      S1 += wd;
+      S2 = fmaf(wd, dm, S2);
+    }
     C0 = fmaf(f.x, w, C0); C1 = fmaf(f.y, w, C1); C2 = fmaf(f.z, w, C2);
     Dp = fmaf(c.z * alpha, Ta, Dp);
     N0 = fmaf(f.w, w, N0); N1 = fmaf(g.x, w, N1); N2 = fmaf(g.y, w, N2);
@@ -160,6 +176,14 @@ render_fwd_warp(const uint2* __restrict__ ranges, const uint32_t* __restrict__ p
       out_depth_q[pix_id] = Pq ? rec[(size_t)point_list[range.x + Pq - 1] * REC_FLOATS + REC_DEPTH] : 0.f;
       out_depth_q_pos[pix_id] = Pq;
     }
+    if constexpr (DIST) {
+      // S1^2 <= A S2 up to rounding: a pixel whose records share one depth gets 0, not a negative rounding residue
+      const float R = fmaxf(fmaf(A, S2, -S1 * S1), 0.f);
+      const bool any = A > 0.f;
+      out_dist[pix_id] = R;
+      out_dist_state[pix_id] = any ? m0 + S1 / A : 0.f;
+      out_dist_state[HW + pix_id] = any ? R / A : 0.f;
+    }
   }
 }
 
@@ -170,8 +194,9 @@ enum class FwdOut { LOCAL_OR_PEERS, LOCAL, PEERS };
 
 // The one blend forward.  Each option is a template argument; a trailing parameter an instantiation does not read
 // (off without JITTER, extras without HAS_EXTRA) costs nothing, and new parameters go at the end of the list.
-// QDEPTH (the depth quantile) is instantiated only with local outputs and without extras, with and without jitter.
-template <bool HAS_EXTRA, bool JITTER, FwdOut OUT, bool QDEPTH>
+// QDEPTH (the depth quantile) and DIST (the depth distortion) are instantiated one at a time, only with local outputs
+// and without extras, with and without jitter.
+template <bool HAS_EXTRA, bool JITTER, FwdOut OUT, bool QDEPTH, bool DIST>
 __global__ void __launch_bounds__(BLEND_THREADS)
 render_fwd_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list,
                   const unsigned char* __restrict__ inst_mask, const uint32_t* __restrict__ hdr, int W, int H,
@@ -180,14 +205,16 @@ render_fwd_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__
                   float* __restrict__ out_norm_raw, float* __restrict__ out_alpha, uint32_t* __restrict__ n_contrib,
                   const OutPeers peers, const float* __restrict__ extras, int ED, float* __restrict__ out_extra,
                   const float2* __restrict__ off, float t, float* __restrict__ out_depth_q,
-                  uint32_t* __restrict__ out_depth_q_pos) {
+                  uint32_t* __restrict__ out_depth_q_pos, float* __restrict__ out_dist,
+                  float* __restrict__ out_dist_state) {
   constexpr bool local = OUT != FwdOut::PEERS;
   const OutPeers none{};
-  render_fwd_warp<HAS_EXTRA, JITTER, QDEPTH>(ranges, point_list, inst_mask, hdr, W, H, band0, rec, bg_color,
-                                             local ? out_color : nullptr, local ? out_depth : nullptr,
-                                             local ? out_norm : nullptr, out_norm_raw, local ? out_alpha : nullptr,
-                                             n_contrib, OUT == FwdOut::LOCAL ? none : peers, extras, ED, out_extra,
-                                             off, t, out_depth_q, out_depth_q_pos);
+  render_fwd_warp<HAS_EXTRA, JITTER, QDEPTH, DIST>(ranges, point_list, inst_mask, hdr, W, H, band0, rec, bg_color,
+                                                   local ? out_color : nullptr, local ? out_depth : nullptr,
+                                                   local ? out_norm : nullptr, out_norm_raw,
+                                                   local ? out_alpha : nullptr, n_contrib,
+                                                   OUT == FwdOut::LOCAL ? none : peers, extras, ED, out_extra, off, t,
+                                                   out_depth_q, out_depth_q_pos, out_dist, out_dist_state);
 }
 
 // max |off_x|, max |off_y| over the frame into HDR_OFF_EX / HDR_OFF_EY (non-negative floats order as their bits), and
@@ -225,10 +252,11 @@ void sfgs_launch_offset_bound(const ImageLayout& im, int W, int H, const float* 
   offset_bound_kernel<<<blocks, 256, 0, st>>>(n, reinterpret_cast<const float2*>(off), im.hdr);
 }
 
-// out_depth_q != NULL: the depth quantile at t = 1 - q (the entry's checks leave it no extras, peers or band)
+// out_depth_q != NULL: the depth quantile at t = 1 - q; out_dist != NULL: the depth distortion and its state [2,H,W]
+// (the entries' checks leave either no extras, peers or band, and never both)
 void sfgs_launch_render_fwd(const sfgs_forward_args* a, const GeomLayout& g, const ImageLayout& im,
                             const BinningLayout& b, const float* off, float t, float* out_depth_q,
-                            uint32_t* out_depth_q_pos, cudaStream_t st) {
+                            uint32_t* out_depth_q_pos, float* out_dist, float* out_dist_state, cudaStream_t st) {
   dim3 grid;
   int band0;
   if (!blend_grid(a->tile_row_begin, a->tile_row_end, im, grid, band0)) return;
@@ -237,15 +265,19 @@ void sfgs_launch_render_fwd(const sfgs_forward_args* a, const GeomLayout& g, con
     for (op.n = 0; op.n < a->n_out_peers && op.n < 8; op.n++) op.p[op.n] = a->out_peers[op.n];
   // extra_attrs only without offsets (the _subpixel entries reject them)
   const auto kernel = out_depth_q != nullptr
-                          ? (off != nullptr ? render_fwd_kernel<false, true, FwdOut::LOCAL, true>
-                                            : render_fwd_kernel<false, false, FwdOut::LOCAL, true>)
-                      : off != nullptr ? (op.n > 0 ? render_fwd_kernel<false, true, FwdOut::PEERS, false>
-                                                   : render_fwd_kernel<false, true, FwdOut::LOCAL, false>)
-                      : a->ED > 0      ? render_fwd_kernel<true, false, FwdOut::LOCAL_OR_PEERS, false>
-                                       : render_fwd_kernel<false, false, FwdOut::LOCAL_OR_PEERS, false>;
+                          ? (off != nullptr ? render_fwd_kernel<false, true, FwdOut::LOCAL, true, false>
+                                            : render_fwd_kernel<false, false, FwdOut::LOCAL, true, false>)
+                      : out_dist != nullptr
+                          ? (off != nullptr ? render_fwd_kernel<false, true, FwdOut::LOCAL, false, true>
+                                            : render_fwd_kernel<false, false, FwdOut::LOCAL, false, true>)
+                      : off != nullptr ? (op.n > 0 ? render_fwd_kernel<false, true, FwdOut::PEERS, false, false>
+                                                   : render_fwd_kernel<false, true, FwdOut::LOCAL, false, false>)
+                      : a->ED > 0      ? render_fwd_kernel<true, false, FwdOut::LOCAL_OR_PEERS, false, false>
+                                       : render_fwd_kernel<false, false, FwdOut::LOCAL_OR_PEERS, false, false>;
   SFGS_COUNT_LAUNCH();
   kernel<<<grid, BLEND_THREADS, 0, st>>>(im.ranges, b.point_list, b.inst_mask, im.hdr, a->width, a->height, band0,
                                          g.rec, a->background, a->out_color, a->out_depth, a->out_norm, a->out_norm_raw,
                                          a->out_alpha, im.n_contrib, op, a->extra_attrs, a->ED, a->out_extra,
-                                         reinterpret_cast<const float2*>(off), t, out_depth_q, out_depth_q_pos);
+                                         reinterpret_cast<const float2*>(off), t, out_depth_q, out_depth_q_pos, out_dist,
+                                         out_dist_state);
 }

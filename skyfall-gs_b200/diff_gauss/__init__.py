@@ -10,7 +10,9 @@ RAST/diff_gauss/__init__.py:182-254 defines):
 Returned tuple: (color[3,H,W], depth[1,H,W], unit normal[3,H,W], alpha[1,H,W],
 radii[P] int32, extra[F,H,W] | empty), and with GaussianRasterizer(settings, depth_quantile=q) a 7th output,
 depth_q[1,H,W]: the depth at which the pixel's accumulated opacity crosses q (q = 0.5: the median depth), 0 where
-it never does, differentiable like the others.  `means2D` is a dummy [P,3] leaf whose
+it never does, differentiable like the others; with GaussianRasterizer(settings, depth_distortion=True) a 7th output,
+distortion[1,H,W]: sum_{i<j} w_i w_j (m_i - m_j)^2 over the pixel's blended splats, the distortion loss of Mip-NeRF
+360 / 2DGS, differentiable like the others.  `means2D` is a dummy [P,3] leaf whose
 .grad receives (dL/dx_ndc * W/2, dL/dy_ndc * H/2, sum |.|) — the densification
 statistics consumed by scene/gaussian_model.py:744-749.
 """
@@ -113,9 +115,12 @@ class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                 norm3Ds_precomp, extra_attrs, raster_settings, fuse_normalize=False, viewmatrix=None, projmatrix=None,
-                campos=None, tanfovx=None, tanfovy=None, depth_quantile=None):
+                campos=None, tanfovx=None, tanfovy=None, depth_quantile=None, depth_distortion=False):
         rs = raster_settings
         ctx.depth_q = depth_quantile is not None
+        ctx.dist = bool(depth_distortion)
+        # the option inputs after the intrinsics slots: none, the quantile, or the quantile slot and the distortion flag
+        ctx.n_options = 2 if ctx.dist else int(ctx.depth_q)
         ctx.intrinsics = None if tanfovx is None else (tanfovx, tanfovy)
         viewmatrix = rs.viewmatrix if viewmatrix is None else viewmatrix
         projmatrix = rs.projmatrix if projmatrix is None else projmatrix
@@ -136,6 +141,8 @@ class _RasterizeGaussians(torch.autograd.Function):
         if ctx.graph:
             if ctx.depth_q:
                 raise _C.SfgsError("diff_gauss: the depth quantile cannot be captured in a CUDA graph")
+            if ctx.dist:
+                raise _C.SfgsError("diff_gauss: the depth distortion cannot be captured in a CUDA graph")
             if rs.debug:
                 raise _C.SfgsError("diff_gauss: debug=True synchronises after every stage and cannot be captured in a "
                                    "CUDA graph")
@@ -144,11 +151,14 @@ class _RasterizeGaussians(torch.autograd.Function):
             fwd = functools.partial(fwd, capacity_hint=capacity, graph=True)
         if ctx.depth_q:
             fwd = functools.partial(fwd, depth_quantile=depth_quantile)
+        if ctx.dist:
+            fwd = functools.partial(fwd, depth_distortion=True)
         if off is not None:
             # the offsets travel as the last argument, so that the debug snapshot holds them too
             fwd, native_args = _with_offset(fwd), native_args + (off,)
         out = _guarded(fwd, native_args, rs.debug, "snapshot_fw.dump", "forward")
-        depth_q, depth_q_pos = out[-2:] if ctx.depth_q else (None, torch.empty(0, device=means3D.device))
+        # the 7th output and the state its backward reads: (depth_q, depth_q_pos) or (distortion, distortion_state)
+        side, side_state = out[-2:] if ctx.n_options else (None, torch.empty(0, device=means3D.device))
         if ctx.fused:
             (num_rendered, color, depth, norm, alpha, radii, extra, geom_buf, binning_buf, img_buf,
              norm_raw) = out[:11]
@@ -162,17 +172,17 @@ class _RasterizeGaussians(torch.autograd.Function):
         # the graph backward is given the capacity in place of num_rendered (not known on the host under capture)
         ctx.num_rendered = capacity if ctx.graph else num_rendered
         ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, norm3Ds_precomp, radii,
-                              extra_attrs, sh, geom_buf, binning_buf, img_buf, alpha, norm_raw, depth_q_pos)
+                              extra_attrs, sh, geom_buf, binning_buf, img_buf, alpha, norm_raw, side_state)
         ctx.mark_non_differentiable(radii)
-        if ctx.depth_q:
-            return color, depth, norm, alpha, radii, extra, depth_q
+        if ctx.n_options:
+            return color, depth, norm, alpha, radii, extra, side
         return color, depth, norm, alpha, radii, extra
 
     @staticmethod
-    def backward(ctx, g_color, g_depth, g_norm, g_alpha, _g_radii, g_extra, g_depth_q=None):
+    def backward(ctx, g_color, g_depth, g_norm, g_alpha, _g_radii, g_extra, g_side=None):
         rs = ctx.raster_settings
         (colors_precomp, means3D, scales, rotations, cov3Ds_precomp, norm3Ds_precomp, radii, extra_attrs, sh,
-         geom_buf, binning_buf, img_buf, alpha, norm_raw, depth_q_pos) = ctx.saved_tensors
+         geom_buf, binning_buf, img_buf, alpha, norm_raw, side_state) = ctx.saved_tensors
         viewmatrix, projmatrix, campos = ctx.camera
         native_args = (rs.bg, means3D, radii, colors_precomp, scales, rotations, extra_attrs, rs.scale_modifier,
                        cov3Ds_precomp, norm3Ds_precomp, viewmatrix, projmatrix, rs.tanfovx, rs.tanfovy,
@@ -193,7 +203,9 @@ class _RasterizeGaussians(torch.autograd.Function):
         if ctx.graph:
             bwd = functools.partial(bwd, graph=True)
         if ctx.depth_q:
-            bwd = functools.partial(bwd, depth_q_pos=depth_q_pos, dL_dout_depth_q=g_depth_q.contiguous())
+            bwd = functools.partial(bwd, depth_q_pos=side_state, dL_dout_depth_q=g_side.contiguous())
+        if ctx.dist:
+            bwd = functools.partial(bwd, distortion_state=side_state, dL_dout_distortion=g_side.contiguous())
         if ctx.subpixel_offset is not None:
             bwd, native_args = _with_offset(bwd), native_args + (ctx.subpixel_offset,)
         grads = _guarded(bwd, native_args, rs.debug, "snapshot_bw.dump", "backward")
@@ -203,29 +215,36 @@ class _RasterizeGaussians(torch.autograd.Function):
             g_camera = tuple(g.to(dtype=t.dtype, device=t.device) if need else None for g, t, need in
                              zip(grads[10:13], ctx.camera, ctx.needs_input_grad[_RasterizeGaussians.CAMERA_INPUTS]))
         g_intrinsics = ()
-        if ctx.intrinsics is not None or ctx.depth_q:
+        if ctx.intrinsics is not None or ctx.n_options:
             g_intrinsics = (None, None)
             if intrinsics_grad:
                 g_intrinsics = tuple(
                     g.to(dtype=t.dtype, device=t.device) if need else None for g, t, need in
                     zip(grads[13:15], ctx.intrinsics, ctx.needs_input_grad[_RasterizeGaussians.INTRINSICS_INPUTS]))
-        # order of forward's inputs; the settings tuple, the fusion flag and the quantile get no gradient
+        # order of forward's inputs; the settings tuple, the fusion flag and the options get no gradient
         return (g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rot, g_cov3D, g_norm3D, g_extra_attrs,
-                None, None) + g_camera + g_intrinsics + (None,) * ctx.depth_q
+                None, None) + g_camera + g_intrinsics + (None,) * ctx.n_options
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                        norm3Ds_precomp, extra_attrs, raster_settings, depth_quantile=None):
+                        norm3Ds_precomp, extra_attrs, raster_settings, depth_quantile=None, depth_distortion=False):
     rs = raster_settings
     # tanfovx / tanfovy may be 0-d tensors; the native layer reads them with float(), which for a CUDA tensor is a
     # host sync each forward and backward, so keep the leaves of a focal refinement on the CPU
     intrinsics = (rs.tanfovx, rs.tanfovy) if _requires_grad(rs.tanfovx) or _requires_grad(rs.tanfovy) else ()
-    # the quantile follows the two intrinsics slots (None: the settings' values)
-    quantile = () if depth_quantile is None else (intrinsics or (None, None)) + (float(depth_quantile),)
+    if depth_distortion and depth_quantile is not None:
+        raise _C.SfgsError("diff_gauss: depth_distortion and depth_quantile in one call are not supported; render "
+                           "them in two calls")
+    # the quantile, then the distortion flag, follow the two intrinsics slots (None: the settings' values)
+    options = ()
+    if depth_distortion:
+        options = (intrinsics or (None, None)) + (None, True)
+    elif depth_quantile is not None:
+        options = (intrinsics or (None, None)) + (float(depth_quantile),)
     out = _RasterizeGaussians.apply(
         means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, norm3Ds_precomp,
         extra_attrs, raster_settings, FUSE_NORMALIZE, rs.viewmatrix, rs.projmatrix, rs.campos,
-        *(quantile or intrinsics))
+        *(options or intrinsics))
     color, depth, norm, alpha, radii, extra = out[:6]
     if not FUSE_NORMALIZE:
         # the reference normalises the blended normal map in torch, inside the autograd graph (diff_gauss/__init__.py:48)
@@ -235,12 +254,15 @@ def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales,
 
 class GaussianRasterizer(nn.Module):
     """depth_quantile=q (0 < q < 1): forward() also returns depth_q [1,H,W], the depth at which each pixel's accumulated
-    opacity crosses q (include/sfgs.h, sfgs_rasterize_forward_depth_quantile).  Not under CUDA-graph capture."""
+    opacity crosses q (include/sfgs.h, sfgs_rasterize_forward_depth_quantile).  depth_distortion=True: forward() also
+    returns distortion [1,H,W], sum_{i<j} w_i w_j (m_i - m_j)^2 over each pixel's blended splats in units of depth^2
+    (include/sfgs.h, sfgs_rasterize_forward_distortion).  Not under CUDA-graph capture, and not both in one call."""
 
-    def __init__(self, raster_settings, depth_quantile=None):
+    def __init__(self, raster_settings, depth_quantile=None, depth_distortion=False):
         super().__init__()
         self.raster_settings = raster_settings
         self.depth_quantile = depth_quantile
+        self.depth_distortion = depth_distortion
 
     def markVisible(self, positions):
         """Boolean mask of the points in front of the near plane (view depth > 0.2)."""
@@ -265,4 +287,5 @@ class GaussianRasterizer(nn.Module):
 
         return rasterize_gaussians(means3D, means2D, _or_empty(shs), _or_empty(colors_precomp), opacities, scales,
                                    rotations, _or_empty(cov3Ds_precomp), _or_empty(norm3Ds_precomp),
-                                   _or_empty(extra_attrs), self.raster_settings, self.depth_quantile)
+                                   _or_empty(extra_attrs), self.raster_settings, self.depth_quantile,
+                                   self.depth_distortion)

@@ -101,6 +101,7 @@ EXPORTS = [
     "sfgs_rasterize_forward_graph", "sfgs_rasterize_backward_graph", "sfgs_capacity_estimate",
     "sfgs_rasterize_forward_ortho", "sfgs_rasterize_backward_ortho",
     "sfgs_rasterize_forward_depth_quantile", "sfgs_rasterize_backward_depth_quantile",
+    "sfgs_rasterize_forward_distortion", "sfgs_rasterize_backward_distortion",
 ]
 STAGE_NAMES = ["fwd_zero", "preprocess", "tile_scan", "emit_keys", "tile_sort", "render_fwd", "bwd_zero", "render_bwd",
                "gauss_bwd", "bwd_order"]
@@ -156,6 +157,12 @@ def lib() -> C.CDLL:
     L.sfgs_rasterize_backward_depth_quantile.argtypes = [C.POINTER(BackwardArgs), C.c_void_p, C.c_int, C.c_int,
                                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
     L.sfgs_rasterize_backward_depth_quantile.restype = C.c_int
+    L.sfgs_rasterize_forward_distortion.argtypes = [C.POINTER(ForwardArgs), C.c_void_p, C.c_int, C.c_void_p,
+                                                    C.c_void_p]
+    L.sfgs_rasterize_forward_distortion.restype = C.c_int
+    L.sfgs_rasterize_backward_distortion.argtypes = [C.POINTER(BackwardArgs), C.c_void_p, C.c_int, C.c_int,
+                                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
+    L.sfgs_rasterize_backward_distortion.restype = C.c_int
     L.sfgs_capacity_estimate.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int]
     L.sfgs_capacity_estimate.restype = C.c_longlong
     L.sfgs_mark_visible.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]

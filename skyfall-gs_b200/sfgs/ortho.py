@@ -20,6 +20,7 @@ from typing import NamedTuple, Optional
 import torch
 import torch.nn as nn
 
+from . import native as N
 from . import rasterizer as R
 
 
@@ -98,8 +99,10 @@ def _requires_grad(x):
 class _RasterizeOrtho(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                norm3Ds_precomp, extra_attrs, rs, depth_quantile=None):
+                norm3Ds_precomp, extra_attrs, rs, depth_quantile=None, depth_distortion=False):
         ctx.depth_q = depth_quantile is not None
+        ctx.dist = bool(depth_distortion)
+        ctx.n_options = 2 if ctx.dist else int(ctx.depth_q)
         n_extra = extra_attrs.shape[1] if extra_attrs.shape[0] != 0 else 0
         dev = means3D.device
         campos = torch.zeros(3, dtype=torch.float32, device=dev)      # not read by the orthographic camera
@@ -108,35 +111,43 @@ class _RasterizeOrtho(torch.autograd.Function):
             rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier, cov3Ds_precomp,
             norm3Ds_precomp, extra_attrs, n_extra, rs.viewmatrix, rs.projmatrix, rs.half_width, rs.half_height,
             rs.kernel_size, rs.image_height, rs.image_width, sh, rs.sh_degree, campos, rs.prefiltered, rs.debug,
-            fuse_normalize=True, subpixel_offset=off, ortho=True, depth_quantile=depth_quantile)
+            fuse_normalize=True, subpixel_offset=off, ortho=True, depth_quantile=depth_quantile,
+            depth_distortion=ctx.dist)
         (num_rendered, color, depth, norm, alpha, radii, extra, geom_buf, binning_buf, img_buf, norm_raw) = out[:11]
-        depth_q, depth_q_pos = out[11:] if ctx.depth_q else (None, torch.empty(0, device=dev))
+        # the 7th output and the state its backward reads: (depth_q, depth_q_pos) or (distortion, distortion_state)
+        side, side_state = out[11:] if ctx.n_options else (None, torch.empty(0, device=dev))
         ctx.rs, ctx.campos, ctx.num_rendered = rs, campos, num_rendered
         ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, norm3Ds_precomp, radii,
-                              extra_attrs, sh, geom_buf, binning_buf, img_buf, alpha, norm_raw, depth_q_pos)
+                              extra_attrs, sh, geom_buf, binning_buf, img_buf, alpha, norm_raw, side_state)
         ctx.mark_non_differentiable(radii)
         if ctx.depth_q:
             # depth_q_pos: which splat each pixel selected (0: none), for render_height_map's mask
-            ctx.mark_non_differentiable(radii, depth_q_pos)
-            return color, depth, norm, alpha, radii, extra, depth_q, depth_q_pos
+            ctx.mark_non_differentiable(radii, side_state)
+            return color, depth, norm, alpha, radii, extra, side, side_state
+        if ctx.dist:
+            return color, depth, norm, alpha, radii, extra, side
         return color, depth, norm, alpha, radii, extra
 
     @staticmethod
-    def backward(ctx, g_color, g_depth, g_norm, g_alpha, _g_radii, g_extra, g_depth_q=None, _g_depth_q_pos=None):
+    def backward(ctx, g_color, g_depth, g_norm, g_alpha, _g_radii, g_extra, g_side=None, _g_depth_q_pos=None):
         rs = ctx.rs
         (colors_precomp, means3D, scales, rotations, cov3Ds_precomp, norm3Ds_precomp, radii, extra_attrs, sh,
-         geom_buf, binning_buf, img_buf, alpha, norm_raw, depth_q_pos) = ctx.saved_tensors
-        depth_q = dict(depth_q_pos=depth_q_pos, dL_dout_depth_q=g_depth_q.contiguous()) if ctx.depth_q else {}
+         geom_buf, binning_buf, img_buf, alpha, norm_raw, side_state) = ctx.saved_tensors
+        side = {}
+        if ctx.depth_q:
+            side = dict(depth_q_pos=side_state, dL_dout_depth_q=g_side.contiguous())
+        if ctx.dist:
+            side = dict(distortion_state=side_state, dL_dout_distortion=g_side.contiguous())
         # deterministic under torch.use_deterministic_algorithms(True), as for the perspective backward
         grads = R.rasterize_gaussians_backward(
             rs.bg, means3D, radii, colors_precomp, scales, rotations, extra_attrs, rs.scale_modifier, cov3Ds_precomp,
             norm3Ds_precomp, rs.viewmatrix, rs.projmatrix, rs.half_width, rs.half_height, rs.kernel_size,
             g_color.contiguous(), g_depth.contiguous(), g_norm.contiguous(), g_alpha.contiguous(),
             g_extra.contiguous(), sh, rs.sh_degree, ctx.campos, geom_buf, ctx.num_rendered, binning_buf, img_buf,
-            alpha, rs.debug, norm_raw=norm_raw, subpixel_offset=rs.subpixel_offset, ortho=True, **depth_q)
+            alpha, rs.debug, norm_raw=norm_raw, subpixel_offset=rs.subpixel_offset, ortho=True, **side)
         (g_means2D, g_colors, g_opac, g_means3D, g_cov3D, g_norm3D, g_sh, g_scales, g_rot, g_extra_attrs) = grads
         return ((g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rot, g_cov3D, g_norm3D, g_extra_attrs, None)
-                + (None,) * ctx.depth_q)
+                + (None,) * ctx.n_options)
 
 
 class OrthoRasterizer(nn.Module):
@@ -144,12 +155,14 @@ class OrthoRasterizer(nn.Module):
     (color [3,H,W], depth [1,H,W], unit normal [3,H,W], alpha [1,H,W], radii [P], extra [F,H,W] | empty).  `means2D`'s
     .grad receives (dL/dx_ndc W/2, dL/dy_ndc H/2, sum |.|), the densification statistics.  There are no camera
     gradients: a viewmatrix or projmatrix that requires grad raises.  With depth_quantile=q (0 < q < 1) a 7th output,
-    depth_q [1,H,W], as for diff_gauss.GaussianRasterizer."""
+    depth_q [1,H,W], as for diff_gauss.GaussianRasterizer; with depth_distortion=True a 7th output, distortion [1,H,W],
+    likewise (not both in one call)."""
 
-    def __init__(self, raster_settings: OrthoRasterizationSettings, depth_quantile=None):
+    def __init__(self, raster_settings: OrthoRasterizationSettings, depth_quantile=None, depth_distortion=False):
         super().__init__()
         self.raster_settings = raster_settings
         self.depth_quantile = depth_quantile
+        self.depth_distortion = depth_distortion
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
                 cov3Ds_precomp=None, norm3Ds_precomp=None, extra_attrs=None):
@@ -175,6 +188,9 @@ class OrthoRasterizer(nn.Module):
                              "grad (detach them)")
         if rs.subpixel_offset is not None:
             R.check_subpixel_offset(rs.subpixel_offset, int(rs.image_height), int(rs.image_width))
+        if self.depth_distortion and self.depth_quantile is not None:
+            raise N.SfgsError("OrthoRasterizer: depth_distortion and depth_quantile in one call are not supported; "
+                                "render them in two calls")
 
         def _or_empty(t):
             return torch.Tensor([]) if t is None else t
@@ -182,7 +198,8 @@ class OrthoRasterizer(nn.Module):
         return _RasterizeOrtho.apply(means3D, means2D, _or_empty(shs), _or_empty(colors_precomp), opacities, scales,
                                      rotations, _or_empty(cov3Ds_precomp), _or_empty(norm3Ds_precomp),
                                      _or_empty(extra_attrs), rs,
-                                     *(() if self.depth_quantile is None else (float(self.depth_quantile),)))
+                                     *((None, True) if self.depth_distortion else
+                                       () if self.depth_quantile is None else (float(self.depth_quantile),)))
 
 
 def render_height_map(camera: NadirCamera, means3D, opacities, scales, rotations, shs=None, colors_precomp=None,

@@ -107,12 +107,19 @@ def _ortho_unsupported(where, **opts):
         raise N.SfgsError(f"{where}: {', '.join(what)} not supported with an orthographic camera")
 
 
-def _depth_q_unsupported(where, **opts):
-    """The options the depth quantile cannot take (truthy values of `opts`), as an error raised before any native
-    call."""
+def _unsupported_with(feature, where, **opts):
+    """The options `feature` cannot take (truthy values of `opts`), as an error raised before any native call."""
     what = [k for k, v in opts.items() if v]
     if what:
-        raise N.SfgsError(f"{where}: {', '.join(what)} not supported with the depth quantile")
+        raise N.SfgsError(f"{where}: {', '.join(what)} not supported with {feature}")
+
+
+def _depth_q_unsupported(where, **opts):
+    _unsupported_with("the depth quantile", where, **opts)
+
+
+def _distortion_unsupported(where, **opts):
+    _unsupported_with("the depth distortion", where, **opts)
 
 
 def _check_depth_q(depth_q_pos, dL_dout_depth_q, H, W, dev):
@@ -126,11 +133,23 @@ def _check_depth_q(depth_q_pos, dL_dout_depth_q, H, W, dev):
             raise ValueError(f"{name} must be a {dtype} tensor of shape {shapes[0]} on {dev}, got {what}")
 
 
+def _check_distortion(distortion_state, dL_dout_distortion, H, W, dev):
+    """The depth distortion's backward inputs: the forward's float32 [2,H,W] state and a float32 [1,H,W] (or [H,W])
+    cotangent on the rasterizer's device.  Raises ValueError otherwise."""
+    for name, t, shapes in (("distortion_state", distortion_state, ((2, H, W),)),
+                            ("dL_dout_distortion", dL_dout_distortion, ((1, H, W), (H, W)))):
+        if (not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or t.device != dev or
+                tuple(t.shape) not in shapes):
+            what = f"{t.dtype} {tuple(t.shape)} on {t.device}" if isinstance(t, torch.Tensor) else type(t).__name__
+            raise ValueError(f"{name} must be a torch.float32 tensor of shape {shapes[0]} on {dev}, got {what}")
+
+
 def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations, scale_modifier,
                         cov3Ds_precomp, norm3Ds_precomp, extra_attrs, attr_degree, viewmatrix, projmatrix,
                         tan_fovx, tan_fovy, kernel_size, image_height, image_width, sh, degree, campos,
                         prefiltered, debug, capacity_hint=0, tile_rows=None, fuse_normalize=False, out_planes=None,
-                        out_peers=None, subpixel_offset=None, graph=False, *, ortho=False, depth_quantile=None):
+                        out_peers=None, subpixel_offset=None, graph=False, *, ortho=False, depth_quantile=None,
+                        depth_distortion=False):
     """Same positional signature and return tuple as the reference's `_C.rasterize_gaussians`.  With
     `fuse_normalize=True` the returned normal map is already F.normalize(., dim=0) (the reference's torch post-op,
     diff_gauss/__init__.py:48) and the un-normalised blend is appended to the tuple for the backward.
@@ -155,9 +174,20 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
     crossing level q, the depth of the splat at which the pixel's accumulated opacity crosses q (q = 0.5: the median
     depth), or 0 where none does.  The tuple ends with (depth_q [1,H,W], depth_q_pos [H,W] int32); the backward takes
     depth_q_pos back.  It combines with `ortho` and offsets; graph, tile_rows, out_peers and extra_attrs raise SfgsError.
-    Every other output is bit-identical to the call without it."""
+    Every other output is bit-identical to the call without it.
+
+    `depth_distortion=True` (sfgs_rasterize_forward_distortion, include/sfgs.h): also the depth distortion
+    R = sum_{i<j} w_i w_j (m_i - m_j)^2 over the pixel's blended splats (w = alpha T, m the view depth), the distortion
+    loss of Mip-NeRF 360 / 2DGS, in units of depth^2.  The tuple ends with (distortion [1,H,W], distortion_state
+    [2,H,W]); the backward takes distortion_state back.  It combines with `ortho` and offsets; depth_quantile, graph,
+    tile_rows, out_peers and extra_attrs raise SfgsError.  Every other output is bit-identical to the call without it."""
     if means3D.ndim != 2 or means3D.shape[1] != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")
+    if depth_distortion:
+        _distortion_unsupported("rasterize_gaussians(depth_distortion=True)",
+                                depth_quantile=depth_quantile is not None, graph=graph,
+                                tile_rows=tile_rows is not None, out_peers=out_peers is not None,
+                                extra_attrs=int(attr_degree) > 0)
     if depth_quantile is not None:
         _depth_q_unsupported("rasterize_gaussians(depth_quantile=...)", graph=graph, tile_rows=tile_rows is not None,
                              out_peers=out_peers is not None, extra_attrs=int(attr_degree) > 0)
@@ -188,6 +218,8 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
             ret += (torch.zeros((3, H, W), **fopt),)
         if depth_quantile is not None:
             ret += (torch.zeros((1, H, W), **fopt), torch.zeros((H, W), dtype=torch.int32, device=dev))
+        if depth_distortion:
+            ret += (torch.zeros((1, H, W), **fopt), torch.zeros((2, H, W), **fopt))
         return ret
 
     with torch.cuda.device(dev):
@@ -254,6 +286,13 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
                                                                        float(depth_quantile), depth_q.data_ptr(),
                                                                        depth_q_pos.data_ptr()),
                                "sfgs_rasterize_forward_depth_quantile")
+        elif depth_distortion:
+            distortion = torch.empty((1, H, W), **fopt)
+            distortion_state = torch.empty((2, H, W), **fopt)
+            off = _ptr(subpixel_offset, keep) if subpixel_offset is not None else None
+            rendered = N.check(L.sfgs_rasterize_forward_distortion(C.byref(a), off, int(bool(ortho)),
+                                                                   distortion.data_ptr(), distortion_state.data_ptr()),
+                               "sfgs_rasterize_forward_distortion")
         elif graph:
             from . import graphs
             off = _ptr(subpixel_offset, keep) if subpixel_offset is not None else None
@@ -273,6 +312,8 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
            geom.tensor, binning.tensor, img.tensor)
     if fuse_normalize:
         ret += (norm_raw,)
+    if depth_distortion:
+        return ret + (distortion, distortion_state)
     return ret + (depth_q, depth_q_pos) if depth_quantile is not None else ret
 
 
@@ -313,7 +354,8 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
                                  out_alpha, debug, tile_rows=None, norm_raw=None, phase=0, acc=None,
                                  gauss_range=None, acc_peers=None, peer_slice=0, subpixel_offset=None,
                                  camera_grad=False, intrinsics_grad=False, graph=False, *, ortho=False,
-                                 depth_q_pos=None, dL_dout_depth_q=None):
+                                 depth_q_pos=None, dL_dout_depth_q=None, distortion_state=None,
+                                 dL_dout_distortion=None):
     """Same positional signature and return tuple as the reference's `_C.rasterize_gaussians_backward`.  With
     `norm_raw` (the extra tensor a `fuse_normalize=True` forward returned) `dL_dout_norm` is taken w.r.t. the unit
     normal map and the adjoint of F.normalize is applied inside the blend-adjoint kernel.
@@ -358,7 +400,20 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     `depth_q_pos` (the forward's, with `depth_quantile`) and `dL_dout_depth_q` ([1,H,W]): the backward of a depth
     quantile forward (sfgs_rasterize_backward_depth_quantile), which adds dL/d depth_q to the depth gradient of the
     splat each pixel selected.  It takes offsets, `ortho`, the deterministic mode, phase 1, and camera and focal
-    gradients (not with `ortho`); graph, tile_rows, acc_peers and extra_attrs raise SfgsError."""
+    gradients (not with `ortho`); graph, tile_rows, acc_peers and extra_attrs raise SfgsError.
+
+    `distortion_state` (the forward's, with `depth_distortion=True`) and `dL_dout_distortion` ([1,H,W]): the backward of
+    a depth-distortion forward (sfgs_rasterize_backward_distortion), which adds dL/dR to the blend adjoint's alpha and
+    depth terms.  It takes offsets, `ortho`, the deterministic mode, phase 1, and camera and focal gradients (not with
+    `ortho`); depth_q_pos, graph, tile_rows, acc_peers and extra_attrs raise SfgsError."""
+    dist = distortion_state is not None or dL_dout_distortion is not None
+    if dist:
+        if distortion_state is None or dL_dout_distortion is None:
+            raise ValueError("distortion_state and dL_dout_distortion come together")
+        _distortion_unsupported("rasterize_gaussians_backward(distortion_state=...)",
+                                depth_q_pos=depth_q_pos is not None or dL_dout_depth_q is not None, graph=graph,
+                                tile_rows=tile_rows is not None, acc_peers=acc_peers is not None,
+                                extra_attrs=extra_attrs is not None and extra_attrs.numel() != 0)
     depth_q = depth_q_pos is not None or dL_dout_depth_q is not None
     if depth_q:
         if depth_q_pos is None or dL_dout_depth_q is None:
@@ -380,6 +435,9 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     if depth_q:
         _check_depth_q(depth_q_pos, dL_dout_depth_q, int(dL_dout_color.shape[1]), int(dL_dout_color.shape[2]),
                        means3D.device)
+    if dist:
+        _check_distortion(distortion_state, dL_dout_distortion, int(dL_dout_color.shape[1]),
+                          int(dL_dout_color.shape[2]), means3D.device)
     F = int(extra_attrs.shape[1]) if (extra_attrs is not None and extra_attrs.numel() != 0) else 0
     deterministic = _use_deterministic(F > 0, acc_peers is not None)
     L = N.lib()
@@ -484,6 +542,15 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
                                                              _ptr(depth_q_pos, keep), _ptr(dL_dout_depth_q, keep),
                                                              dL_dcamera.data_ptr() if ncam else None, ncam),
                     "sfgs_rasterize_backward_depth_quantile")
+        elif dist:
+            ncam = (37 if intrinsics_grad else 35) if camera_grad else 0
+            dL_dcamera = torch.empty((ncam,), **fopt) if ncam else None
+            off = _ptr(subpixel_offset, keep) if subpixel_offset is not None else None
+            N.check(L.sfgs_rasterize_backward_distortion(C.byref(a), off, int(bool(ortho)), int(deterministic),
+                                                         _ptr(distortion_state, keep),
+                                                         _ptr(dL_dout_distortion, keep),
+                                                         dL_dcamera.data_ptr() if ncam else None, ncam),
+                    "sfgs_rasterize_backward_distortion")
         elif graph:
             ncam = (37 if intrinsics_grad else 35) if camera_grad else 0
             dL_dcamera = torch.empty((ncam,), **fopt) if ncam else None
