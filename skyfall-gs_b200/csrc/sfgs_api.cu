@@ -406,25 +406,38 @@ bool ortho_extent_ok(float sx, float sy) { return std::isfinite(sx) && std::isfi
 // the depth quantile's level q: finite, 0 < q < 1
 bool quantile_ok(float q) { return std::isfinite(q) && q > 0.f && q < 1.f; }
 
+// "<entry>: <subject> not supported with <feature>"
+int reject_with(const char* entry, const char* subject, const char* feature) {
+  char what[128];
+  snprintf(what, sizeof(what), "%s not supported with %s", subject, feature);
+  return fail_in(entry, SFGS_E_UNSUPPORTED, what);
+}
+
+// The forward's rejections of a per-pixel output (the depth quantile, the depth distortion), in order: null outputs,
+// the output's own bad argument `bad_arg` (or nullptr), then extra_attrs, tile-row bands and out_peers.
+int check_pixel_output(const sfgs_forward_args* a, const char* entry, bool null_out, const char* null_what,
+                       const char* bad_arg, const char* feature) {
+  if (null_out) return fail_in(entry, SFGS_E_BADARG, null_what);
+  if (bad_arg) return fail_in(entry, SFGS_E_BADARG, bad_arg);
+  if (a->ED > 0) return reject_with(entry, "extra_attrs are", feature);
+  if (a->tile_row_begin != 0 || a->tile_row_end != 0) return reject_with(entry, "tile-row bands are", feature);
+  if (a->out_peers != nullptr) return reject_with(entry, "out_peers are", feature);
+  return SFGS_OK;
+}
+
 int check_forward(const sfgs_forward_args* a, const FwdCall& c) {
   const auto reject = [&c](int code, const char* what) { return fail_in(c.name, code, what); };
   if (!a) return reject(SFGS_E_BADARG, "null args");
   if (c.depth_q) {
-    if (!c.out_depth_q || !c.out_depth_q_pos) return reject(SFGS_E_BADARG, "null out_depth_q or out_depth_q_pos");
-    if (!quantile_ok(c.quantile)) return reject(SFGS_E_BADARG, "the quantile must be finite with 0 < q < 1");
-    if (a->ED > 0) return reject(SFGS_E_UNSUPPORTED, "extra_attrs are not supported with the depth quantile");
-    if (a->tile_row_begin != 0 || a->tile_row_end != 0)
-      return reject(SFGS_E_UNSUPPORTED, "tile-row bands are not supported with the depth quantile");
-    if (a->out_peers != nullptr) return reject(SFGS_E_UNSUPPORTED, "out_peers are not supported with the depth quantile");
+    const char* bad_q = quantile_ok(c.quantile) ? nullptr : "the quantile must be finite with 0 < q < 1";
+    if (const int rc = check_pixel_output(a, c.name, !c.out_depth_q || !c.out_depth_q_pos,
+                                          "null out_depth_q or out_depth_q_pos", bad_q, "the depth quantile"))
+      return rc;
   }
   if (c.dist) {
-    if (!c.out_distortion || !c.out_distortion_state)
-      return reject(SFGS_E_BADARG, "null out_distortion or out_distortion_state");
-    if (a->ED > 0) return reject(SFGS_E_UNSUPPORTED, "extra_attrs are not supported with the depth distortion");
-    if (a->tile_row_begin != 0 || a->tile_row_end != 0)
-      return reject(SFGS_E_UNSUPPORTED, "tile-row bands are not supported with the depth distortion");
-    if (a->out_peers != nullptr)
-      return reject(SFGS_E_UNSUPPORTED, "out_peers are not supported with the depth distortion");
+    if (const int rc = check_pixel_output(a, c.name, !c.out_distortion || !c.out_distortion_state,
+                                          "null out_distortion or out_distortion_state", nullptr, "the depth distortion"))
+      return rc;
   }
   if (c.ortho) {
     if (a->tile_row_begin != 0 || a->tile_row_end != 0)
@@ -593,38 +606,37 @@ int rasterize_forward(const sfgs_forward_args* a, const FwdCall& c) {
   return (int)R;
 }
 
+// The backward's rejections of a per-pixel output's adjoint, in order: null inputs, ncam, extra_attrs, tile-row bands,
+// acc_peers, phase 2, and camera gradients with phase 1 or the orthographic camera.
+int check_pixel_output(const sfgs_backward_args* a, const BwdCall& c, bool null_in, const char* null_what,
+                       const char* feature) {
+  const auto reject = [&c](int code, const char* what) { return fail_in(c.name, code, what); };
+  if (null_in) return reject(SFGS_E_BADARG, null_what);
+  if (c.ncam != 0 && c.ncam != 35 && c.ncam != 37) return reject(SFGS_E_BADARG, "ncam must be 0, 35 or 37");
+  if (a->ED > 0) return reject_with(c.name, "extra_attrs are", feature);
+  if (a->tile_row_begin != 0 || a->tile_row_end != 0) return reject_with(c.name, "tile-row bands are", feature);
+  if (a->acc_peers != nullptr) return reject_with(c.name, "acc_peers are", feature);
+  if (a->phase == 2) return reject_with(c.name, "phase 2 is", feature);
+  if (c.ncam > 0 && a->phase == 1)
+    return reject(SFGS_E_UNSUPPORTED, "camera gradients are formed by the one-call backward (phase 0) only");
+  if (c.ncam > 0 && c.ortho) return reject(SFGS_E_UNSUPPORTED, "the orthographic camera has no camera gradients");
+  return SFGS_OK;
+}
+
 // Every rejection of the backward entries, in the order that decides which one an entry reports; all before any CUDA
 // work.  Messages are "<entry>: <what>".  P == 0 passes once the checks that hold for it have run.
 int check_backward(const sfgs_backward_args* a, const BwdCall& c) {
   const auto reject = [&c](int code, const char* what) { return fail_in(c.name, code, what); };
   if (!a) return reject(SFGS_E_BADARG, "null args");
   if (c.depth_q) {
-    if (!c.depth_q_pos || !c.dL_dpix_depth_q) return reject(SFGS_E_BADARG, "null depth_q_pos or dL_dpix_depth_q");
-    if (c.ncam != 0 && c.ncam != 35 && c.ncam != 37) return reject(SFGS_E_BADARG, "ncam must be 0, 35 or 37");
-    if (a->ED > 0) return reject(SFGS_E_UNSUPPORTED, "extra_attrs are not supported with the depth quantile");
-    if (a->tile_row_begin != 0 || a->tile_row_end != 0)
-      return reject(SFGS_E_UNSUPPORTED, "tile-row bands are not supported with the depth quantile");
-    if (a->acc_peers != nullptr) return reject(SFGS_E_UNSUPPORTED, "acc_peers are not supported with the depth quantile");
-    if (a->phase == 2) return reject(SFGS_E_UNSUPPORTED, "phase 2 is not supported with the depth quantile");
-    if (c.ncam > 0 && a->phase == 1)
-      return reject(SFGS_E_UNSUPPORTED, "camera gradients are formed by the one-call backward (phase 0) only");
-    if (c.ncam > 0 && c.ortho)
-      return reject(SFGS_E_UNSUPPORTED, "the orthographic camera has no camera gradients");
+    if (const int rc = check_pixel_output(a, c, !c.depth_q_pos || !c.dL_dpix_depth_q,
+                                          "null depth_q_pos or dL_dpix_depth_q", "the depth quantile"))
+      return rc;
   }
   if (c.dist) {
-    if (!c.distortion_state || !c.dL_dpix_distortion)
-      return reject(SFGS_E_BADARG, "null distortion_state or dL_dpix_distortion");
-    if (c.ncam != 0 && c.ncam != 35 && c.ncam != 37) return reject(SFGS_E_BADARG, "ncam must be 0, 35 or 37");
-    if (a->ED > 0) return reject(SFGS_E_UNSUPPORTED, "extra_attrs are not supported with the depth distortion");
-    if (a->tile_row_begin != 0 || a->tile_row_end != 0)
-      return reject(SFGS_E_UNSUPPORTED, "tile-row bands are not supported with the depth distortion");
-    if (a->acc_peers != nullptr)
-      return reject(SFGS_E_UNSUPPORTED, "acc_peers are not supported with the depth distortion");
-    if (a->phase == 2) return reject(SFGS_E_UNSUPPORTED, "phase 2 is not supported with the depth distortion");
-    if (c.ncam > 0 && a->phase == 1)
-      return reject(SFGS_E_UNSUPPORTED, "camera gradients are formed by the one-call backward (phase 0) only");
-    if (c.ncam > 0 && c.ortho)
-      return reject(SFGS_E_UNSUPPORTED, "the orthographic camera has no camera gradients");
+    if (const int rc = check_pixel_output(a, c, !c.distortion_state || !c.dL_dpix_distortion,
+                                          "null distortion_state or dL_dpix_distortion", "the depth distortion"))
+      return rc;
   }
   if (c.ortho) {
     if (a->phase != 0)

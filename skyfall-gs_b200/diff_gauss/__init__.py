@@ -100,156 +100,151 @@ def _with_offset(fn):
     return lambda *a, **kw: fn(*a[:-1], subpixel_offset=a[-1], **kw)
 
 
-def _requires_grad(x):
-    return isinstance(x, torch.Tensor) and x.requires_grad
+def _checked_inputs(shs, colors_precomp, scales, rotations, cov3Ds_precomp, norm3Ds_precomp, extra_attrs):
+    """The reference's four argument checks (RAST/diff_gauss/__init__.py:209-230), then the optional inputs with the
+    empty tensor the native layer takes for None: (shs, colors_precomp, cov3Ds_precomp, norm3Ds_precomp,
+    extra_attrs)."""
+    if (shs is None) == (colors_precomp is None):
+        raise Exception('Please provide excatly one of either SHs or precomputed colors!')
+    has_sr = scales is not None or rotations is not None
+    if ((scales is None or rotations is None) and cov3Ds_precomp is None) or (has_sr and cov3Ds_precomp is not None):
+        raise Exception('Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!')
+    if scales is None:
+        raise ValueError('To support norm and depth prediction, scales == None is not allowed')
+    if rotations is None:
+        raise ValueError('To support norm and depth prediction, rotations == None is not allowed')
+    return tuple(torch.Tensor([]) if t is None else t
+                 for t in (shs, colors_precomp, cov3Ds_precomp, norm3Ds_precomp, extra_attrs))
 
 
 class _RasterizeGaussians(torch.autograd.Function):
+    """The rasterizer for the pinhole camera (diff_gauss) and the orthographic one (sfgs.ortho).  Every input slot is
+    always passed: the callers resolve the options `fuse_normalize`, `depth_quantile` (q or None), `depth_distortion`,
+    `subpixel_offset` (a [H,W,2] tensor or None) and `ortho`.  With a quantile the outputs end with
+    (depth_q, depth_q_pos); with the distortion, with distortion."""
     # viewmatrix, projmatrix and campos are inputs of their own (the settings tuple is not tracked by autograd), so a
-    # camera built from parameters that require grad (scene/cameras.py: Camera(..., optimizing=True)) gets gradients.
+    # camera built from parameters that require grad (scene/cameras.py: Camera(..., optimizing=True)) gets gradients
     CAMERA_INPUTS = slice(12, 15)
-    # tanfovx and tanfovy likewise, passed only when one of them is a tensor that requires grad (focal refinement);
-    # otherwise the settings' values are used, as they always were
+    # tanfovx and tanfovy likewise: a 0-d tensor that requires grad gets dL/dtanfovx (focal refinement).  The native
+    # layer reads them with float(), which for a CUDA tensor is a host sync each forward and backward, so keep the
+    # leaves of a focal refinement on the CPU
     INTRINSICS_INPUTS = slice(15, 17)
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                norm3Ds_precomp, extra_attrs, raster_settings, fuse_normalize=False, viewmatrix=None, projmatrix=None,
-                campos=None, tanfovx=None, tanfovy=None, depth_quantile=None, depth_distortion=False):
+                norm3Ds_precomp, extra_attrs, raster_settings, fuse_normalize, viewmatrix, projmatrix, campos, tanfovx,
+                tanfovy, depth_quantile, depth_distortion, subpixel_offset=None, ortho=False):
         rs = raster_settings
-        ctx.depth_q = depth_quantile is not None
-        ctx.dist = bool(depth_distortion)
-        # the option inputs after the intrinsics slots: none, the quantile, or the quantile slot and the distortion flag
-        ctx.n_options = 2 if ctx.dist else int(ctx.depth_q)
-        ctx.intrinsics = None if tanfovx is None else (tanfovx, tanfovy)
-        viewmatrix = rs.viewmatrix if viewmatrix is None else viewmatrix
-        projmatrix = rs.projmatrix if projmatrix is None else projmatrix
-        campos = rs.campos if campos is None else campos
+        ctx.depth_q, ctx.dist = depth_quantile is not None, bool(depth_distortion)
         n_extra = extra_attrs.shape[1] if extra_attrs.shape[0] != 0 else 0
         assert n_extra <= MAX_EXTRA_DIMS
-        native_args = (rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier,
-                       cov3Ds_precomp, norm3Ds_precomp, extra_attrs, n_extra, viewmatrix, projmatrix,
-                       rs.tanfovx, rs.tanfovy, rs.kernel_size, rs.image_height, rs.image_width, sh, rs.sh_degree,
-                       campos, rs.prefiltered, rs.debug)
-        ctx.fused = bool(fuse_normalize)
-        off = _subpixel_offset(rs)
-        fwd = _C.rasterize_gaussians_fused if ctx.fused else _C.rasterize_gaussians
         # under stream capture (torch.cuda.graph) the capture-safe entries run: no host wait, intrinsics that are 0-d
         # CUDA tensors read at replay time, a capacity fixed at capture (sfgs.graphs)
         ctx.graph = means3D.is_cuda and torch.cuda.is_current_stream_capturing()
         capacity = 0
+        opts = {}
         if ctx.graph:
-            if ctx.depth_q:
-                raise _C.SfgsError("diff_gauss: the depth quantile cannot be captured in a CUDA graph")
-            if ctx.dist:
-                raise _C.SfgsError("diff_gauss: the depth distortion cannot be captured in a CUDA graph")
+            for on, what in ((ctx.depth_q, "the depth quantile"), (ctx.dist, "the depth distortion"),
+                             (ortho, "the orthographic camera")):
+                if on:
+                    raise _C.SfgsError(f"diff_gauss: {what} cannot be captured in a CUDA graph")
             if rs.debug:
                 raise _C.SfgsError("diff_gauss: debug=True synchronises after every stage and cannot be captured in a "
                                    "CUDA graph")
             P = int(means3D.shape[0])
             capacity = _graphs.resolve_capacity(means3D.device, P, rs.image_width, rs.image_height) if P > 0 else 1
-            fwd = functools.partial(fwd, capacity_hint=capacity, graph=True)
+            opts.update(capacity_hint=capacity, graph=True)
+        if ortho:
+            opts["ortho"] = True
         if ctx.depth_q:
-            fwd = functools.partial(fwd, depth_quantile=depth_quantile)
+            opts["depth_quantile"] = depth_quantile
         if ctx.dist:
-            fwd = functools.partial(fwd, depth_distortion=True)
-        if off is not None:
+            opts["depth_distortion"] = True
+        native_args = (rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier,
+                       cov3Ds_precomp, norm3Ds_precomp, extra_attrs, n_extra, viewmatrix, projmatrix,
+                       tanfovx, tanfovy, rs.kernel_size, rs.image_height, rs.image_width, sh, rs.sh_degree,
+                       campos, rs.prefiltered, rs.debug)
+        ctx.fused = bool(fuse_normalize)
+        fwd = functools.partial(_C.rasterize_gaussians_fused if ctx.fused else _C.rasterize_gaussians, **opts)
+        if subpixel_offset is not None:
             # the offsets travel as the last argument, so that the debug snapshot holds them too
-            fwd, native_args = _with_offset(fwd), native_args + (off,)
+            fwd, native_args = _with_offset(fwd), native_args + (subpixel_offset,)
         out = _guarded(fwd, native_args, rs.debug, "snapshot_fw.dump", "forward")
+        (num_rendered, color, depth, norm, alpha, radii, extra, geom_buf, binning_buf, img_buf) = out[:10]
+        norm_raw = out[10] if ctx.fused else torch.empty(0, device=means3D.device)
         # the 7th output and the state its backward reads: (depth_q, depth_q_pos) or (distortion, distortion_state)
-        side, side_state = out[-2:] if ctx.n_options else (None, torch.empty(0, device=means3D.device))
-        if ctx.fused:
-            (num_rendered, color, depth, norm, alpha, radii, extra, geom_buf, binning_buf, img_buf,
-             norm_raw) = out[:11]
-        else:
-            (num_rendered, color, depth, norm, alpha, radii, extra,
-             geom_buf, binning_buf, img_buf) = out[:10]
-            norm_raw = torch.empty(0, device=means3D.device)
-        ctx.subpixel_offset = off
-        ctx.raster_settings = rs
-        ctx.camera = (viewmatrix, projmatrix, campos)
+        side, side_state = out[-2:] if ctx.depth_q or ctx.dist else (None, torch.empty(0, device=means3D.device))
+        ctx.raster_settings, ctx.subpixel_offset, ctx.ortho = rs, subpixel_offset, bool(ortho)
+        ctx.camera, ctx.intrinsics = (viewmatrix, projmatrix, campos), (tanfovx, tanfovy)
         # the graph backward is given the capacity in place of num_rendered (not known on the host under capture)
         ctx.num_rendered = capacity if ctx.graph else num_rendered
         ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, norm3Ds_precomp, radii,
                               extra_attrs, sh, geom_buf, binning_buf, img_buf, alpha, norm_raw, side_state)
         ctx.mark_non_differentiable(radii)
-        if ctx.n_options:
-            return color, depth, norm, alpha, radii, extra, side
-        return color, depth, norm, alpha, radii, extra
+        if ctx.depth_q:
+            # depth_q_pos: which splat each pixel selected (0: none), for render_height_map's mask
+            ctx.mark_non_differentiable(radii, side_state)
+            return color, depth, norm, alpha, radii, extra, side, side_state
+        return (color, depth, norm, alpha, radii, extra) + ((side,) if ctx.dist else ())
 
     @staticmethod
-    def backward(ctx, g_color, g_depth, g_norm, g_alpha, _g_radii, g_extra, g_side=None):
+    def backward(ctx, g_color, g_depth, g_norm, g_alpha, _g_radii, g_extra, g_side=None, _g_depth_q_pos=None):
         rs = ctx.raster_settings
         (colors_precomp, means3D, scales, rotations, cov3Ds_precomp, norm3Ds_precomp, radii, extra_attrs, sh,
          geom_buf, binning_buf, img_buf, alpha, norm_raw, side_state) = ctx.saved_tensors
         viewmatrix, projmatrix, campos = ctx.camera
         native_args = (rs.bg, means3D, radii, colors_precomp, scales, rotations, extra_attrs, rs.scale_modifier,
-                       cov3Ds_precomp, norm3Ds_precomp, viewmatrix, projmatrix, rs.tanfovx, rs.tanfovy,
+                       cov3Ds_precomp, norm3Ds_precomp, viewmatrix, projmatrix, *ctx.intrinsics,
                        rs.kernel_size, g_color, g_depth, g_norm, g_alpha, g_extra, sh, rs.sh_degree, campos,
                        geom_buf, ctx.num_rendered, binning_buf, img_buf, alpha, rs.debug)
-        bwd = _C.rasterize_gaussians_backward
-        if ctx.fused:
-            bwd = lambda *a, **kw: _C.rasterize_gaussians_backward_fused(*a, norm_raw=norm_raw, **kw)  # noqa: E731
-        camera_grad = any(ctx.needs_input_grad[_RasterizeGaussians.CAMERA_INPUTS])
-        intrinsics_grad = ctx.intrinsics is not None and any(
-            ctx.needs_input_grad[_RasterizeGaussians.INTRINSICS_INPUTS])
-        if intrinsics_grad:
-            # the focal-length gradients come with the camera gradients, from one native call
-            bwd = functools.partial(bwd, camera_grad=True, intrinsics_grad=True)
-        elif camera_grad:
-            # only when asked for: a camera without requires_grad keeps the default native call
-            bwd = functools.partial(bwd, camera_grad=True)
+        need_camera = ctx.needs_input_grad[_RasterizeGaussians.CAMERA_INPUTS]
+        need_intrinsics = ctx.needs_input_grad[_RasterizeGaussians.INTRINSICS_INPUTS]
+        opts = dict(norm_raw=norm_raw) if ctx.fused else {}
+        # only when asked for: a camera without requires_grad keeps the default native call, and the focal-length
+        # gradients come with the camera gradients, from one native call
+        if any(need_intrinsics):
+            opts.update(camera_grad=True, intrinsics_grad=True)
+        elif any(need_camera):
+            opts.update(camera_grad=True)
         if ctx.graph:
-            bwd = functools.partial(bwd, graph=True)
+            opts["graph"] = True
+        if ctx.ortho:
+            opts["ortho"] = True
         if ctx.depth_q:
-            bwd = functools.partial(bwd, depth_q_pos=side_state, dL_dout_depth_q=g_side.contiguous())
+            opts.update(depth_q_pos=side_state, dL_dout_depth_q=g_side.contiguous())
         if ctx.dist:
-            bwd = functools.partial(bwd, distortion_state=side_state, dL_dout_distortion=g_side.contiguous())
+            opts.update(distortion_state=side_state, dL_dout_distortion=g_side.contiguous())
+        bwd = functools.partial(_C.rasterize_gaussians_backward_fused if ctx.fused else
+                                _C.rasterize_gaussians_backward, **opts)
         if ctx.subpixel_offset is not None:
             bwd, native_args = _with_offset(bwd), native_args + (ctx.subpixel_offset,)
         grads = _guarded(bwd, native_args, rs.debug, "snapshot_bw.dump", "backward")
+
+        def cast(gs, inputs, need):
+            return tuple(g.to(dtype=t.dtype, device=t.device) if n else None for g, t, n in zip(gs, inputs, need))
+        g_camera = cast(grads[10:13], ctx.camera, need_camera) if opts.get("camera_grad") else (None,) * 3
+        g_intrinsics = cast(grads[13:15], ctx.intrinsics, need_intrinsics) if any(need_intrinsics) else (None,) * 2
         (g_means2D, g_colors, g_opac, g_means3D, g_cov3D, g_norm3D, g_sh, g_scales, g_rot, g_extra_attrs) = grads[:10]
-        g_camera = (None, None, None)
-        if camera_grad or intrinsics_grad:
-            g_camera = tuple(g.to(dtype=t.dtype, device=t.device) if need else None for g, t, need in
-                             zip(grads[10:13], ctx.camera, ctx.needs_input_grad[_RasterizeGaussians.CAMERA_INPUTS]))
-        g_intrinsics = ()
-        if ctx.intrinsics is not None or ctx.n_options:
-            g_intrinsics = (None, None)
-            if intrinsics_grad:
-                g_intrinsics = tuple(
-                    g.to(dtype=t.dtype, device=t.device) if need else None for g, t, need in
-                    zip(grads[13:15], ctx.intrinsics, ctx.needs_input_grad[_RasterizeGaussians.INTRINSICS_INPUTS]))
-        # order of forward's inputs; the settings tuple, the fusion flag and the options get no gradient
-        return (g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rot, g_cov3D, g_norm3D, g_extra_attrs,
-                None, None) + g_camera + g_intrinsics + (None,) * ctx.n_options
+        # order of forward's inputs; the settings tuple and the options get no gradient
+        return ((g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rot, g_cov3D, g_norm3D, g_extra_attrs)
+                + (None, None) + g_camera + g_intrinsics + (None,) * 4)
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                         norm3Ds_precomp, extra_attrs, raster_settings, depth_quantile=None, depth_distortion=False):
     rs = raster_settings
-    # tanfovx / tanfovy may be 0-d tensors; the native layer reads them with float(), which for a CUDA tensor is a
-    # host sync each forward and backward, so keep the leaves of a focal refinement on the CPU
-    intrinsics = (rs.tanfovx, rs.tanfovy) if _requires_grad(rs.tanfovx) or _requires_grad(rs.tanfovy) else ()
     if depth_distortion and depth_quantile is not None:
         raise _C.SfgsError("diff_gauss: depth_distortion and depth_quantile in one call are not supported; render "
                            "them in two calls")
-    # the quantile, then the distortion flag, follow the two intrinsics slots (None: the settings' values)
-    options = ()
-    if depth_distortion:
-        options = (intrinsics or (None, None)) + (None, True)
-    elif depth_quantile is not None:
-        options = (intrinsics or (None, None)) + (float(depth_quantile),)
     out = _RasterizeGaussians.apply(
         means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, norm3Ds_precomp,
-        extra_attrs, raster_settings, FUSE_NORMALIZE, rs.viewmatrix, rs.projmatrix, rs.campos,
-        *(options or intrinsics))
+        extra_attrs, rs, FUSE_NORMALIZE, rs.viewmatrix, rs.projmatrix, rs.campos, rs.tanfovx, rs.tanfovy,
+        None if depth_quantile is None else float(depth_quantile), bool(depth_distortion), _subpixel_offset(rs), False)
     color, depth, norm, alpha, radii, extra = out[:6]
     if not FUSE_NORMALIZE:
         # the reference normalises the blended normal map in torch, inside the autograd graph (diff_gauss/__init__.py:48)
         norm = torch.nn.functional.normalize(norm, p=2, dim=0)
-    return (color, depth, norm, alpha, radii, extra) + tuple(out[6:])
+    return (color, depth, norm, alpha, radii, extra) + tuple(out[6:7])
 
 
 class GaussianRasterizer(nn.Module):
@@ -272,20 +267,8 @@ class GaussianRasterizer(nn.Module):
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
                 cov3Ds_precomp=None, norm3Ds_precomp=None, extra_attrs=None):
-        if (shs is None) == (colors_precomp is None):
-            raise Exception('Please provide excatly one of either SHs or precomputed colors!')
-        has_sr = scales is not None or rotations is not None
-        if ((scales is None or rotations is None) and cov3Ds_precomp is None) or (has_sr and cov3Ds_precomp is not None):
-            raise Exception('Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!')
-        if scales is None:
-            raise ValueError('To support norm and depth prediction, scales == None is not allowed')
-        if rotations is None:
-            raise ValueError('To support norm and depth prediction, rotations == None is not allowed')
-
-        def _or_empty(t):
-            return torch.Tensor([]) if t is None else t
-
-        return rasterize_gaussians(means3D, means2D, _or_empty(shs), _or_empty(colors_precomp), opacities, scales,
-                                   rotations, _or_empty(cov3Ds_precomp), _or_empty(norm3Ds_precomp),
-                                   _or_empty(extra_attrs), self.raster_settings, self.depth_quantile,
+        shs, colors_precomp, cov3Ds_precomp, norm3Ds_precomp, extra_attrs = _checked_inputs(
+            shs, colors_precomp, scales, rotations, cov3Ds_precomp, norm3Ds_precomp, extra_attrs)
+        return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                                   norm3Ds_precomp, extra_attrs, self.raster_settings, self.depth_quantile,
                                    self.depth_distortion)

@@ -20,6 +20,8 @@ from typing import NamedTuple, Optional
 import torch
 import torch.nn as nn
 
+import diff_gauss
+
 from . import native as N
 from . import rasterizer as R
 
@@ -92,64 +94,6 @@ def nadir_camera(xmin, xmax, ymin, ymax, resolution, z_top):
     return NadirCamera(H, W, s_x, s_y, view, proj, float(z_top), float(xmin), float(ymax), r)
 
 
-def _requires_grad(x):
-    return isinstance(x, torch.Tensor) and x.requires_grad
-
-
-class _RasterizeOrtho(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                norm3Ds_precomp, extra_attrs, rs, depth_quantile=None, depth_distortion=False):
-        ctx.depth_q = depth_quantile is not None
-        ctx.dist = bool(depth_distortion)
-        ctx.n_options = 2 if ctx.dist else int(ctx.depth_q)
-        n_extra = extra_attrs.shape[1] if extra_attrs.shape[0] != 0 else 0
-        dev = means3D.device
-        campos = torch.zeros(3, dtype=torch.float32, device=dev)      # not read by the orthographic camera
-        off = rs.subpixel_offset
-        out = R.rasterize_gaussians(
-            rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier, cov3Ds_precomp,
-            norm3Ds_precomp, extra_attrs, n_extra, rs.viewmatrix, rs.projmatrix, rs.half_width, rs.half_height,
-            rs.kernel_size, rs.image_height, rs.image_width, sh, rs.sh_degree, campos, rs.prefiltered, rs.debug,
-            fuse_normalize=True, subpixel_offset=off, ortho=True, depth_quantile=depth_quantile,
-            depth_distortion=ctx.dist)
-        (num_rendered, color, depth, norm, alpha, radii, extra, geom_buf, binning_buf, img_buf, norm_raw) = out[:11]
-        # the 7th output and the state its backward reads: (depth_q, depth_q_pos) or (distortion, distortion_state)
-        side, side_state = out[11:] if ctx.n_options else (None, torch.empty(0, device=dev))
-        ctx.rs, ctx.campos, ctx.num_rendered = rs, campos, num_rendered
-        ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, norm3Ds_precomp, radii,
-                              extra_attrs, sh, geom_buf, binning_buf, img_buf, alpha, norm_raw, side_state)
-        ctx.mark_non_differentiable(radii)
-        if ctx.depth_q:
-            # depth_q_pos: which splat each pixel selected (0: none), for render_height_map's mask
-            ctx.mark_non_differentiable(radii, side_state)
-            return color, depth, norm, alpha, radii, extra, side, side_state
-        if ctx.dist:
-            return color, depth, norm, alpha, radii, extra, side
-        return color, depth, norm, alpha, radii, extra
-
-    @staticmethod
-    def backward(ctx, g_color, g_depth, g_norm, g_alpha, _g_radii, g_extra, g_side=None, _g_depth_q_pos=None):
-        rs = ctx.rs
-        (colors_precomp, means3D, scales, rotations, cov3Ds_precomp, norm3Ds_precomp, radii, extra_attrs, sh,
-         geom_buf, binning_buf, img_buf, alpha, norm_raw, side_state) = ctx.saved_tensors
-        side = {}
-        if ctx.depth_q:
-            side = dict(depth_q_pos=side_state, dL_dout_depth_q=g_side.contiguous())
-        if ctx.dist:
-            side = dict(distortion_state=side_state, dL_dout_distortion=g_side.contiguous())
-        # deterministic under torch.use_deterministic_algorithms(True), as for the perspective backward
-        grads = R.rasterize_gaussians_backward(
-            rs.bg, means3D, radii, colors_precomp, scales, rotations, extra_attrs, rs.scale_modifier, cov3Ds_precomp,
-            norm3Ds_precomp, rs.viewmatrix, rs.projmatrix, rs.half_width, rs.half_height, rs.kernel_size,
-            g_color.contiguous(), g_depth.contiguous(), g_norm.contiguous(), g_alpha.contiguous(),
-            g_extra.contiguous(), sh, rs.sh_degree, ctx.campos, geom_buf, ctx.num_rendered, binning_buf, img_buf,
-            alpha, rs.debug, norm_raw=norm_raw, subpixel_offset=rs.subpixel_offset, ortho=True, **side)
-        (g_means2D, g_colors, g_opac, g_means3D, g_cov3D, g_norm3D, g_sh, g_scales, g_rot, g_extra_attrs) = grads
-        return ((g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rot, g_cov3D, g_norm3D, g_extra_attrs, None)
-                + (None,) * ctx.n_options)
-
-
 class OrthoRasterizer(nn.Module):
     """diff_gauss.GaussianRasterizer for an orthographic camera: same call, same checks, same returned
     (color [3,H,W], depth [1,H,W], unit normal [3,H,W], alpha [1,H,W], radii [P], extra [F,H,W] | empty).  `means2D`'s
@@ -174,32 +118,28 @@ class OrthoRasterizer(nn.Module):
                    cov3Ds_precomp=None, norm3Ds_precomp=None, extra_attrs=None):
         """forward()'s checks and call; with a quantile the tuple also ends with depth_q_pos [H,W]."""
         rs = self.raster_settings
-        if (shs is None) == (colors_precomp is None):
-            raise Exception('Please provide excatly one of either SHs or precomputed colors!')
-        has_sr = scales is not None or rotations is not None
-        if ((scales is None or rotations is None) and cov3Ds_precomp is None) or (has_sr and cov3Ds_precomp is not None):
-            raise Exception('Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!')
-        if scales is None:
-            raise ValueError('To support norm and depth prediction, scales == None is not allowed')
-        if rotations is None:
-            raise ValueError('To support norm and depth prediction, rotations == None is not allowed')
-        if _requires_grad(rs.viewmatrix) or _requires_grad(rs.projmatrix):
+        shs, colors_precomp, cov3Ds_precomp, norm3Ds_precomp, extra_attrs = diff_gauss._checked_inputs(
+            shs, colors_precomp, scales, rotations, cov3Ds_precomp, norm3Ds_precomp, extra_attrs)
+        if any(isinstance(m, torch.Tensor) and m.requires_grad for m in (rs.viewmatrix, rs.projmatrix)):
             raise ValueError("OrthoRasterizer forms no camera gradients: viewmatrix and projmatrix must not require "
                              "grad (detach them)")
         if rs.subpixel_offset is not None:
             R.check_subpixel_offset(rs.subpixel_offset, int(rs.image_height), int(rs.image_width))
         if self.depth_distortion and self.depth_quantile is not None:
             raise N.SfgsError("OrthoRasterizer: depth_distortion and depth_quantile in one call are not supported; "
-                                "render them in two calls")
-
-        def _or_empty(t):
-            return torch.Tensor([]) if t is None else t
-
-        return _RasterizeOrtho.apply(means3D, means2D, _or_empty(shs), _or_empty(colors_precomp), opacities, scales,
-                                     rotations, _or_empty(cov3Ds_precomp), _or_empty(norm3Ds_precomp),
-                                     _or_empty(extra_attrs), rs,
-                                     *((None, True) if self.depth_distortion else
-                                       () if self.depth_quantile is None else (float(self.depth_quantile),)))
+                              "render them in two calls")
+        # the half-extents travel in the tan_fov fields (as numbers: they get no gradient), and campos is not read
+        s_x, s_y = float(rs.half_width), float(rs.half_height)
+        campos = torch.zeros(3, dtype=torch.float32, device=means3D.device)
+        settings = diff_gauss.GaussianRasterizationSettings(
+            rs.image_height, rs.image_width, s_x, s_y, rs.kernel_size, rs.subpixel_offset, rs.bg, rs.scale_modifier,
+            rs.viewmatrix, rs.projmatrix, rs.sh_degree, campos, rs.prefiltered, rs.debug)
+        # deterministic under torch.use_deterministic_algorithms(True), as for the perspective backward
+        return diff_gauss._RasterizeGaussians.apply(
+            means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, norm3Ds_precomp,
+            extra_attrs, settings, True, rs.viewmatrix, rs.projmatrix, campos, s_x, s_y,
+            None if self.depth_quantile is None else float(self.depth_quantile), bool(self.depth_distortion),
+            rs.subpixel_offset, True)
 
 
 def render_height_map(camera: NadirCamera, means3D, opacities, scales, rotations, shs=None, colors_precomp=None,

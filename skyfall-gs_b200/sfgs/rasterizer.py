@@ -90,58 +90,35 @@ def _tan_fov(tan_fovx, tan_fovy, dev):
     return 1.0, 1.0, torch.stack(parts)
 
 
-def _graph_unsupported(where, debug, tile_rows=None, peers=None, phase=0):
-    """The options a captured call cannot take, as a readable error raised before any work is queued."""
-    what = (["debug=True (it synchronises after every stage)"] * bool(debug) +
-            ["tile_rows"] * (tile_rows is not None) + [peers] * (peers is not None) +
-            [f"phase={phase} (the two-phase backward)"] * (phase != 0))
-    if what:
-        raise N.SfgsError(f"{where}: {', '.join(what)} cannot be captured in a CUDA graph")
+GRAPH = "cannot be captured in a CUDA graph"
+ORTHO = "not supported with an orthographic camera"
+DEPTH_Q = "not supported with the depth quantile"
+DISTORTION = "not supported with the depth distortion"
 
 
-def _ortho_unsupported(where, **opts):
-    """The options an orthographic call cannot take (truthy values of `opts`), as an error raised before any native
-    call."""
+def _reject(where, tail, **opts):
+    """The options of `opts` that are set (truthy values, in order) as one SfgsError, raised before any native call:
+    "<where>: <names> <tail>"."""
     what = [k for k, v in opts.items() if v]
     if what:
-        raise N.SfgsError(f"{where}: {', '.join(what)} not supported with an orthographic camera")
+        raise N.SfgsError(f"{where}: {', '.join(what)} {tail}")
 
 
-def _unsupported_with(feature, where, **opts):
-    """The options `feature` cannot take (truthy values of `opts`), as an error raised before any native call."""
-    what = [k for k, v in opts.items() if v]
-    if what:
-        raise N.SfgsError(f"{where}: {', '.join(what)} not supported with {feature}")
+def _given_together(a_name, a, b_name, b):
+    """Whether the pair of a per-pixel output's backward inputs is given; one without the other raises ValueError."""
+    if (a is None) != (b is None):
+        raise ValueError(f"{a_name} and {b_name} come together")
+    return a is not None
 
 
-def _depth_q_unsupported(where, **opts):
-    _unsupported_with("the depth quantile", where, **opts)
-
-
-def _distortion_unsupported(where, **opts):
-    _unsupported_with("the depth distortion", where, **opts)
-
-
-def _check_depth_q(depth_q_pos, dL_dout_depth_q, H, W, dev):
-    """The depth quantile's backward inputs: the forward's int32 [H,W] positions and a float32 [1,H,W] (or [H,W])
-    cotangent on the rasterizer's device.  Raises ValueError otherwise."""
-    for name, t, dtype, shapes in (("depth_q_pos", depth_q_pos, torch.int32, ((H, W),)),
-                                   ("dL_dout_depth_q", dL_dout_depth_q, torch.float32, ((1, H, W), (H, W)))):
-        if (not isinstance(t, torch.Tensor) or t.dtype != dtype or t.device != dev or
-                tuple(t.shape) not in shapes):
+def _check_pixel_inputs(state_name, state, dtype, shape, cot_name, cot, H, W, dev):
+    """A per-pixel output's backward inputs: the forward's `state` (`dtype`, `shape`) and a float32 [1,H,W] (or [H,W])
+    cotangent `cot`, on the rasterizer's device.  Raises ValueError otherwise."""
+    for name, t, dt, shapes in ((state_name, state, dtype, (shape,)),
+                                (cot_name, cot, torch.float32, ((1, H, W), (H, W)))):
+        if not isinstance(t, torch.Tensor) or t.dtype != dt or t.device != dev or tuple(t.shape) not in shapes:
             what = f"{t.dtype} {tuple(t.shape)} on {t.device}" if isinstance(t, torch.Tensor) else type(t).__name__
-            raise ValueError(f"{name} must be a {dtype} tensor of shape {shapes[0]} on {dev}, got {what}")
-
-
-def _check_distortion(distortion_state, dL_dout_distortion, H, W, dev):
-    """The depth distortion's backward inputs: the forward's float32 [2,H,W] state and a float32 [1,H,W] (or [H,W])
-    cotangent on the rasterizer's device.  Raises ValueError otherwise."""
-    for name, t, shapes in (("distortion_state", distortion_state, ((2, H, W),)),
-                            ("dL_dout_distortion", dL_dout_distortion, ((1, H, W), (H, W)))):
-        if (not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or t.device != dev or
-                tuple(t.shape) not in shapes):
-            what = f"{t.dtype} {tuple(t.shape)} on {t.device}" if isinstance(t, torch.Tensor) else type(t).__name__
-            raise ValueError(f"{name} must be a torch.float32 tensor of shape {shapes[0]} on {dev}, got {what}")
+            raise ValueError(f"{name} must be a {dt} tensor of shape {shapes[0]} on {dev}, got {what}")
 
 
 def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations, scale_modifier,
@@ -183,20 +160,18 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
     tile_rows, out_peers and extra_attrs raise SfgsError.  Every other output is bit-identical to the call without it."""
     if means3D.ndim != 2 or means3D.shape[1] != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")
+    banded = dict(tile_rows=tile_rows is not None, out_peers=out_peers is not None)
     if depth_distortion:
-        _distortion_unsupported("rasterize_gaussians(depth_distortion=True)",
-                                depth_quantile=depth_quantile is not None, graph=graph,
-                                tile_rows=tile_rows is not None, out_peers=out_peers is not None,
-                                extra_attrs=int(attr_degree) > 0)
+        _reject("rasterize_gaussians(depth_distortion=True)", DISTORTION, depth_quantile=depth_quantile is not None,
+                graph=graph, **banded, extra_attrs=int(attr_degree) > 0)
     if depth_quantile is not None:
-        _depth_q_unsupported("rasterize_gaussians(depth_quantile=...)", graph=graph, tile_rows=tile_rows is not None,
-                             out_peers=out_peers is not None, extra_attrs=int(attr_degree) > 0)
+        _reject("rasterize_gaussians(depth_quantile=...)", DEPTH_Q, graph=graph, **banded,
+                extra_attrs=int(attr_degree) > 0)
     if ortho:
-        _ortho_unsupported("rasterize_gaussians(ortho=True)", graph=graph, tile_rows=tile_rows is not None,
-                           out_peers=out_peers is not None)
+        _reject("rasterize_gaussians(ortho=True)", ORTHO, graph=graph, **banded)
     if graph:
-        _graph_unsupported("rasterize_gaussians(graph=True)", debug, tile_rows,
-                           "out_peers" if out_peers is not None else None)
+        _reject("rasterize_gaussians(graph=True)", GRAPH, **{"debug=True (it synchronises after every stage)": debug},
+                **banded)
         if int(capacity_hint) <= 0:
             raise N.SfgsError("rasterize_gaussians(graph=True) needs capacity_hint > 0 (see sfgs.graphs.capacity)")
     H, W, F = int(image_height), int(image_width), int(attr_degree)
@@ -206,115 +181,96 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
     P = int(means3D.shape[0])
     dev = means3D.device
     fopt = dict(dtype=torch.float32, device=dev)
+    alloc = torch.zeros if P == 0 else torch.empty      # the reference returns zero images for P == 0
+    # one allocation for the 8 image planes: colour(3) depth(1) alpha(1) normal(3)
+    # multi-GPU tile-row mode: `out_planes` is this rank's symmetric [8,H,W] frame block and `out_peers` the
+    # peer-mapped pointers of every rank's block; the blend kernel then stores the band into all of them
+    if out_planes is not None and P > 0:
+        planes = out_planes.view(8, H, W)
+        norm_raw = torch.empty((3, H, W), **fopt) if fuse_normalize else None
+    else:
+        planes = alloc((11 if fuse_normalize else 8, H, W), **fopt)
+        norm_raw = planes[8:11] if fuse_normalize else None
+    out_color, out_depth, out_alpha, out_norm = planes[0:3], planes[3:4], planes[4:5], planes[5:8]
+    radii = alloc((P,), dtype=torch.int32, device=dev)
+    out_extra = alloc((F, H, W), **fopt) if F > 0 else torch.empty(0, **fopt)
+    # the per-pixel output and the state its backward reads
+    side = ()
+    if depth_quantile is not None:
+        side = (alloc((1, H, W), **fopt), alloc((H, W), dtype=torch.int32, device=dev))     # depth_q, depth_q_pos
+    elif depth_distortion:
+        side = (alloc((1, H, W), **fopt), alloc((2, H, W), **fopt))     # distortion, distortion_state
 
     if P == 0:
         # the reference short-circuits: zero images, empty scratch (rasterize_points.cu:94)
-        out_extra = torch.zeros((F, H, W), **fopt) if F > 0 else torch.empty(0, **fopt)
         empty = torch.empty(0, dtype=torch.uint8, device=dev)
-        ret = (0, torch.zeros((NUM_CHANNELS, H, W), **fopt), torch.zeros((1, H, W), **fopt),
-               torch.zeros((3, H, W), **fopt), torch.zeros((1, H, W), **fopt),
-               torch.zeros((P,), dtype=torch.int32, device=dev), out_extra, empty, empty.clone(), empty.clone())
-        if fuse_normalize:
-            ret += (torch.zeros((3, H, W), **fopt),)
-        if depth_quantile is not None:
-            ret += (torch.zeros((1, H, W), **fopt), torch.zeros((H, W), dtype=torch.int32, device=dev))
-        if depth_distortion:
-            ret += (torch.zeros((1, H, W), **fopt), torch.zeros((2, H, W), **fopt))
-        return ret
-
-    with torch.cuda.device(dev):
-        # one allocation for the 8 image planes: colour(3) depth(1) alpha(1) normal(3)
-        # multi-GPU tile-row mode: `out_planes` is this rank's symmetric [8,H,W] frame block and `out_peers` the
-        # peer-mapped pointers of every rank's block; the blend kernel then stores the band into all of them
-        if out_planes is not None:
-            planes = out_planes.view(8, H, W)
-            norm_raw = torch.empty((3, H, W), **fopt) if fuse_normalize else None
-        else:
-            planes = torch.empty((11 if fuse_normalize else 8, H, W), **fopt)
-            norm_raw = planes[8:11] if fuse_normalize else None
-        out_color, out_depth, out_alpha, out_norm = planes[0:3], planes[3:4], planes[4:5], planes[5:8]
-        radii = torch.empty((P,), dtype=torch.int32, device=dev)
-        out_extra = torch.empty((F, H, W), **fopt) if F > 0 else torch.empty(0, **fopt)
-
-        geom, binning, img = _Arena(dev), _Arena(dev), _Arena(dev)
-        keep = []
-        M = int(sh.shape[1]) if (sh is not None and sh.numel() != 0) else 0
-        a = N.ForwardArgs()
-        a.geom_alloc, a.binning_alloc, a.image_alloc = geom.cb, binning.cb, img.cb
-        a.P, a.D, a.M, a.ED = P, int(degree), M, F
-        a.width, a.height = W, H
-        a.background = _ptr(background, keep)
-        a.means3D = _ptr(means3D, keep)
-        a.shs = _ptr(sh, keep)
-        a.colors_precomp = _ptr(colors, keep)
-        a.opacities = _ptr(opacity, keep)
-        a.scales = _ptr(scales, keep)
-        a.scale_modifier = float(scale_modifier)
-        a.rotations = _ptr(rotations, keep)
-        a.cov3D_precomp = _ptr(cov3Ds_precomp, keep)
-        a.norm3D_precomp = _ptr(norm3Ds_precomp, keep)
-        a.extra_attrs = _ptr(extra_attrs, keep)
-        a.viewmatrix = _ptr(viewmatrix, keep)
-        a.projmatrix = _ptr(projmatrix, keep)
-        a.cam_pos = _ptr(campos, keep)
-        if graph:
-            a.tan_fovx, a.tan_fovy, tan_fov = _tan_fov(tan_fovx, tan_fovy, dev)
-            a.kernel_size = float(kernel_size)
-        else:
-            a.tan_fovx, a.tan_fovy, a.kernel_size = float(tan_fovx), float(tan_fovy), float(kernel_size)
-        a.prefiltered = int(bool(prefiltered))
-        a.out_color, a.out_depth = out_color.data_ptr(), out_depth.data_ptr()
-        a.out_norm, a.out_alpha = out_norm.data_ptr(), out_alpha.data_ptr()
-        a.out_extra = out_extra.data_ptr() if F > 0 else None
-        a.out_norm_raw = norm_raw.data_ptr() if fuse_normalize else None
-        if out_peers is not None:
-            peer_arr = (C.c_void_p * len(out_peers))(*[int(p) for p in out_peers])
-            keep.append(peer_arr)
-            a.out_peers = C.cast(peer_arr, C.POINTER(C.c_void_p))
-            a.n_out_peers = len(out_peers)
-        a.radii = radii.data_ptr()
-        a.debug = int(bool(debug))
-        a.stream = torch.cuda.current_stream(dev).cuda_stream
-        a.capacity_hint = int(capacity_hint)
-        if tile_rows is not None:
-            a.tile_row_begin, a.tile_row_end = _band(tile_rows)
-        if depth_quantile is not None:
-            depth_q = torch.empty((1, H, W), **fopt)
-            depth_q_pos = torch.empty((H, W), dtype=torch.int32, device=dev)
-            off = _ptr(subpixel_offset, keep) if subpixel_offset is not None else None
-            rendered = N.check(L.sfgs_rasterize_forward_depth_quantile(C.byref(a), off, int(bool(ortho)),
-                                                                       float(depth_quantile), depth_q.data_ptr(),
-                                                                       depth_q_pos.data_ptr()),
-                               "sfgs_rasterize_forward_depth_quantile")
-        elif depth_distortion:
-            distortion = torch.empty((1, H, W), **fopt)
-            distortion_state = torch.empty((2, H, W), **fopt)
-            off = _ptr(subpixel_offset, keep) if subpixel_offset is not None else None
-            rendered = N.check(L.sfgs_rasterize_forward_distortion(C.byref(a), off, int(bool(ortho)),
-                                                                   distortion.data_ptr(), distortion_state.data_ptr()),
-                               "sfgs_rasterize_forward_distortion")
-        elif graph:
-            from . import graphs
-            off = _ptr(subpixel_offset, keep) if subpixel_offset is not None else None
-            N.check(L.sfgs_rasterize_forward_graph(C.byref(a), off, tan_fov.data_ptr() if tan_fov is not None else None,
-                                                   graphs.status_word(dev).data_ptr()),
-                    "sfgs_rasterize_forward_graph")
-            rendered = -1
-        elif ortho:
-            off = _ptr(subpixel_offset, keep) if subpixel_offset is not None else None
-            rendered = N.check(L.sfgs_rasterize_forward_ortho(C.byref(a), off), "sfgs_rasterize_forward_ortho")
-        elif subpixel_offset is not None:
-            entry = "sfgs_rasterize_forward_subpixel" + ("_peers" if out_peers is not None else "")
-            rendered = N.check(getattr(L, entry)(C.byref(a), _ptr(subpixel_offset, keep)), entry)
-        else:
-            rendered = N.check(L.sfgs_rasterize_forward(C.byref(a)), "sfgs_rasterize_forward")
-    ret = (rendered, out_color, out_depth, out_norm, out_alpha, radii, out_extra,
-           geom.tensor, binning.tensor, img.tensor)
-    if fuse_normalize:
-        ret += (norm_raw,)
-    if depth_distortion:
-        return ret + (distortion, distortion_state)
-    return ret + (depth_q, depth_q_pos) if depth_quantile is not None else ret
+        rendered, buffers = 0, (empty, empty.clone(), empty.clone())
+    else:
+        with torch.cuda.device(dev):
+            geom, binning, img = _Arena(dev), _Arena(dev), _Arena(dev)
+            keep = []
+            M = int(sh.shape[1]) if (sh is not None and sh.numel() != 0) else 0
+            a = N.ForwardArgs()
+            a.geom_alloc, a.binning_alloc, a.image_alloc = geom.cb, binning.cb, img.cb
+            a.P, a.D, a.M, a.ED = P, int(degree), M, F
+            a.width, a.height = W, H
+            a.background = _ptr(background, keep)
+            a.means3D = _ptr(means3D, keep)
+            a.shs = _ptr(sh, keep)
+            a.colors_precomp = _ptr(colors, keep)
+            a.opacities = _ptr(opacity, keep)
+            a.scales = _ptr(scales, keep)
+            a.scale_modifier = float(scale_modifier)
+            a.rotations = _ptr(rotations, keep)
+            a.cov3D_precomp = _ptr(cov3Ds_precomp, keep)
+            a.norm3D_precomp = _ptr(norm3Ds_precomp, keep)
+            a.extra_attrs = _ptr(extra_attrs, keep)
+            a.viewmatrix = _ptr(viewmatrix, keep)
+            a.projmatrix = _ptr(projmatrix, keep)
+            a.cam_pos = _ptr(campos, keep)
+            if graph:
+                a.tan_fovx, a.tan_fovy, tan_fov = _tan_fov(tan_fovx, tan_fovy, dev)
+                a.kernel_size = float(kernel_size)
+            else:
+                a.tan_fovx, a.tan_fovy, a.kernel_size = float(tan_fovx), float(tan_fovy), float(kernel_size)
+            a.prefiltered = int(bool(prefiltered))
+            a.out_color, a.out_depth = out_color.data_ptr(), out_depth.data_ptr()
+            a.out_norm, a.out_alpha = out_norm.data_ptr(), out_alpha.data_ptr()
+            a.out_extra = out_extra.data_ptr() if F > 0 else None
+            a.out_norm_raw = norm_raw.data_ptr() if fuse_normalize else None
+            if out_peers is not None:
+                peer_arr = (C.c_void_p * len(out_peers))(*[int(p) for p in out_peers])
+                keep.append(peer_arr)
+                a.out_peers = C.cast(peer_arr, C.POINTER(C.c_void_p))
+                a.n_out_peers = len(out_peers)
+            a.radii = radii.data_ptr()
+            a.debug = int(bool(debug))
+            a.stream = torch.cuda.current_stream(dev).cuda_stream
+            a.capacity_hint = int(capacity_hint)
+            if tile_rows is not None:
+                a.tile_row_begin, a.tile_row_end = _band(tile_rows)
+            # the entry and its arguments after the struct, in the order of precedence of the options
+            off = _ptr(subpixel_offset, keep)
+            if depth_quantile is not None:
+                entry, args = "sfgs_rasterize_forward_depth_quantile", (off, int(bool(ortho)), float(depth_quantile),
+                                                                        side[0].data_ptr(), side[1].data_ptr())
+            elif depth_distortion:
+                entry, args = "sfgs_rasterize_forward_distortion", (off, int(bool(ortho)), side[0].data_ptr(),
+                                                                    side[1].data_ptr())
+            elif graph:
+                from . import graphs
+                entry, args = "sfgs_rasterize_forward_graph", (off, tan_fov.data_ptr() if tan_fov is not None else None,
+                                                               graphs.status_word(dev).data_ptr())
+            elif ortho:
+                entry, args = "sfgs_rasterize_forward_ortho", (off,)
+            elif off is not None:
+                entry, args = "sfgs_rasterize_forward_subpixel" + ("_peers" if out_peers is not None else ""), (off,)
+            else:
+                entry, args = "sfgs_rasterize_forward", ()
+            rendered = N.check(getattr(L, entry)(C.byref(a), *args), entry)
+        rendered, buffers = -1 if graph else rendered, (geom.tensor, binning.tensor, img.tensor)
+    return ((rendered, out_color, out_depth, out_norm, out_alpha, radii, out_extra) + buffers +
+            (norm_raw,) * bool(fuse_normalize) + side)
 
 
 def _use_deterministic(has_extra, has_peers):
@@ -406,201 +362,172 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     a depth-distortion forward (sfgs_rasterize_backward_distortion), which adds dL/dR to the blend adjoint's alpha and
     depth terms.  It takes offsets, `ortho`, the deterministic mode, phase 1, and camera and focal gradients (not with
     `ortho`); depth_q_pos, graph, tile_rows, acc_peers and extra_attrs raise SfgsError."""
-    dist = distortion_state is not None or dL_dout_distortion is not None
+    banded = dict(tile_rows=tile_rows is not None, acc_peers=acc_peers is not None)
+    has_extra = extra_attrs is not None and extra_attrs.numel() != 0
+    dist = _given_together("distortion_state", distortion_state, "dL_dout_distortion", dL_dout_distortion)
     if dist:
-        if distortion_state is None or dL_dout_distortion is None:
-            raise ValueError("distortion_state and dL_dout_distortion come together")
-        _distortion_unsupported("rasterize_gaussians_backward(distortion_state=...)",
-                                depth_q_pos=depth_q_pos is not None or dL_dout_depth_q is not None, graph=graph,
-                                tile_rows=tile_rows is not None, acc_peers=acc_peers is not None,
-                                extra_attrs=extra_attrs is not None and extra_attrs.numel() != 0)
-    depth_q = depth_q_pos is not None or dL_dout_depth_q is not None
+        _reject("rasterize_gaussians_backward(distortion_state=...)", DISTORTION,
+                depth_q_pos=depth_q_pos is not None or dL_dout_depth_q is not None, graph=graph, **banded,
+                extra_attrs=has_extra)
+    depth_q = _given_together("depth_q_pos", depth_q_pos, "dL_dout_depth_q", dL_dout_depth_q)
     if depth_q:
-        if depth_q_pos is None or dL_dout_depth_q is None:
-            raise ValueError("depth_q_pos and dL_dout_depth_q come together")
-        _depth_q_unsupported("rasterize_gaussians_backward(depth_q_pos=...)", graph=graph,
-                             tile_rows=tile_rows is not None, acc_peers=acc_peers is not None,
-                             extra_attrs=extra_attrs is not None and extra_attrs.numel() != 0)
+        _reject("rasterize_gaussians_backward(depth_q_pos=...)", DEPTH_Q, graph=graph, **banded, extra_attrs=has_extra)
     if ortho:
-        _ortho_unsupported("rasterize_gaussians_backward(ortho=True)", graph=graph, tile_rows=tile_rows is not None,
-                           acc_peers=acc_peers is not None, **{f"phase={int(phase)}": int(phase) != 0},
-                           camera_grad=camera_grad, intrinsics_grad=intrinsics_grad)
+        _reject("rasterize_gaussians_backward(ortho=True)", ORTHO, graph=graph, **banded,
+                **{f"phase={int(phase)}": int(phase) != 0}, camera_grad=camera_grad, intrinsics_grad=intrinsics_grad)
     if intrinsics_grad and not camera_grad:
         raise ValueError("intrinsics_grad=True needs camera_grad=True")
     if graph:
-        _graph_unsupported("rasterize_gaussians_backward(graph=True)", debug, tile_rows,
-                           "acc_peers" if acc_peers is not None else None, int(phase))
+        _reject("rasterize_gaussians_backward(graph=True)", GRAPH,
+                **{"debug=True (it synchronises after every stage)": debug}, **banded,
+                **{f"phase={int(phase)} (the two-phase backward)": int(phase) != 0})
+    H, W = int(dL_dout_color.shape[1]), int(dL_dout_color.shape[2])
+    dev = means3D.device
     if subpixel_offset is not None:
-        check_subpixel_offset(subpixel_offset, int(dL_dout_color.shape[1]), int(dL_dout_color.shape[2]))
+        check_subpixel_offset(subpixel_offset, H, W)
     if depth_q:
-        _check_depth_q(depth_q_pos, dL_dout_depth_q, int(dL_dout_color.shape[1]), int(dL_dout_color.shape[2]),
-                       means3D.device)
+        _check_pixel_inputs("depth_q_pos", depth_q_pos, torch.int32, (H, W), "dL_dout_depth_q", dL_dout_depth_q,
+                            H, W, dev)
     if dist:
-        _check_distortion(distortion_state, dL_dout_distortion, int(dL_dout_color.shape[1]),
-                          int(dL_dout_color.shape[2]), means3D.device)
-    F = int(extra_attrs.shape[1]) if (extra_attrs is not None and extra_attrs.numel() != 0) else 0
+        _check_pixel_inputs("distortion_state", distortion_state, torch.float32, (2, H, W), "dL_dout_distortion",
+                            dL_dout_distortion, H, W, dev)
+    F = int(extra_attrs.shape[1]) if has_extra else 0
     deterministic = _use_deterministic(F > 0, acc_peers is not None)
     L = N.lib()
     P = int(means3D.shape[0])
-    H, W = int(dL_dout_color.shape[1]), int(dL_dout_color.shape[2])
     M = int(sh.shape[1]) if (sh is not None and sh.numel() != 0) else 0
-    dev = means3D.device
     fopt = dict(dtype=torch.float32, device=dev)
+    ncam = (37 if intrinsics_grad else 35) if camera_grad else 0
+    # phase 2 returns the camera terms as one float64 partial, formed by sfgs_rasterize_backward_camera_partial; the
+    # quantile and distortion entries take float32 terms (and reject phase 2), and P == 0 returns zeros as a partial
+    partial = camera_grad and phase == 2
+    alloc = torch.zeros if P == 0 else torch.empty      # the reference returns zero gradients for P == 0
 
-    if P == 0:
-        z = lambda *s: torch.zeros(s, **fopt)  # noqa: E731
-        ret = (z(P, 3), z(P, 3), z(P, 1), z(P, 3), z(P, 6), z(P, 3), z(P, M, 3), z(P, 3), z(P, 4),
-               z(P, F) if F > 0 else torch.empty(0, **fopt))
-        if camera_grad and phase == 2:
-            return ret + (torch.zeros((37 if intrinsics_grad else 35,), dtype=torch.float64, device=dev),)
-        if camera_grad:
-            ret += (z(4, 4), z(4, 4), z(3))
-        return ret + (z(), z()) if intrinsics_grad else ret
-
-    with torch.cuda.device(dev), _no_fill(deterministic):
+    with _no_fill(deterministic):
         # one allocation for all fixed-width per-Gaussian gradients (every element is written by the kernel)
         widths = dict(means3D=3, means2D=3, colors=3, depths=1, conic=4, opacity=1, cov3D=6, norm3D=3, scales=3, rot=4)
         pad = lambda n: (n + 3) & ~3                       # keep every sub-array 16-byte aligned  # noqa: E731
-        flat = torch.empty((sum(pad(P * w) for w in widths.values()),), **fopt)
-        outs, off = {}, 0
+        flat = alloc((sum(pad(P * w) for w in widths.values()),), **fopt)
+        outs, pos = {}, 0
         for k, w in widths.items():
-            outs[k] = flat[off:off + P * w].view(P, w)
-            off += pad(P * w)
-        dL_dsh = torch.empty((P, M, 3), **fopt) if M > 0 else torch.zeros((P, 0, 3), **fopt)
-        dL_dextra = torch.empty((P, F), **fopt) if F > 0 else torch.empty(0, **fopt)
-        scratch = _Arena(dev)
-        keep = []
-        a = N.BackwardArgs()
-        a.phase = int(phase)
-        if acc_peers is not None:
-            # phase 1 with the reduce-scatter fused into the kernel: peer-mapped slice pointers, nothing allocated here
-            if phase != 1:
-                raise ValueError("acc_peers is a phase-1 option")
-            peer_arr = (C.c_void_p * len(acc_peers))(*[int(p) for p in acc_peers])
-            keep.append(peer_arr)                      # must outlive the call
-            a.acc_peers = C.cast(peer_arr, C.POINTER(C.c_void_p))
-            a.n_peers, a.peer_slice = len(acc_peers), int(peer_slice)
-        elif phase == 1 and acc is None:
-            acc = torch.empty((P, 16), **fopt)
-        if acc is not None:
-            a.acc = _ptr(acc, keep)
-        if gauss_range is not None:
-            a.gauss_begin, a.gauss_end = int(gauss_range[0]), int(gauss_range[1])
-        a.P, a.D, a.M, a.R, a.ED = P, int(degree), M, int(R), F
-        a.width, a.height = W, H
-        a.background = _ptr(background, keep)
-        a.means3D = _ptr(means3D, keep)
-        a.shs = _ptr(sh, keep)
-        a.colors_precomp = _ptr(colors, keep)
-        a.scales = _ptr(scales, keep)
-        a.scale_modifier = float(scale_modifier)
-        a.rotations = _ptr(rotations, keep)
-        a.cov3D_precomp = _ptr(cov3Ds_precomp, keep)
-        a.norm3D_precomp = _ptr(norm3Ds_precomp, keep)
-        a.extra_attrs = _ptr(extra_attrs, keep)
-        a.viewmatrix = _ptr(viewmatrix, keep)
-        a.projmatrix = _ptr(projmatrix, keep)
-        a.cam_pos = _ptr(campos, keep)
-        if graph:
-            a.tan_fovx, a.tan_fovy, tan_fov = _tan_fov(tan_fovx, tan_fovy, dev)
-            a.kernel_size = float(kernel_size)
-        else:
-            a.tan_fovx, a.tan_fovy, a.kernel_size = float(tan_fovx), float(tan_fovy), float(kernel_size)
-        a.radii = _ptr(radii, keep)
-        a.geom_buffer = _ptr(geomBuffer, keep)
-        a.binning_buffer = _ptr(binningBuffer, keep)
-        a.image_buffer = _ptr(imageBuffer, keep)
-        a.accum_alphas = _ptr(out_alpha, keep)
-        a.dL_dpix = _ptr(dL_dout_color, keep)
-        a.dL_dpix_depth = _ptr(dL_dout_depth, keep)
-        a.dL_dpix_norm = _ptr(dL_dout_norm, keep)
-        a.dL_dpix_alpha = _ptr(dL_dout_alpha, keep)
-        a.norm_raw = _ptr(norm_raw, keep) if norm_raw is not None else None
-        a.dL_dpix_extra = _ptr(dL_dout_extra, keep) if F > 0 else None
-        a.dL_dmean2D = outs["means2D"].data_ptr()
-        a.dL_dconic = outs["conic"].data_ptr()
-        a.dL_dopacity = outs["opacity"].data_ptr()
-        a.dL_dcolor = outs["colors"].data_ptr()
-        a.dL_ddepth = outs["depths"].data_ptr()
-        a.dL_dmean3D = outs["means3D"].data_ptr()
-        a.dL_dcov3D = outs["cov3D"].data_ptr()
-        a.dL_dnorm3D = outs["norm3D"].data_ptr()
-        a.dL_dsh = dL_dsh.data_ptr() if M > 0 else None
-        a.dL_dscale = outs["scales"].data_ptr()
-        a.dL_drot = outs["rot"].data_ptr()
-        a.dL_dextra = dL_dextra.data_ptr() if F > 0 else None
-        a.scratch_alloc = scratch.cb
-        a.debug = int(bool(debug))
-        a.stream = torch.cuda.current_stream(dev).cuda_stream
-        if tile_rows is not None:
-            a.tile_row_begin, a.tile_row_end = _band(tile_rows)
-        if depth_q:
-            ncam = (37 if intrinsics_grad else 35) if camera_grad else 0
-            dL_dcamera = torch.empty((ncam,), **fopt) if ncam else None
-            off = _ptr(subpixel_offset, keep) if subpixel_offset is not None else None
-            N.check(L.sfgs_rasterize_backward_depth_quantile(C.byref(a), off, int(bool(ortho)), int(deterministic),
-                                                             _ptr(depth_q_pos, keep), _ptr(dL_dout_depth_q, keep),
-                                                             dL_dcamera.data_ptr() if ncam else None, ncam),
-                    "sfgs_rasterize_backward_depth_quantile")
-        elif dist:
-            ncam = (37 if intrinsics_grad else 35) if camera_grad else 0
-            dL_dcamera = torch.empty((ncam,), **fopt) if ncam else None
-            off = _ptr(subpixel_offset, keep) if subpixel_offset is not None else None
-            N.check(L.sfgs_rasterize_backward_distortion(C.byref(a), off, int(bool(ortho)), int(deterministic),
-                                                         _ptr(distortion_state, keep),
-                                                         _ptr(dL_dout_distortion, keep),
-                                                         dL_dcamera.data_ptr() if ncam else None, ncam),
-                    "sfgs_rasterize_backward_distortion")
-        elif graph:
-            ncam = (37 if intrinsics_grad else 35) if camera_grad else 0
-            dL_dcamera = torch.empty((ncam,), **fopt) if ncam else None
-            off = _ptr(subpixel_offset, keep) if subpixel_offset is not None else None
-            N.check(L.sfgs_rasterize_backward_graph(C.byref(a), off, int(deterministic),
-                                                    tan_fov.data_ptr() if tan_fov is not None else None,
-                                                    dL_dcamera.data_ptr() if ncam else None, ncam),
-                    "sfgs_rasterize_backward_graph")
-        elif ortho:
-            off = _ptr(subpixel_offset, keep) if subpixel_offset is not None else None
-            N.check(L.sfgs_rasterize_backward_ortho(C.byref(a), off, int(deterministic)), "sfgs_rasterize_backward_ortho")
-        elif camera_grad and phase == 2:
-            ncam = 37 if intrinsics_grad else 35
-            dL_dcamera = torch.empty((ncam,), dtype=torch.float64, device=dev)
-            off = _ptr(subpixel_offset, keep) if subpixel_offset is not None else None
-            N.check(L.sfgs_rasterize_backward_camera_partial(C.byref(a), off, int(deterministic), ncam,
-                                                             dL_dcamera.data_ptr()),
-                    "sfgs_rasterize_backward_camera_partial")
-        elif camera_grad:
-            dL_dcamera = torch.empty((37 if intrinsics_grad else 35,), **fopt)
-            off = _ptr(subpixel_offset, keep) if subpixel_offset is not None else None
-            entry = "sfgs_rasterize_backward_camera_intrinsics" if intrinsics_grad else "sfgs_rasterize_backward_camera"
-            N.check(getattr(L, entry)(C.byref(a), off, int(deterministic), dL_dcamera.data_ptr()), entry)
-        elif subpixel_offset is not None:
-            off = _ptr(subpixel_offset, keep)
-            if deterministic:
-                N.check(L.sfgs_rasterize_backward_deterministic_subpixel(C.byref(a), off),
-                        "sfgs_rasterize_backward_deterministic_subpixel")
-            else:
-                entry = "sfgs_rasterize_backward_subpixel" + ("_peers" if acc_peers is not None else "")
-                N.check(getattr(L, entry)(C.byref(a), off), entry)
-        elif deterministic:
-            N.check(L.sfgs_rasterize_backward_deterministic(C.byref(a)), "sfgs_rasterize_backward_deterministic")
-        else:
-            N.check(L.sfgs_rasterize_backward(C.byref(a)), "sfgs_rasterize_backward")
-        # the arena and its callback form a reference cycle: drop the scratch now (stream-ordered, like any freed
-        # tensor) instead of whenever the garbage collector runs — the deterministic path's scratch is ~0.5 KB per
-        # tile instance
-        scratch.tensor = None
-    if phase == 1:
-        return acc      # None when the sums went straight to the peers' slices
+            outs[k] = flat[pos:pos + P * w].view(P, w)
+            pos += pad(P * w)
+        dL_dsh = alloc((P, M, 3), **fopt)
+        dL_dextra = alloc((P, F), **fopt) if F > 0 else torch.empty(0, **fopt)
+        f64 = partial and (P == 0 or not (depth_q or dist))
+        dL_dcamera = alloc((ncam,), dtype=torch.float64 if f64 else torch.float32, device=dev) if ncam else None
+        if P > 0:
+            with torch.cuda.device(dev):
+                scratch = _Arena(dev)
+                keep = []
+                a = N.BackwardArgs()
+                a.phase = int(phase)
+                if acc_peers is not None:
+                    # phase 1 with the reduce-scatter fused into the kernel: peer-mapped slice pointers, nothing
+                    # allocated here
+                    if phase != 1:
+                        raise ValueError("acc_peers is a phase-1 option")
+                    peer_arr = (C.c_void_p * len(acc_peers))(*[int(p) for p in acc_peers])
+                    keep.append(peer_arr)                      # must outlive the call
+                    a.acc_peers = C.cast(peer_arr, C.POINTER(C.c_void_p))
+                    a.n_peers, a.peer_slice = len(acc_peers), int(peer_slice)
+                elif phase == 1 and acc is None:
+                    acc = torch.empty((P, 16), **fopt)
+                if acc is not None:
+                    a.acc = _ptr(acc, keep)
+                if gauss_range is not None:
+                    a.gauss_begin, a.gauss_end = int(gauss_range[0]), int(gauss_range[1])
+                a.P, a.D, a.M, a.R, a.ED = P, int(degree), M, int(R), F
+                a.width, a.height = W, H
+                a.background = _ptr(background, keep)
+                a.means3D = _ptr(means3D, keep)
+                a.shs = _ptr(sh, keep)
+                a.colors_precomp = _ptr(colors, keep)
+                a.scales = _ptr(scales, keep)
+                a.scale_modifier = float(scale_modifier)
+                a.rotations = _ptr(rotations, keep)
+                a.cov3D_precomp = _ptr(cov3Ds_precomp, keep)
+                a.norm3D_precomp = _ptr(norm3Ds_precomp, keep)
+                a.extra_attrs = _ptr(extra_attrs, keep)
+                a.viewmatrix = _ptr(viewmatrix, keep)
+                a.projmatrix = _ptr(projmatrix, keep)
+                a.cam_pos = _ptr(campos, keep)
+                if graph:
+                    a.tan_fovx, a.tan_fovy, tan_fov = _tan_fov(tan_fovx, tan_fovy, dev)
+                    a.kernel_size = float(kernel_size)
+                else:
+                    a.tan_fovx, a.tan_fovy, a.kernel_size = float(tan_fovx), float(tan_fovy), float(kernel_size)
+                a.radii = _ptr(radii, keep)
+                a.geom_buffer = _ptr(geomBuffer, keep)
+                a.binning_buffer = _ptr(binningBuffer, keep)
+                a.image_buffer = _ptr(imageBuffer, keep)
+                a.accum_alphas = _ptr(out_alpha, keep)
+                a.dL_dpix = _ptr(dL_dout_color, keep)
+                a.dL_dpix_depth = _ptr(dL_dout_depth, keep)
+                a.dL_dpix_norm = _ptr(dL_dout_norm, keep)
+                a.dL_dpix_alpha = _ptr(dL_dout_alpha, keep)
+                a.norm_raw = _ptr(norm_raw, keep) if norm_raw is not None else None
+                a.dL_dpix_extra = _ptr(dL_dout_extra, keep) if F > 0 else None
+                a.dL_dmean2D = outs["means2D"].data_ptr()
+                a.dL_dconic = outs["conic"].data_ptr()
+                a.dL_dopacity = outs["opacity"].data_ptr()
+                a.dL_dcolor = outs["colors"].data_ptr()
+                a.dL_ddepth = outs["depths"].data_ptr()
+                a.dL_dmean3D = outs["means3D"].data_ptr()
+                a.dL_dcov3D = outs["cov3D"].data_ptr()
+                a.dL_dnorm3D = outs["norm3D"].data_ptr()
+                a.dL_dsh = dL_dsh.data_ptr() if M > 0 else None
+                a.dL_dscale = outs["scales"].data_ptr()
+                a.dL_drot = outs["rot"].data_ptr()
+                a.dL_dextra = dL_dextra.data_ptr() if F > 0 else None
+                a.scratch_alloc = scratch.cb
+                a.debug = int(bool(debug))
+                a.stream = torch.cuda.current_stream(dev).cuda_stream
+                if tile_rows is not None:
+                    a.tile_row_begin, a.tile_row_end = _band(tile_rows)
+                # the entry and its arguments after the struct, in the order of precedence of the options
+                off = _ptr(subpixel_offset, keep)
+                det = int(deterministic)
+                cam = dL_dcamera.data_ptr() if ncam else None
+                if depth_q:
+                    entry, args = "sfgs_rasterize_backward_depth_quantile", (off, int(bool(ortho)), det,
+                                                                             _ptr(depth_q_pos, keep),
+                                                                             _ptr(dL_dout_depth_q, keep), cam, ncam)
+                elif dist:
+                    entry, args = "sfgs_rasterize_backward_distortion", (off, int(bool(ortho)), det,
+                                                                         _ptr(distortion_state, keep),
+                                                                         _ptr(dL_dout_distortion, keep), cam, ncam)
+                elif graph:
+                    entry, args = "sfgs_rasterize_backward_graph", (off, det, tan_fov.data_ptr() if tan_fov is not None
+                                                                    else None, cam, ncam)
+                elif ortho:
+                    entry, args = "sfgs_rasterize_backward_ortho", (off, det)
+                elif partial:
+                    entry, args = "sfgs_rasterize_backward_camera_partial", (off, det, ncam, cam)
+                elif camera_grad:
+                    entry = "sfgs_rasterize_backward_camera" + ("_intrinsics" if intrinsics_grad else "")
+                    args = (off, det, cam)
+                elif off is not None:
+                    entry = ("sfgs_rasterize_backward_deterministic_subpixel" if deterministic else
+                             "sfgs_rasterize_backward_subpixel" + ("_peers" if acc_peers is not None else ""))
+                    args = (off,)
+                else:
+                    entry, args = "sfgs_rasterize_backward" + ("_deterministic" if deterministic else ""), ()
+                N.check(getattr(L, entry)(C.byref(a), *args), entry)
+                # the arena and its callback form a reference cycle: drop the scratch now (stream-ordered, like any
+                # freed tensor) instead of whenever the garbage collector runs — the deterministic path's scratch is
+                # ~0.5 KB per tile instance
+                scratch.tensor = None
+            if phase == 1:
+                return acc      # None when the sums went straight to the peers' slices
     ret = (outs["means2D"], outs["colors"], outs["opacity"], outs["means3D"], outs["cov3D"], outs["norm3D"],
            dL_dsh, outs["scales"], outs["rot"], dL_dextra)
-    if camera_grad and phase == 2:
+    if not ncam:
+        return ret
+    if partial:
         return ret + (dL_dcamera,)
-    if camera_grad:
-        ret += (dL_dcamera[0:16].view(4, 4), dL_dcamera[16:32].view(4, 4), dL_dcamera[32:35])
-    if intrinsics_grad:
-        ret += (dL_dcamera[35], dL_dcamera[36])
-    return ret
+    ret += (dL_dcamera[0:16].view(4, 4), dL_dcamera[16:32].view(4, 4), dL_dcamera[32:35])
+    return ret + (dL_dcamera[35], dL_dcamera[36]) if intrinsics_grad else ret
 
 
 def mark_visible(means3D, viewmatrix, projmatrix):

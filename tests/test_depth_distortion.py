@@ -224,6 +224,31 @@ def test_modules_reject_before_native_calls(monkeypatch):
                                                rs, False, None, None, None, None, None, None, True)
 
 
+def test_ortho_rasterizer_rejects_capture_before_native_calls(monkeypatch):
+    """OrthoRasterizer runs through diff_gauss's Function: under stream capture it raises before any capture-time
+    work (the capacity is not resolved) and before any native call."""
+    import diff_gauss
+    from sfgs import native as N
+    from sfgs.ortho import OrthoRasterizationSettings, OrthoRasterizer
+
+    def no_lib():
+        raise AssertionError("native library called")
+
+    def no_capacity(*a, **k):
+        raise AssertionError("capture-time work before the orthographic camera's check")
+    monkeypatch.setattr(N, "lib", no_lib)
+    monkeypatch.setattr(diff_gauss._graphs, "resolve_capacity", no_capacity)
+    monkeypatch.setattr(torch.cuda, "is_current_stream_capturing", lambda: True)
+    monkeypatch.setattr(torch.Tensor, "is_cuda", property(lambda self: True))
+    m = torch.zeros((4, 3))
+    kw = dict(shs=torch.zeros((4, 16, 3)), scales=torch.ones((4, 3)), rotations=torch.zeros((4, 4)))
+    ors = OrthoRasterizationSettings(8, 8, 1.0, 1.0, 0.1, torch.zeros(3), 1.0, torch.eye(4), torch.eye(4), 3, False,
+                                     False)
+    for opts, what in ((dict(), "the orthographic camera"), (dict(depth_distortion=True), "the depth distortion")):
+        with pytest.raises(N.SfgsError, match=f"diff_gauss: {what} cannot be captured in a CUDA graph"):
+            OrthoRasterizer(ors, **opts)(m, m, torch.ones((4, 1)), **kw)
+
+
 def test_ortho_rasterizer_is_an_ordinary_module():
     from sfgs.ortho import OrthoRasterizationSettings, OrthoRasterizer
     rs = OrthoRasterizationSettings(8, 8, 1.0, 1.0, 0.1, torch.zeros(3), 1.0, torch.eye(4), torch.eye(4), 0, False, False)
