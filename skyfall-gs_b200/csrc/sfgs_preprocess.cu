@@ -200,6 +200,8 @@ constexpr int PRE_SPAN = 1024;        // Gaussians per block: four per thread in
 // Upper bound of the screen-space radius the exact projection can produce (for the conservative pre-cull).
 //   radius = ceil(3 sqrt(lambda_max)),  lambda_max <= mid + sqrt(max(0.1, mid^2 - det)) <= 2 mid + 0.32 = trace(cov2D') + 0.32,
 //   trace(cov2D') = trace(T Sigma T^T) + 2 k <= |J|_F^2 |W|_F^2 trace(Sigma) + 2 k   (T = W J, kernel_size k on the diagonal)
+//   for a PSD Sigma; for any symmetric Sigma, lambda_max(T Sigma T^T) <= |T|_F^2 |Sigma|_F, and the same sum bounds lambda_max
+//   with |Sigma|_F in place of trace(Sigma) (the caller passes whichever applies).
 //   |J|_F^2 = (fx^2 (1 + (tx/tz)^2) + fy^2 (1 + (ty/tz)^2)) / tz^2 with |tx/tz| <= 1.3 tan(fovx/2) after the reference's clamp.
 // Every factor is rounded up generously (1 %, +3 px): the bound only has to be safe, not tight — a Gaussian passes the
 // pre-cull when the tile rectangle of (centre, bound) is non-empty, and the exact path then decides.
@@ -272,10 +274,10 @@ preprocess_kernel(int P, int D, int M,
     const int i = base + j * PRE_THREADS + tid;
     const size_t ii = (size_t)(i < P ? i : P - 1);
     pos4[j] = make_float3(means3D[3 * ii], means3D[3 * ii + 1], means3D[3 * ii + 2]);
-    if (cov3D_precomp != nullptr) {
+    if (cov3D_precomp != nullptr) {     // diagonal in scl4, off-diagonal in rot4
       const float* c = cov3D_precomp + 6 * ii;
       scl4[j] = make_float3(c[0], c[3], c[5]);
-      rot4[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+      rot4[j] = make_float4(c[1], c[2], c[4], 0.f);
     } else {
       scl4[j] = make_float3(scales[3 * ii], scales[3 * ii + 1], scales[3 * ii + 2]);
       rot4[j] = *reinterpret_cast<const float4*>(rotations + 4 * ii);
@@ -300,9 +302,15 @@ preprocess_kernel(int P, int D, int M,
           const float p_w = 1.0f / (hw + 0.0000001f);
           pix_x = ndc_to_pix(hx * p_w, W); pix_y = ndc_to_pix(hy * p_w, H);
         }
-        float trace_sigma;
+        float trace_sigma;     // a bound of |lambda| of Sigma
         if (cov3D_precomp != nullptr) {
-          trace_sigma = scl4[j].x + scl4[j].y + scl4[j].z;
+          // a precomputed Sigma need not be positive semi-definite (the reference projects any Sigma whose 2D
+          // determinant is non-zero), and its trace bounds no eigenvalue then: diag(4, -4, 0) has trace 0 and projects
+          // to hundreds of pixels.  The Frobenius norm bounds |lambda| for every symmetric Sigma, and is never above
+          // the trace of a PSD one.
+          const float3 dg = scl4[j];
+          const float4 od = rot4[j];
+          trace_sigma = sqrtf(dg.x * dg.x + dg.y * dg.y + dg.z * dg.z + 2.f * (od.x * od.x + od.y * od.y + od.z * od.z));
         } else {
           const float sx = scl4[j].x, sy = scl4[j].y, sz = scl4[j].z;
           const float4 q = rot4[j];
