@@ -423,6 +423,44 @@ int sfgs_rasterize_backward_distortion(const sfgs_backward_args* a, const float*
                                        int deterministic, const float* distortion_state,
                                        const float* dL_dpix_distortion, float* dL_dcamera, int ncam);
 
+/* ---- Ray depth ---------------------------------------------------------------------------------------------------
+ * The one-call forward whose depth is each splat's depth where the pixel's ray meets it, not its centre's depth, and
+ * the backward that differentiates it.  A flat splat on a slope (a roof, the ground seen obliquely) then reports a
+ * depth that changes across its pixels, and the depth's gradient reaches its rotation and scale.
+ *   - Record i contributes at the sample position p (the pixel centre, or the jittered position under offsets)
+ *         d_i(p) = z_i + g_i . (p - mu_i)
+ *     with z_i the view depth t_z of its centre (the depth word), mu_i its projected centre in pixels, and the slope
+ *     g_i = C s (depth units per pixel): C the record's conic (Sigma2D + kernel_size I)^-1, s = (w3^T Sigma T0^T,
+ *     w3^T Sigma T1^T) the covariance of view depth with the two pixel coordinates under the EWA linearisation
+ *     (T = J W, Sigma the 3D covariance after scale_modifier, w3 = (view[2], view[6], view[10])).  d_i(p) is the
+ *     conditional mean of the splat's depth given the pixel; |d_i(p) - z_i| <= sigma_z sqrt(2 ln(255 o_i)) for an
+ *     applied pair (sigma_z^2 = w3^T Sigma w3), so it stays within about 3.3 sigma_z of z_i.
+ *   - out_depth = sum (d_i(p) alpha_i) T_i.  With a quantile (out_depth_q != NULL, as
+ *     sfgs_rasterize_forward_depth_quantile), out_depth_q is the selected record's d_j(p); the selection and
+ *     out_depth_q_pos are unchanged.  Colour, alpha, normals, n_contrib, radii and binning are bit-identical to the
+ *     matching entry without the option; record words 14-15 (0 otherwise) hold g.
+ *   - Gradient, with c the pixel's depth cotangent: the blend adjoint uses d_i(p) as the depth attribute; acc words
+ *     14-15 sum w c (p - mu_i) (dL/dg) beside word 3 (w c); dL/dmu_i gains -g_i word 3 in dL_dmean2D[:, 0:2] (not in
+ *     the abs channel [:, 2]); dL/dg reaches the conic, cov3D, scales, rotations, means3D and the camera terms.  With a
+ *     quantile, dL_dpix_depth_q adds c (p - mu_j) to words 14-15 of the selected record as well.  With every depth
+ *     cotangent 0 the deterministic gradients are those of the matching entry (up to the sign of a zero).
+ * ortho, subpixel_offset, deterministic, ncam and dL_dcamera as for the depth quantile's entries.  The backward must be
+ * given the forward's option (its records carry g), camera form and offsets; depth_q_pos and dL_dpix_depth_q are
+ * both NULL (no quantile) or both given.  Phase 1 over the whole frame is accepted.
+ * Before any CUDA work, in this order:
+ *   forward:  a NULL args (SFGS_E_BADARG); with out_depth_q given, a NULL out_depth_q_pos or q not finite with
+ *             0 < q < 1 (SFGS_E_BADARG); ED > 0, a tile-row band, out_peers (SFGS_E_UNSUPPORTED); then the checks
+ *             of the matching entry.
+ *   backward: a NULL args (SFGS_E_BADARG); one of depth_q_pos, dL_dpix_depth_q without the other, ncam not 0, 35 or
+ *             37 (SFGS_E_BADARG); ED > 0, a tile-row band, acc_peers, phase 2, ncam > 0 with phase 1, ncam > 0 with
+ *             ortho (SFGS_E_UNSUPPORTED); then the checks of the matching entry.
+ * Not available under graph capture, with tile-row sharding, with extra_attrs or together with the depth distortion. */
+int sfgs_rasterize_forward_ray_depth(const sfgs_forward_args* a, const float* subpixel_offset, int ortho,
+                                     float quantile, float* out_depth_q, uint32_t* out_depth_q_pos);
+int sfgs_rasterize_backward_ray_depth(const sfgs_backward_args* a, const float* subpixel_offset, int ortho,
+                                      int deterministic, const uint32_t* depth_q_pos, const float* dL_dpix_depth_q,
+                                      float* dL_dcamera, int ncam);
+
 /* ---- markVisible --------------------------------------------------------- */
 int sfgs_mark_visible(int P, const float* means3D, const float* viewmatrix,
                       const float* projmatrix, unsigned char* present, void* stream);

@@ -26,7 +26,7 @@ std::atomic<long long> g_sfgs_launches{0};
 
 void sfgs_launch_preprocess(const sfgs_forward_args* a, const GeomLayout& g, const ImageLayout& im,
                             const BinningLayout& b, unsigned long long capacity, float focal_x, float focal_y,
-                            const float* tan_fov, bool ortho, cudaStream_t st);
+                            const float* tan_fov, bool ortho, bool ray_depth, cudaStream_t st);
 void sfgs_launch_mark_visible(int P, const float* means3D, const float* viewmatrix, unsigned char* present,
                               cudaStream_t st);
 void sfgs_launch_tile_scan(const ImageLayout& im, unsigned long long capacity, cudaStream_t st);
@@ -38,13 +38,15 @@ void sfgs_launch_tile_sort(const GeomLayout& g, const ImageLayout& im, const Bin
 void sfgs_launch_offset_bound(const ImageLayout& im, int W, int H, const float* off, cudaStream_t st);
 void sfgs_launch_render_fwd(const sfgs_forward_args* a, const GeomLayout& g, const ImageLayout& im,
                             const BinningLayout& b, const float* off, float t, float* out_depth_q,
-                            uint32_t* out_depth_q_pos, float* out_dist, float* out_dist_state, cudaStream_t st);
+                            uint32_t* out_depth_q_pos, float* out_dist, float* out_dist_state, bool ray_depth,
+                            cudaStream_t st);
 void sfgs_launch_render_bwd(const sfgs_backward_args* a, const GeomLayout& g, const ImageLayout& im,
                             const BinningLayout& b, float* acc, float* part, unsigned char* written, const float* off,
-                            bool guarded, const float* dist_state, const float* dL_dpix_dist, cudaStream_t st);
-void sfgs_launch_depth_q_adjoint(const sfgs_backward_args* a, const ImageLayout& im, const BinningLayout& b,
-                                 const uint32_t* depth_q_pos, const float* dL_dpix_depth_q, float* acc, float* part,
-                                 cudaStream_t st);
+                            bool guarded, const float* dist_state, const float* dL_dpix_dist, bool ray_depth,
+                            cudaStream_t st);
+void sfgs_launch_depth_q_adjoint(const sfgs_backward_args* a, const GeomLayout& g, const ImageLayout& im,
+                                 const BinningLayout& b, const uint32_t* depth_q_pos, const float* dL_dpix_depth_q,
+                                 float* acc, float* part, bool ray_depth, const float* off, cudaStream_t st);
 size_t sfgs_order_scratch_bytes(int P, long long R);
 SfgsOrderScratch sfgs_order_scratch(char* base, int P, long long R);
 void sfgs_launch_order_prepare(int P, const GeomLayout& g, const ImageLayout& im, const BinningLayout& b,
@@ -61,7 +63,7 @@ int sfgs_launch_activations_bwd(int P, const float* opacity_raw, const float* sc
                                 float* g_rotation_raw, cudaStream_t st);
 void sfgs_launch_gauss_bwd(const sfgs_backward_args* a, const GeomLayout& g, float focal_x, float focal_y,
                            const float* acc, int g_begin, int g_end, int acc_row0, double* cam_part, int ncam,
-                           const float* tan_fov, bool ortho, cudaStream_t st);
+                           const float* tan_fov, bool ortho, bool ray_depth, cudaStream_t st);
 size_t sfgs_camera_scratch_bytes(int P, int ncam);
 void sfgs_launch_camera_reduce(int P, int ncam, const double* cam_part, float* dL_dcamera, cudaStream_t st);
 void sfgs_launch_camera_partial_reduce(int n, int ncam, const double* cam_part, double* dL_dcamera, cudaStream_t st);
@@ -224,6 +226,7 @@ struct FwdCall {
   bool dist = false;                  // the depth distortion (sfgs_rasterize_forward_distortion): R [H,W] ...
   float* out_distortion = nullptr;
   float* out_distortion_state = nullptr;   // ... and the state (mu, M2) [2,H,W] its adjoint reads
+  bool ray_depth = false;             // ray depth (sfgs_rasterize_forward_ray_depth), with or without depth_q
 };
 
 struct BwdCall {
@@ -243,6 +246,7 @@ struct BwdCall {
   bool dist = false;                  // the depth distortion's adjoint (sfgs_rasterize_backward_distortion) ...
   const float* distortion_state = nullptr;    // ... from the forward's state [2,H,W] ...
   const float* dL_dpix_distortion = nullptr;  // ... and the cotangent of R [H,W]
+  bool ray_depth = false;             // ray depth's adjoint (sfgs_rasterize_backward_ray_depth), with or without depth_q
 };
 
 int rasterize_forward(const sfgs_forward_args* a, const FwdCall& c);
@@ -395,6 +399,32 @@ int sfgs_rasterize_backward_distortion(const sfgs_backward_args* a, const float*
   return rasterize_backward(a, c);
 }
 
+int sfgs_rasterize_forward_ray_depth(const sfgs_forward_args* a, const float* subpixel_offset, int ortho,
+                                     float quantile, float* out_depth_q, uint32_t* out_depth_q_pos) {
+  FwdCall c{"forward_ray_depth", false, subpixel_offset};
+  c.ortho = ortho != 0;
+  c.ray_depth = true;
+  c.depth_q = out_depth_q != nullptr;     // NULL: no quantile
+  c.quantile = quantile;
+  c.out_depth_q = out_depth_q;
+  c.out_depth_q_pos = out_depth_q_pos;
+  return rasterize_forward(a, c);
+}
+
+int sfgs_rasterize_backward_ray_depth(const sfgs_backward_args* a, const float* subpixel_offset, int ortho,
+                                      int deterministic, const uint32_t* depth_q_pos, const float* dL_dpix_depth_q,
+                                      float* dL_dcamera, int ncam) {
+  // ncam > 0: the checks and the stages of sfgs_rasterize_backward_camera[_intrinsics] (a bad ncam is rejected first)
+  BwdCall c{"backward_ray_depth", ncam > 0 ? BwdCall::CAMERA : BwdCall::EAGER, subpixel_offset, false,
+            deterministic != 0, ncam, ncam > 0 ? dL_dcamera : nullptr};
+  c.ortho = ortho != 0;
+  c.ray_depth = true;
+  c.depth_q = depth_q_pos != nullptr || dL_dpix_depth_q != nullptr;   // both NULL: no quantile
+  c.depth_q_pos = depth_q_pos;
+  c.dL_dpix_depth_q = dL_dpix_depth_q;
+  return rasterize_backward(a, c);
+}
+
 }  // extern "C"
 
 namespace {
@@ -428,6 +458,14 @@ int check_pixel_output(const sfgs_forward_args* a, const char* entry, bool null_
 int check_forward(const sfgs_forward_args* a, const FwdCall& c) {
   const auto reject = [&c](int code, const char* what) { return fail_in(c.name, code, what); };
   if (!a) return reject(SFGS_E_BADARG, "null args");
+  if (c.ray_depth) {
+    // with a quantile (out_depth_q given) its own arguments first; every unsupported option is then reported as ray
+    // depth's (the quantile's check below finds nothing left)
+    const char* bad_q = !c.depth_q || quantile_ok(c.quantile) ? nullptr : "the quantile must be finite with 0 < q < 1";
+    if (const int rc = check_pixel_output(a, c.name, c.depth_q && !c.out_depth_q_pos, "null out_depth_q_pos", bad_q,
+                                          "ray depth"))
+      return rc;
+  }
   if (c.depth_q) {
     const char* bad_q = quantile_ok(c.quantile) ? nullptr : "the quantile must be finite with 0 < q < 1";
     if (const int rc = check_pixel_output(a, c.name, !c.out_depth_q || !c.out_depth_q_pos,
@@ -526,7 +564,8 @@ int rasterize_forward(const sfgs_forward_args* a, const FwdCall& c) {
 
     if (P > 0) {
       PROF_BEGIN(ST_PREPROCESS);
-      sfgs_launch_preprocess(a, g, im, b, (unsigned long long)capacity, focal_x, focal_y, c.tan_fov, c.ortho, st);
+      sfgs_launch_preprocess(a, g, im, b, (unsigned long long)capacity, focal_x, focal_y, c.tan_fov, c.ortho,
+                             c.ray_depth, st);
       PROF_END();
       STAGE_CHECK("preprocess");
     }
@@ -549,7 +588,7 @@ int rasterize_forward(const sfgs_forward_args* a, const FwdCall& c) {
     PROF_BEGIN(ST_RENDER_FWD);
     // t = 1 - q in float32: the transmittance the selected record crosses
     sfgs_launch_render_fwd(a, g, im, b, off, 1.0f - c.quantile, c.depth_q ? c.out_depth_q : nullptr, c.out_depth_q_pos,
-                           c.dist ? c.out_distortion : nullptr, c.out_distortion_state, st);
+                           c.dist ? c.out_distortion : nullptr, c.out_distortion_state, c.ray_depth, st);
     PROF_END();
     STAGE_CHECK("render_fwd");
     return SFGS_OK;
@@ -628,6 +667,11 @@ int check_pixel_output(const sfgs_backward_args* a, const BwdCall& c, bool null_
 int check_backward(const sfgs_backward_args* a, const BwdCall& c) {
   const auto reject = [&c](int code, const char* what) { return fail_in(c.name, code, what); };
   if (!a) return reject(SFGS_E_BADARG, "null args");
+  if (c.ray_depth) {
+    if (const int rc = check_pixel_output(a, c, c.depth_q && (!c.depth_q_pos || !c.dL_dpix_depth_q),
+                                          "null depth_q_pos or dL_dpix_depth_q", "ray depth"))
+      return rc;
+  }
   if (c.depth_q) {
     if (const int rc = check_pixel_output(a, c, !c.depth_q_pos || !c.dL_dpix_depth_q,
                                           "null depth_q_pos or dL_dpix_depth_q", "the depth quantile"))
@@ -784,8 +828,10 @@ int rasterize_backward(const sfgs_backward_args* a, const BwdCall& c) {
     if (R > 0) {   // graph: R is the capacity (> 0), so the adjoint always runs
       PROF_BEGIN(ST_RENDER_BWD);
       sfgs_launch_render_bwd(a, g, im, b, acc, order.part, order.written, off, graph,
-                             c.dist ? c.distortion_state : nullptr, c.dL_dpix_distortion, st);
-      if (c.depth_q) sfgs_launch_depth_q_adjoint(a, im, b, c.depth_q_pos, c.dL_dpix_depth_q, acc, order.part, st);
+                             c.dist ? c.distortion_state : nullptr, c.dL_dpix_distortion, c.ray_depth, st);
+      if (c.depth_q)
+        sfgs_launch_depth_q_adjoint(a, g, im, b, c.depth_q_pos, c.dL_dpix_depth_q, acc, order.part, c.ray_depth, off,
+                                    st);
       PROF_END();
       STAGE_CHECK("render_bwd");
     }
@@ -809,8 +855,9 @@ int rasterize_backward(const sfgs_backward_args* a, const BwdCall& c) {
     if (a->R > 0 || graph) {
       PROF_BEGIN(ST_RENDER_BWD);
       sfgs_launch_render_bwd(a, g, im, b, acc, nullptr, nullptr, off, graph, c.dist ? c.distortion_state : nullptr,
-                             c.dL_dpix_distortion, st);
-      if (c.depth_q) sfgs_launch_depth_q_adjoint(a, im, b, c.depth_q_pos, c.dL_dpix_depth_q, acc, nullptr, st);
+                             c.dL_dpix_distortion, c.ray_depth, st);
+      if (c.depth_q)
+        sfgs_launch_depth_q_adjoint(a, g, im, b, c.depth_q_pos, c.dL_dpix_depth_q, acc, nullptr, c.ray_depth, off, st);
       PROF_END();
       STAGE_CHECK("render_bwd");
     }
@@ -818,7 +865,7 @@ int rasterize_backward(const sfgs_backward_args* a, const BwdCall& c) {
   if (do_gauss) {
     PROF_BEGIN(ST_GAUSS_BWD);
     sfgs_launch_gauss_bwd(a, g, focal_x, focal_y, acc, g_begin, g_end, phase == 2 ? g_begin : 0, cam_part, ncam,
-                          c.tan_fov, c.ortho, st);
+                          c.tan_fov, c.ortho, c.ray_depth, st);
     if (dL_dcamera) sfgs_launch_camera_reduce(P, ncam, cam_part, dL_dcamera, st);
     // an empty slice has no spans: the reduction writes zeros
     if (dL_dcamera_partial) sfgs_launch_camera_partial_reduce(g_end - g_begin, ncam, cam_part, dL_dcamera_partial, st);

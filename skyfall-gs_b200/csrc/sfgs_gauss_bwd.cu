@@ -104,13 +104,20 @@ __device__ __forceinline__ float3 dnormvdv3(float3 v, float3 dv) {
 // J = [[h_x, 0, 0], [0, h_y, 0]], which contributes no dL/dt; the projected centre [m, 1]·proj has no divide, so
 // dL/dm = proj rows 0-1 times dL/dndc; the SH view direction is the view's +z axis (view[2], view[6], view[10]) and has
 // no dL/dm term.  The depth term is the perspective one.  Only with NCAM == 0.
-template <int NCAM, bool ORTHO, class SH>
+// RAYD: ray depth (sfgs_rasterize_backward_ray_depth).  The record's depth slope g = C s (rec3.zw; C the conic,
+// s = (w3^T Sigma T0^T, w3^T Sigma T1^T), w3 = (view[2], view[6], view[10])) moves its depth at pixel p by g . (p - mu):
+// dL/dmu = -g A0.w joins dL/dmean2D[0:2] (as dL/dndc: times W/2, H/2), and dL/dg = A3.zw goes down the chain:
+// dL/ds = C dL/dg; the conic cotangent gains (s0 gx, (s1 gx + s0 gy) / 2, s1 gy) (words 10-12 hold half the
+// off-diagonal derivative) before the conic -> cov2D chain; dL/dSigma gains sym(w3 (dL/ds T)) and dL/dT gains
+// dL/ds (Sigma w3), which reach cov3D, scales, rotations, t, means3D and the focal terms; w3 itself gives direct
+// viewmatrix terms.  C is formed again from the 2D covariance (the stage holds record words 4-15 only).
+template <int NCAM, bool ORTHO, bool RAYD, class SH>
 __device__ __forceinline__ void gauss_adjoint(
     int D, float mx, float my, float mz, bool has_scales, float4 q_in, float scx, float scy, float scz,
     float scale_modifier, bool has_sh, unsigned cm, SH sh, const float* cov3D, bool norm_precomp, float4 A0,
     float4 A1, float4 A2, float4 A3, float4 rec1, float4 rec2, float4 rec3, const float* __restrict__ view,
     const float* __restrict__ proj, float h_x, float h_y, float tan_fovx, float tan_fovy, float kernel_size,
-    const float* __restrict__ campos, float (&out)[GB_ROW], float (&cam)[GB_CAM]) {
+    const float* __restrict__ campos, float (&out)[GB_ROW], float (&cam)[GB_CAM], int W, int H) {
   if constexpr (NCAM > 0) {
 #pragma unroll
     for (int j = 0; j < NCAM; j++) cam[j] = 0.f;
@@ -132,7 +139,7 @@ __device__ __forceinline__ void gauss_adjoint(
 
   // ---------------- conic -> cov2D -> cov3D, t (computeCov2DCUDA) ----------------
   {
-    const float dLcx = o_conic[0], dLcy = o_conic[1], dLcz = o_conic[3];
+    float dLcx = o_conic[0], dLcy = o_conic[1], dLcz = o_conic[3];
     float tx = view[0] * mx + view[4] * my + view[8] * mz + view[12];
     float ty = view[1] * mx + view[5] * my + view[9] * mz + view[13];
     const float tz = view[2] * mx + view[6] * my + view[10] * mz + view[14];
@@ -180,6 +187,22 @@ __device__ __forceinline__ void gauss_adjoint(
 
     const float a = c00 + kernel_size, b = c01, c = c11 + kernel_size;
     const float denom = a * c - b * b;
+    // RAYD: dL/ds and w3, and the conic cotangent of g = C s
+    float dLds0 = 0.f, dLds1 = 0.f;
+    const float w3[3] = {view[2], view[6], view[10]};
+    if constexpr (RAYD) {
+      const float s0 = w3[0] * X[0][0] + w3[1] * X[1][0] + w3[2] * X[2][0];
+      const float s1 = w3[0] * X[0][1] + w3[1] * X[1][1] + w3[2] * X[2][1];
+      const float inv = 1.f / denom;
+      const float Cx = c * inv, Cy = -b * inv, Cz = a * inv;
+      const float dgx = A3.z, dgy = A3.w;
+      dLds0 = Cx * dgx + Cy * dgy;
+      dLds1 = Cy * dgx + Cz * dgy;
+      dLcx += s0 * dgx;
+      dLcy += 0.5f * (s1 * dgx + s0 * dgy);
+      dLcz += s1 * dgy;
+      o_conic[0] = dLcx; o_conic[1] = dLcy; o_conic[3] = dLcz;
+    }
     float dL_da = 0, dL_db = 0, dL_dc = 0;
     const float denom2inv = 1.0f / ((denom * denom) + 0.0000001f);
     if (denom2inv != 0) {
@@ -199,19 +222,39 @@ __device__ __forceinline__ void gauss_adjoint(
       o_cov[2] = 2 * T[0][0] * T[0][2] * dL_da + (T[0][0] * T[1][2] + T[0][2] * T[1][0]) * dL_db + 2 * T[1][0] * T[1][2] * dL_dc;
       o_cov[4] = 2 * T[0][2] * T[0][1] * dL_da + (T[0][1] * T[1][2] + T[0][2] * T[1][1]) * dL_db + 2 * T[1][1] * T[1][2] * dL_dc;
     }
+    // RAYD: u = dL/ds T; dL/dSigma += sym(w3 u^T) (o_cov holds the full derivative of each off-diagonal element)
+    float u[3] = {0.f, 0.f, 0.f};
+    if constexpr (RAYD) {
+#pragma unroll
+      for (int r = 0; r < 3; r++) u[r] = dLds0 * T[0][r] + dLds1 * T[1][r];
+      o_cov[0] += w3[0] * u[0];
+      o_cov[1] += w3[0] * u[1] + w3[1] * u[0];
+      o_cov[2] += w3[0] * u[2] + w3[2] * u[0];
+      o_cov[3] += w3[1] * u[1];
+      o_cov[4] += w3[1] * u[2] + w3[2] * u[1];
+      o_cov[5] += w3[2] * u[2];
+    }
     // dL/dT (upper 2x3), dL/dJ, dL/dt
-    const float dL_dT00 = 2 * (T[0][0] * Vrk[0][0] + T[0][1] * Vrk[0][1] + T[0][2] * Vrk[0][2]) * dL_da +
+    float dL_dT00 = 2 * (T[0][0] * Vrk[0][0] + T[0][1] * Vrk[0][1] + T[0][2] * Vrk[0][2]) * dL_da +
                           (T[1][0] * Vrk[0][0] + T[1][1] * Vrk[0][1] + T[1][2] * Vrk[0][2]) * dL_db;
-    const float dL_dT01 = 2 * (T[0][0] * Vrk[1][0] + T[0][1] * Vrk[1][1] + T[0][2] * Vrk[1][2]) * dL_da +
+    float dL_dT01 = 2 * (T[0][0] * Vrk[1][0] + T[0][1] * Vrk[1][1] + T[0][2] * Vrk[1][2]) * dL_da +
                           (T[1][0] * Vrk[1][0] + T[1][1] * Vrk[1][1] + T[1][2] * Vrk[1][2]) * dL_db;
-    const float dL_dT02 = 2 * (T[0][0] * Vrk[2][0] + T[0][1] * Vrk[2][1] + T[0][2] * Vrk[2][2]) * dL_da +
+    float dL_dT02 = 2 * (T[0][0] * Vrk[2][0] + T[0][1] * Vrk[2][1] + T[0][2] * Vrk[2][2]) * dL_da +
                           (T[1][0] * Vrk[2][0] + T[1][1] * Vrk[2][1] + T[1][2] * Vrk[2][2]) * dL_db;
-    const float dL_dT10 = 2 * (T[1][0] * Vrk[0][0] + T[1][1] * Vrk[0][1] + T[1][2] * Vrk[0][2]) * dL_dc +
+    float dL_dT10 = 2 * (T[1][0] * Vrk[0][0] + T[1][1] * Vrk[0][1] + T[1][2] * Vrk[0][2]) * dL_dc +
                           (T[0][0] * Vrk[0][0] + T[0][1] * Vrk[0][1] + T[0][2] * Vrk[0][2]) * dL_db;
-    const float dL_dT11 = 2 * (T[1][0] * Vrk[1][0] + T[1][1] * Vrk[1][1] + T[1][2] * Vrk[1][2]) * dL_dc +
+    float dL_dT11 = 2 * (T[1][0] * Vrk[1][0] + T[1][1] * Vrk[1][1] + T[1][2] * Vrk[1][2]) * dL_dc +
                           (T[0][0] * Vrk[1][0] + T[0][1] * Vrk[1][1] + T[0][2] * Vrk[1][2]) * dL_db;
-    const float dL_dT12 = 2 * (T[1][0] * Vrk[2][0] + T[1][1] * Vrk[2][1] + T[1][2] * Vrk[2][2]) * dL_dc +
+    float dL_dT12 = 2 * (T[1][0] * Vrk[2][0] + T[1][1] * Vrk[2][1] + T[1][2] * Vrk[2][2]) * dL_dc +
                           (T[0][0] * Vrk[2][0] + T[0][1] * Vrk[2][1] + T[0][2] * Vrk[2][2]) * dL_db;
+    if constexpr (RAYD) {
+      // dL/dT_i += dL/ds_i (Sigma w3)
+      float v[3];
+#pragma unroll
+      for (int r = 0; r < 3; r++) v[r] = Vrk[r][0] * w3[0] + Vrk[r][1] * w3[1] + Vrk[r][2] * w3[2];
+      dL_dT00 += dLds0 * v[0]; dL_dT01 += dLds0 * v[1]; dL_dT02 += dLds0 * v[2];
+      dL_dT10 += dLds1 * v[0]; dL_dT11 += dLds1 * v[1]; dL_dT12 += dLds1 * v[2];
+    }
     const float dL_dJ00 = Wm[0][0] * dL_dT00 + Wm[0][1] * dL_dT01 + Wm[0][2] * dL_dT02;
     const float dL_dJ02 = Wm[2][0] * dL_dT00 + Wm[2][1] * dL_dT01 + Wm[2][2] * dL_dT02;
     const float dL_dJ11 = Wm[1][0] * dL_dT10 + Wm[1][1] * dL_dT11 + Wm[1][2] * dL_dT12;
@@ -244,6 +287,11 @@ __device__ __forceinline__ void gauss_adjoint(
         cam[C_VIEW + 4 * r + 1] += b1 * dT1[r];
         cam[C_VIEW + 4 * r + 2] += a2 * dT0[r] + b2 * dT1[r];
       }
+      if constexpr (RAYD) {
+        // s_i = w3^T Sigma T_i^T: dL/dw3 = Sigma u
+#pragma unroll
+        for (int k = 0; k < 3; k++) cam[C_VIEW + 4 * k + 2] += Vrk[k][0] * u[0] + Vrk[k][1] * u[1] + Vrk[k][2] * u[2];
+      }
     }
     if constexpr (NCAM > C_TANY) {
       // The focal terms.  h = W / (2 tan) enters J00 = h_x / tz and J02 = -h_x tx / tz^2 (tx the clamped t_x), so
@@ -268,6 +316,11 @@ __device__ __forceinline__ void gauss_adjoint(
     const float m_w = 1.0f / (hw + 0.0000001f);
     const float mul1 = (proj[0] * mx + proj[4] * my + proj[8] * mz + proj[12]) * m_w * m_w;
     const float mul2 = (proj[1] * mx + proj[5] * my + proj[9] * mz + proj[13]) * m_w * m_w;
+    if constexpr (RAYD) {
+      // dL/dmu = -g dL/dz, as dL/dndc (dpix/dndc = W/2, H/2); the abs channel o_mean2D[2] is left as it is
+      o_mean2D[0] -= rec3.z * A0.w * (0.5f * W);
+      o_mean2D[1] -= rec3.w * A0.w * (0.5f * H);
+    }
     const float gx = o_mean2D[0], gy = o_mean2D[1];
     // ORTHO: ndc = ([m, 1]·proj).xy, no divide
     const float d0 = ORTHO ? proj[0] * gx + proj[1] * gy
@@ -518,8 +571,9 @@ static_assert(sizeof(float) * (GB_CAM_STAGE + GB_CAM * GB_SLOTS) <= sizeof(GbInp
 // from device memory and the focal lengths are formed from it as the host forms them (W / (2 tan_fovx),
 // H / (2 tan_fovy)), as in preprocess_kernel<DEV_FOV>.  A trailing parameter an instantiation does not read costs
 // nothing, and new parameters go at the end of the list.  ORTHO: the orthographic camera's adjoint (gauss_adjoint); only
-// <0, false, true> is instantiated.
-template <int NCAM, bool DEV_FOV, bool ORTHO>
+// <0, false, true> is instantiated.  RAYD: ray depth (gauss_adjoint), with host intrinsics: <0 | 35 | 37, false, false,
+// true> and <0, false, true, true>.
+template <int NCAM, bool DEV_FOV, bool ORTHO, bool RAYD = false>
 __global__ void __launch_bounds__(GB_THREADS, GB_CTAS_PER_SM)
 gauss_bwd_kernel(int g_begin, int g_end, int spans_per_cta, int acc_row0, int D, int M,
                  const float* __restrict__ means3D, const int* __restrict__ radii, const float* __restrict__ shs,
@@ -655,14 +709,14 @@ gauss_bwd_kernel(int g_begin, int g_end, int spans_per_cta, int acc_row0, int D,
       const float* shk = reinterpret_cast<const float*>(&in.sh[0][k]);   // float j at word (j >> 2) * 4 * SLOTS + (j & 3)
       const float cov3D[6] = {in.cov[0][k], in.cov[1][k], in.cov[2][k], in.cov[3][k], in.cov[4][k], in.cov[5][k]};
       const unsigned cm = has_sh ? (in.clamped[k] >> (8 * (S.gidx[b][k] & 3))) & 0xffu : 0u;
-      gauss_adjoint<NCAM, ORTHO>(D, in.mean[0][k], in.mean[1][k], in.mean[2][k], has_scales,
+      gauss_adjoint<NCAM, ORTHO, RAYD>(D, in.mean[0][k], in.mean[1][k], in.mean[2][k], has_scales,
                     has_scales ? in.rot[k] : make_float4(0.f, 0.f, 0.f, 0.f),
                     has_scales ? in.scale[0][k] : 0.f, has_scales ? in.scale[1][k] : 0.f,
                     has_scales ? in.scale[2][k] : 0.f, scale_modifier, has_sh, cm,
                     [&](int j) { return shk[(j >> 2) * (4 * GB_SLOTS) + (j & 3)]; }, cov3D,
                     norm3D_precomp != nullptr, in.acc[0][k], in.acc[1][k], in.acc[2][k], in.acc[3][k],
                     in.rec[0][k], in.rec[1][k], in.rec[2][k], view, proj, h_x, h_y, tan_fovx, tan_fovy,
-                    kernel_size, campos, o, cam);
+                    kernel_size, campos, o, cam, W, H);
     }
     // ---------------- epilogue, span by span: stage the span's outputs, then write each output's range once ----------
     // Staged over the consumed inputs: the dL_dsh factor rows, then one image per fixed-width array laid out as its
@@ -808,14 +862,19 @@ void sfgs_launch_camera_partial_reduce(int n, int ncam, const double* cam_part, 
 // tan_fov: NULL (the launch parameters a->tan_fovx / a->tan_fovy, focal_x, focal_y are used) or DEVICE float [2], read
 // by the kernel (DEV_FOV)
 // ortho: the orthographic adjoint (focal_x / focal_y are its pixel scales); cam_part and tan_fov are then NULL
+// ray_depth: the ray-depth adjoint (tan_fov NULL)
 void sfgs_launch_gauss_bwd(const sfgs_backward_args* a, const GeomLayout& g, float focal_x, float focal_y,
                            const float* acc, int g_begin, int g_end, int acc_row0, double* cam_part, int ncam,
-                           const float* tan_fov, bool ortho, cudaStream_t st) {
+                           const float* tan_fov, bool ortho, bool ray_depth, cudaStream_t st) {
   if (g_end <= g_begin) return;
   const bool dev_fov = tan_fov != nullptr;
   const size_t smem = sizeof(GbShared);
   const auto kernel =
-      ortho               ? sfgs_smem_kernel<gauss_bwd_kernel<0, false, true>>(smem)
+      ray_depth ? (ortho                ? sfgs_smem_kernel<gauss_bwd_kernel<0, false, true, true>>(smem)
+                   : cam_part == nullptr ? sfgs_smem_kernel<gauss_bwd_kernel<0, false, false, true>>(smem)
+                   : ncam == GB_CAM      ? sfgs_smem_kernel<gauss_bwd_kernel<GB_CAM, false, false, true>>(smem)
+                                         : sfgs_smem_kernel<gauss_bwd_kernel<GB_CAM_POSE, false, false, true>>(smem))
+      : ortho               ? sfgs_smem_kernel<gauss_bwd_kernel<0, false, true>>(smem)
       : cam_part == nullptr ? (dev_fov ? sfgs_smem_kernel<gauss_bwd_kernel<0, true, false>>(smem)
                                        : sfgs_smem_kernel<gauss_bwd_kernel<0, false, false>>(smem))
       : ncam == GB_CAM    ? (dev_fov ? sfgs_smem_kernel<gauss_bwd_kernel<GB_CAM, true, false>>(smem)

@@ -88,11 +88,14 @@ __device__ __forceinline__ void normal_from_scale_rot(float sx, float sy, float 
 // Mirrors computeCov2D, forward.cu:74-124. Returns (cov00+k, cov01, cov11+k, coef).
 // ORTHO: the orthographic camera's constant Jacobian J = [[h_x, 0, 0], [0, h_y, 0]] (focal_x / focal_y carry the pixel
 // scales h = W / (2 s)): no clamp and no t dependence; everything after J is the perspective code.
-template <bool ORTHO>
+// RAYD: also s = (w3^T Sigma T0^T, w3^T Sigma T1^T) into *s_out, w3 = (vm[2], vm[6], vm[10]) the view's depth row: the
+// covariance of view depth with the two pixel coordinates, from the products X = T Sigma the 2D covariance is formed of.
+template <bool ORTHO, bool RAYD = false>
 __device__ __forceinline__ float4 cov2d_project(float mx, float my, float mz,
                                                 float focal_x, float focal_y,
                                                 float tan_fovx, float tan_fovy, float kernel_size,
-                                                const Sym3& V, const float* __restrict__ vm) {
+                                                const Sym3& V, const float* __restrict__ vm,
+                                                float2* s_out = nullptr) {
   float a0, a2, b1, b2;   // J columns: (a0, 0, a2), (0, b1, b2), 0
   if constexpr (ORTHO) {
     a0 = focal_x; a2 = 0.0f; b1 = focal_y; b2 = 0.0f;
@@ -132,6 +135,8 @@ __device__ __forceinline__ float4 cov2d_project(float mx, float my, float mz,
   float c00 = X0[0] * T0[0] + X0[1] * T0[1] + X0[2] * T0[2];
   float c01 = X1[0] * T0[0] + X1[1] * T0[1] + X1[2] * T0[2];
   float c11 = X1[0] * T1[0] + X1[1] * T1[1] + X1[2] * T1[2];
+  if constexpr (RAYD)
+    *s_out = make_float2(vm[2] * X0[0] + vm[6] * X0[1] + vm[10] * X0[2], vm[2] * X1[0] + vm[6] * X1[1] + vm[10] * X1[2]);
 
   const float det_0 = fmax(1e-6, (double)(c00 * c11 - c01 * c01));
   const float det_1 = fmax(1e-6, (double)((c00 + kernel_size) * (c11 + kernel_size) - c01 * c01));
@@ -219,7 +224,10 @@ __device__ __forceinline__ float radius_bound(float trace_sigma, float view_z, f
 // with no divide; J is constant (cov2d_project<true>), so the cull bound has no 1 / t_z^2; and the view direction of SH
 // and of the normal's sign flip is the view's +z axis in world space, (vm[2], vm[6], vm[10]), for every Gaussian, in
 // place of m - campos.  cam_pos is not read.  Only <false, true> is instantiated.
-template <bool DEV_FOV, bool ORTHO>
+// RAYD: ray depth (sfgs_rasterize_forward_ray_depth).  Record words 14-15 get the depth slope g = C s in depth units
+// per pixel, C = (con.x, con.y, con.z) the record's conic and s from cov2d_project<ORTHO, true>; without it they are
+// 0.  Nothing else changes.  Instantiated with host intrinsics only.
+template <bool DEV_FOV, bool ORTHO, bool RAYD = false>
 __global__ void __launch_bounds__(PRE_THREADS, 3)
 preprocess_kernel(int P, int D, int M,
                   const float* __restrict__ means3D, const float* __restrict__ scales, float scale_modifier,
@@ -368,6 +376,7 @@ preprocess_kernel(int P, int D, int M,
     float px = 0.f, py = 0.f, pz = 0.f, sx = 0.f, sy = 0.f, sz = 0.f, opac_in = 0.f;
     float4 q = make_float4(0.f, 0.f, 0.f, 0.f);
     float g_pix_x = 0.f, g_pix_y = 0.f, g_conx = 0.f, g_cony = 0.f, g_conz = 0.f, g_coef = 0.f;
+    float g_slx = 0.f, g_sly = 0.f;      // RAYD: the depth slope
     Sym3 g_V = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
 
     if (in_range) {
@@ -406,7 +415,9 @@ preprocess_kernel(int P, int D, int M,
           V = cov3d_from_scale_rot(sx, sy, sz, scale_modifier, q.x, q.y, q.z, q.w);
         }
 
-        const float4 cov = cov2d_project<ORTHO>(px, py, pz, focal_x, focal_y, tan_fovx, tan_fovy, kernel_size, V, vm);
+        float2 s = make_float2(0.f, 0.f);
+        const float4 cov =
+            cov2d_project<ORTHO, RAYD>(px, py, pz, focal_x, focal_y, tan_fovx, tan_fovy, kernel_size, V, vm, &s);
         const float det = (cov.x * cov.z - cov.y * cov.y);
         if (det != 0.0f) {
           const float det_inv = 1.f / det;
@@ -427,6 +438,10 @@ preprocess_kernel(int P, int D, int M,
             visible = true;
             g_pix_x = pix_x; g_pix_y = pix_y; g_conx = conx; g_cony = cony; g_conz = conz; g_coef = cov.w;
             g_V = V;
+            if constexpr (RAYD) {
+              g_slx = s.x * conx + s.y * cony;
+              g_sly = s.x * cony + s.y * conz;
+            }
             out_radius = iradius;
             out_tiles = ntiles;
             vis_rect = rb;
@@ -481,7 +496,7 @@ preprocess_kernel(int P, int D, int M,
         o[0] = make_float4(g_pix_x, g_pix_y, g_conx, g_cony);
         o[1] = make_float4(g_conz, opac_in * g_coef, vis_depth, 0.f);
         o[2] = make_float4(rgb[0], rgb[1], rgb[2], n[0]);
-        o[3] = make_float4(n[1], n[2], 0.f, 0.f);
+        o[3] = make_float4(n[1], n[2], RAYD ? g_slx : 0.f, RAYD ? g_sly : 0.f);
       }
       radii[idx] = out_radius;
       tiles_touched[idx] = out_tiles;
@@ -533,7 +548,7 @@ __global__ void mark_visible_kernel(int P, const float* __restrict__ means3D,
 
 void sfgs_launch_preprocess(const sfgs_forward_args* a, const GeomLayout& g, const ImageLayout& im,
                             const BinningLayout& b, unsigned long long capacity, float focal_x, float focal_y,
-                            const float* tan_fov, bool ortho, cudaStream_t st) {
+                            const float* tan_fov, bool ortho, bool ray_depth, cudaStream_t st) {
   const int blocks = (a->P + PRE_SPAN - 1) / PRE_SPAN;
   constexpr size_t smem = PRE_THREADS * (12 * sizeof(float4) + sizeof(uint32_t) + sizeof(int4) + sizeof(uint32_t)) +
                           PRE_SPAN * sizeof(unsigned short);
@@ -542,12 +557,16 @@ void sfgs_launch_preprocess(const sfgs_forward_args* a, const GeomLayout& g, con
     cudaFuncSetAttribute(preprocess_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     cudaFuncSetAttribute(preprocess_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     cudaFuncSetAttribute(preprocess_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(preprocess_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(preprocess_kernel<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   }
   const SfgsBand band = sfgs_band(a->tile_row_begin, a->tile_row_end, im.tiles_y);
   const int band0 = band.b0, band1 = band.b1;
   SFGS_COUNT_LAUNCH();
-  // ortho: tan_fov is NULL (the orthographic entries take the intrinsics as launch parameters)
-  const auto kernel = ortho ? preprocess_kernel<false, true>
+  // ortho: tan_fov is NULL (the orthographic entries take the intrinsics as launch parameters); ray depth: likewise
+  // (its entries are not capturable)
+  const auto kernel = ray_depth ? (ortho ? preprocess_kernel<false, true, true> : preprocess_kernel<false, false, true>)
+                      : ortho   ? preprocess_kernel<false, true>
                       : tan_fov != nullptr ? preprocess_kernel<true, false> : preprocess_kernel<false, false>;
   kernel<<<blocks, PRE_THREADS, smem, st>>>(
       a->P, a->D, a->M, a->means3D, a->scales, a->scale_modifier, a->rotations, a->opacities, a->shs,

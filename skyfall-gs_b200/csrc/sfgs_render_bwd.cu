@@ -92,7 +92,12 @@ struct WarpSmemDist : Base {
 // it to every alpha -- the M2 term is the same for every record and joins the alpha cotangent, the other is formed per
 // slot from (2 c A, mu) in the warp's table `dist`; dR/dm_i = 2 A w_i (m_i - mu) joins the depth word (3) of phase 2,
 // formed per (pixel, slot) as the difference m_i - mu.  With c = 0 every sum is what it is without the option.
-template <bool PEER, bool HAS_EXTRA, bool ORDERED, bool JITTER, bool DIST>
+// RAYD: ray depth (sfgs_rasterize_backward_ray_depth).  Phase 1 takes the record's depth at the pixel's sample
+// position, d(p) = z + g . (p - mu) (g: the slope words, staged in quad [3].zw), as the depth attribute of g; phase 2
+// adds the sums of w c (p - mu) over the record's pixels (c the pixel's depth cotangent), formed against the pixels'
+// offsets from the half's centre and shifted to the record's centre by the expansion of the h-moments, into the free
+// words 14-15.  Word 3 still sums w c.  With c = 0 every sum is what it is without the option.
+template <bool PEER, bool HAS_EXTRA, bool ORDERED, bool JITTER, bool DIST, bool RAYD>
 __device__ __forceinline__ void
 render_bwd_warp(const uint2* __restrict__ ranges, const char* __restrict__ binning_base,
                 const uint32_t* __restrict__ hdr, int W, int H, int band0,
@@ -239,6 +244,7 @@ render_bwd_warp(const uint2* __restrict__ ranges, const char* __restrict__ binni
     float s0 = 0, s1 = 0, s2 = 0, s3 = 0, s4 = 0, s5 = 0, s6 = 0;      // sum w * dL/dpix_c
     float sab = 0;
     float sh, shx, shy, shxx, shxy, shyy;     // sums of h * {1, dx, dy, dx^2, dx dy, dy^2} over the half
+    float sdx = 0, sdy = 0;                   // RAYD: sums of w c * {x, y} over the half (c: the depth cotangent)
     if constexpr (JITTER) {
       // pixel i samples at (x, y) = its sample position - the half's centre (exact: the two are close), i.e. its
       // compile-time offset plus its own subpixel offset: the sums of h * {1, x, y, x^2, x y, y^2} run over those, the
@@ -256,6 +262,10 @@ render_bwd_warp(const uint2* __restrict__ ranges, const char* __restrict__ binni
         s0 = fmaf(wh.x, p0.x, s0); s1 = fmaf(wh.x, p0.y, s1); s2 = fmaf(wh.x, p0.z, s2);
         s3 = fmaf(wh.x, dLd_of(i, p0.w), s3);
         s4 = fmaf(wh.x, p1.x, s4); s5 = fmaf(wh.x, p1.y, s5); s6 = fmaf(wh.x, p1.z, s6);
+        if constexpr (RAYD) {
+          const float wc = wh.x * p0.w;
+          sdx = fmaf(wc, x, sdx); sdy = fmaf(wc, y, sdy);
+        }
         const float hx = wh.y * x, hy = wh.y * y;
         sh += wh.y;
         sx += hx; sy += hy;
@@ -278,6 +288,10 @@ render_bwd_warp(const uint2* __restrict__ ranges, const char* __restrict__ binni
         s0 = fmaf(wh.x, p0.x, s0); s1 = fmaf(wh.x, p0.y, s1); s2 = fmaf(wh.x, p0.z, s2);
         s3 = fmaf(wh.x, dLd_of(i, p0.w), s3);
         s4 = fmaf(wh.x, p1.x, s4); s5 = fmaf(wh.x, p1.y, s5); s6 = fmaf(wh.x, p1.z, s6);
+        if constexpr (RAYD) {
+          const float wc = wh.x * p0.w;
+          sdx = fmaf(wc, x, sdx); sdy = fmaf(wc, r ? 0.5f : -0.5f, sdy);
+        }
         h1[r] += wh.y;
         hx[r] = fmaf(wh.y, x, hx[r]);
         sxx = fmaf(wh.y, x * x, sxx);
@@ -294,9 +308,16 @@ render_bwd_warp(const uint2* __restrict__ ranges, const char* __restrict__ binni
       shxy = fmaf(DX, shy, -fmaf(DY, sx, -sxy));
       shyy = fmaf(DY, shy, -fmaf(DY, sy, -syy));
     }
+    // RAYD: sum w c (p - mu) = sum w c (x - DX, y - DY) over the half, before the halves are added (DX, DY differ)
+    float e14 = 0.f, e15 = 0.f;
+    if constexpr (RAYD) {
+      e14 = fmaf(-DX, s3, sdx);
+      e15 = fmaf(-DY, s3, sdy);
+    }
 #define XH(v) v += __shfl_xor_sync(0xffffffffu, v, 16)
     XH(s0); XH(s1); XH(s2); XH(s3); XH(s4); XH(s5); XH(s6);
     XH(sh); XH(shx); XH(shy); XH(shxx); XH(shxy); XH(shyy); XH(sab);
+    if constexpr (RAYD) { XH(e14); XH(e15); }
 #undef XH
     if (ORDERED && have_rec) {
       const float o = rb.y;
@@ -308,7 +329,7 @@ render_bwd_warp(const uint2* __restrict__ ranges, const char* __restrict__ binni
         written[row] = 1;
       } else {
         dst[2] = make_float4(-o * fmaf(bv, shy, av * shx), fabsf(o) * sab, -0.5f * o * shxx, -0.5f * o * shxy);
-        dst[3] = make_float4(-0.5f * o * shyy, sh, 0.f, 0.f);
+        dst[3] = make_float4(-0.5f * o * shyy, sh, e14, e15);
       }
     } else if (have_rec) {
       const float o = rb.y;
@@ -325,7 +346,7 @@ render_bwd_warp(const uint2* __restrict__ ranges, const char* __restrict__ binni
       } else {
         red_add_v4<PEER>(dst + 8, make_float4(-o * fmaf(bv, shy, av * shx), fabsf(o) * sab,
                                               -0.5f * o * shxx, -0.5f * o * shxy));
-        red_add_v4<PEER>(dst + 12, make_float4(-0.5f * o * shyy, sh, 0.f, 0.f));
+        red_add_v4<PEER>(dst + 12, make_float4(-0.5f * o * shyy, sh, e14, e15));
       }
     }
     __syncwarp();
@@ -354,7 +375,7 @@ render_bwd_warp(const uint2* __restrict__ ranges, const char* __restrict__ binni
     float g = rc.x * dLc0, g2 = rc.w * dLn0;
     g += rc.y * dLc1; g2 += rd.x * dLn1;
     g += rc.z * dLc2; g2 += rd.y * dLn2;
-    g += rb.z * dLd;  g2 += dLa;
+    g += (RAYD ? fmaf(-rd.z, dx, fmaf(-rd.w, dy, rb.z)) : rb.z) * dLd;  g2 += dLa;
     g += g2;
     if constexpr (DIST) {
       const float dm = rb.z - dmu;
@@ -415,9 +436,11 @@ render_bwd_warp(const uint2* __restrict__ ranges, const char* __restrict__ binni
 // launched whatever the frame's instance count, so it first checks the forward's overflow flag -- after an overflow the
 // ranges run past the binning capacity and nothing may read point_list or write partial rows.
 // DIST (the depth distortion) is instantiated only without peers, extras and GUARDED, at two CTAs per SM: at the 80
-// registers of three its instantiations spilled (8 to 20 bytes).
-template <bool PEER, bool HAS_EXTRA, bool ORDERED, bool JITTER, bool GUARDED, bool DIST>
-__global__ void __launch_bounds__(BLEND_THREADS, DIST ? 2 : 3)
+// registers of three its instantiations spilled (8 to 20 bytes).  RAYD (ray depth) likewise without peers, extras,
+// GUARDED and DIST: at three CTAs per SM without jitter (80 registers, no spills) and at two with it (the two jitter
+// instantiations spilled 4 bytes at 80 registers).
+template <bool PEER, bool HAS_EXTRA, bool ORDERED, bool JITTER, bool GUARDED, bool DIST, bool RAYD = false>
+__global__ void __launch_bounds__(BLEND_THREADS, DIST || (RAYD && JITTER) ? 2 : 3)
 render_bwd_kernel(const uint2* __restrict__ ranges, const char* __restrict__ binning_base,
                   const uint32_t* __restrict__ hdr, int W, int H, int band0,
                   const float* __restrict__ bg_color, const float* __restrict__ rec,
@@ -430,7 +453,7 @@ render_bwd_kernel(const uint2* __restrict__ ranges, const char* __restrict__ bin
                   float* __restrict__ part, unsigned char* __restrict__ written, const float2* __restrict__ off,
                   const float* __restrict__ dist_state, const float* __restrict__ dL_dpix_dist) {
   if (GUARDED && hdr[HDR_OVERFLOW]) return;
-  render_bwd_warp<PEER, HAS_EXTRA, ORDERED, JITTER, DIST>(ranges, binning_base, hdr, W, H, band0, bg_color, rec,
+  render_bwd_warp<PEER, HAS_EXTRA, ORDERED, JITTER, DIST, RAYD>(ranges, binning_base, hdr, W, H, band0, bg_color, rec,
                                                           accum_alphas, n_contrib, dL_dpixels, dL_dpixel_depths,
                                                           dL_dpixel_norms, dL_dpixel_alphas, norm_raw, acc, peers,
                                                           extras, dL_dpixel_extras, dL_dextras, ED, part, written, off,
@@ -443,9 +466,9 @@ constexpr size_t render_bwd_smem() {
   return BLEND_WARPS * sizeof(std::conditional_t<DIST, WarpSmemDist<Base>, Base>);
 }
 
-template <bool PEER, bool HAS_EXTRA, bool ORDERED, bool JITTER, bool GUARDED, bool DIST = false>
+template <bool PEER, bool HAS_EXTRA, bool ORDERED, bool JITTER, bool GUARDED, bool DIST = false, bool RAYD = false>
 auto render_bwd_instance() {
-  return sfgs_smem_kernel<render_bwd_kernel<PEER, HAS_EXTRA, ORDERED, JITTER, GUARDED, DIST>>(
+  return sfgs_smem_kernel<render_bwd_kernel<PEER, HAS_EXTRA, ORDERED, JITTER, GUARDED, DIST, RAYD>>(
       render_bwd_smem<JITTER, DIST>());
 }
 
@@ -462,52 +485,83 @@ auto render_bwd_instance() {
 //            warp owns a row, so the sums stay bit-reproducible.
 // Kept out of render_bwd_kernel, which is bound by instruction issue at its register budget: this costs one launch and
 // 8 bytes read per pixel.
-template <bool ORDERED>
+// RAYD: ray depth, where depth_q = d_j(p) = z_j + g_j . (p - mu_j): each lane also forms c (p - mu_j) at its sample
+// position p (off: the forward's offsets, or NULL), and the group's first lane adds those in the same order into words
+// 14-15 (dL/dg) beside word 3; the dL/dmu = -g dL/dz part follows in the per-Gaussian adjoint.
+template <bool ORDERED, bool RAYD = false>
 __global__ void __launch_bounds__(BLEND_THREADS)
 depth_q_adjoint_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list, int W, int H,
                        int band0,
                        const uint32_t* __restrict__ depth_q_pos, const float* __restrict__ dL_dpix_depth_q,
-                       float* __restrict__ acc, float* __restrict__ part) {
+                       float* __restrict__ acc, float* __restrict__ part, const float* __restrict__ rec,
+                       const float2* __restrict__ off) {
   __shared__ float s_g[BLEND_WARPS][32];
+  __shared__ float2 s_gp[RAYD ? BLEND_WARPS : 1][32];
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   const BlendPixel px(band0, W, H, wid, lane);
   const uint32_t pos = px.inside ? depth_q_pos[px.id] : 0u;
   s_g[wid][lane] = px.inside ? dL_dpix_depth_q[px.id] : 0.f;
+  if constexpr (RAYD) {
+    float2 v = make_float2(0.f, 0.f);
+    if (pos != 0) {
+      const float* r = rec + (size_t)point_list[ranges[px.tile].x + pos - 1] * REC_FLOATS;
+      const float2 o = off != nullptr ? off[px.id] : make_float2(0.f, 0.f);
+      const float c = s_g[wid][lane];
+      v = make_float2(c * ((px.x + o.x) - r[0]), c * ((px.y + o.y) - r[1]));
+    }
+    s_gp[wid][lane] = v;
+  }
   const unsigned group = __match_any_sync(0xffffffffu, pos);
   __syncwarp();
   if (pos == 0 || lane != __ffs(group) - 1) return;
-  float s = 0.f;
-  for (unsigned m = group; m != 0; m &= m - 1) s += s_g[wid][__ffs(m) - 1];
+  float s = 0.f, sx = 0.f, sy = 0.f;
+  for (unsigned m = group; m != 0; m &= m - 1) {
+    s += s_g[wid][__ffs(m) - 1];
+    if constexpr (RAYD) { sx += s_gp[wid][__ffs(m) - 1].x; sy += s_gp[wid][__ffs(m) - 1].y; }
+  }
   const uint32_t inst = ranges[px.tile].x + pos - 1;
   if (ORDERED) {
     part[((size_t)inst * BLEND_WARPS + wid) * 16 + 3] += s;
+    if constexpr (RAYD) {
+      part[((size_t)inst * BLEND_WARPS + wid) * 16 + 14] += sx;
+      part[((size_t)inst * BLEND_WARPS + wid) * 16 + 15] += sy;
+    }
   } else {
     float* dst = acc + (size_t)point_list[inst] * 16 + 3;
     asm volatile("red.global.add.f32 [%0], %1;\n" ::"l"(dst), "f"(s) : "memory");
+    if constexpr (RAYD) {
+      asm volatile("red.global.add.f32 [%0], %1;\n" ::"l"(dst + 11), "f"(sx) : "memory");
+      asm volatile("red.global.add.f32 [%0], %1;\n" ::"l"(dst + 12), "f"(sy) : "memory");
+    }
   }
 }
 
 }  // namespace
 
-// After the blend adjoint: part != NULL for the ORDERED (deterministic) backward, whose partial rows it updates
-void sfgs_launch_depth_q_adjoint(const sfgs_backward_args* a, const ImageLayout& im, const BinningLayout& b,
-                                 const uint32_t* depth_q_pos, const float* dL_dpix_depth_q, float* acc, float* part,
-                                 cudaStream_t st) {
+// After the blend adjoint: part != NULL for the ORDERED (deterministic) backward, whose partial rows it updates;
+// ray_depth: the ray-depth form, which reads the records and the offsets (off, or NULL)
+void sfgs_launch_depth_q_adjoint(const sfgs_backward_args* a, const GeomLayout& g, const ImageLayout& im,
+                                 const BinningLayout& b, const uint32_t* depth_q_pos, const float* dL_dpix_depth_q,
+                                 float* acc, float* part, bool ray_depth, const float* off, cudaStream_t st) {
   dim3 grid;
   int band0;
   if (!blend_grid(a->tile_row_begin, a->tile_row_end, im, grid, band0)) return;
-  const auto kernel = part != nullptr ? depth_q_adjoint_kernel<true> : depth_q_adjoint_kernel<false>;
+  const auto kernel = ray_depth ? (part != nullptr ? depth_q_adjoint_kernel<true, true>
+                                                   : depth_q_adjoint_kernel<false, true>)
+                      : part != nullptr ? depth_q_adjoint_kernel<true> : depth_q_adjoint_kernel<false>;
   SFGS_COUNT_LAUNCH();
   kernel<<<grid, BLEND_THREADS, 0, st>>>(im.ranges, b.point_list, a->width, a->height, band0, depth_q_pos,
-                                         dL_dpix_depth_q, acc, part);
+                                         dL_dpix_depth_q, acc, part, g.rec, reinterpret_cast<const float2*>(off));
 }
 
 // guarded: the graph backward's blend adjoint.  The entry points' checks leave these combinations: peers only in the
 // eager non-deterministic backward; extra_attrs only without offsets and without the ordered form (part != nullptr);
-// the depth distortion (dist_state != nullptr) only eager, without peers and extra_attrs.
+// the depth distortion (dist_state != nullptr) and ray depth (ray_depth) only eager, without peers and extra_attrs,
+// and not together.
 void sfgs_launch_render_bwd(const sfgs_backward_args* a, const GeomLayout& g, const ImageLayout& im,
                             const BinningLayout& b, float* acc, float* part, unsigned char* written, const float* off,
-                            bool guarded, const float* dist_state, const float* dL_dpix_dist, cudaStream_t st) {
+                            bool guarded, const float* dist_state, const float* dL_dpix_dist, bool ray_depth,
+                            cudaStream_t st) {
   dim3 grid;
   int band0;
   if (!blend_grid(a->tile_row_begin, a->tile_row_end, im, grid, band0)) return;
@@ -520,7 +574,11 @@ void sfgs_launch_render_bwd(const sfgs_backward_args* a, const GeomLayout& g, co
   const bool ordered = part != nullptr, extra = a->ED > 0, dist = dist_state != nullptr;
   // render_bwd_instance<PEER, HAS_EXTRA, ORDERED, JITTER, GUARDED[, DIST]>
   const auto kernel =
-      dist ? (off != nullptr ? (ordered ? render_bwd_instance<false, false, true, true, false, true>()
+      ray_depth ? (off != nullptr ? (ordered ? render_bwd_instance<false, false, true, true, false, false, true>()
+                                             : render_bwd_instance<false, false, false, true, false, false, true>())
+                   : ordered      ? render_bwd_instance<false, false, true, false, false, false, true>()
+                                  : render_bwd_instance<false, false, false, false, false, false, true>())
+      : dist ? (off != nullptr ? (ordered ? render_bwd_instance<false, false, true, true, false, true>()
                                         : render_bwd_instance<false, false, false, true, false, true>())
               : ordered      ? render_bwd_instance<false, false, true, false, false, true>()
                              : render_bwd_instance<false, false, false, false, false, true>())

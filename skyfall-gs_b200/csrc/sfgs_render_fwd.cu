@@ -43,7 +43,11 @@ using PeersArg = std::conditional_t<HAS_EXTRA, const OutPeers, const OutPeers&>;
 // alpha >= 1/255).  The epilogue writes R = A S2 - S1^2 = sum_{i<j} w_i w_j (m_i - m_j)^2, whose rounding is relative
 // to A S2 and does not grow with the depth itself (the unshifted A sum w m^2 - (sum w m)^2 cancels at depths of
 // hundreds), and the state (mu, M2) = (m0 + S1 / A, R / A) the adjoint reads.
-template <bool HAS_EXTRA, bool JITTER, bool QDEPTH, bool DIST>
+// RAYD: ray depth (sfgs_rasterize_forward_ray_depth).  A record's depth at the sample position p is
+// d(p) = z + g . (p - mu), with g the slope words 14-15 (staged in the slot's quad [3].zw) and mu its centre: two FFMAs
+// on the pair's (dx, dy) = mu - p, and d(p) takes the depth word's place in out_depth.  With QDEPTH the epilogue
+// recomputes the selected record's d(p) with the same operations from its record.
+template <bool HAS_EXTRA, bool JITTER, bool QDEPTH, bool DIST, bool RAYD>
 __device__ __forceinline__ void
 render_fwd_warp(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list,
                 const unsigned char* __restrict__ inst_mask, const uint32_t* __restrict__ hdr, int W, int H,
@@ -100,6 +104,7 @@ render_fwd_warp(const uint2* __restrict__ ranges, const uint32_t* __restrict__ p
       Pq = sel ? __float_as_uint(c.w) : Pq;
     }
     const float Ta = apply ? T : 0.0f;
+    const float dep = RAYD ? fmaf(-g.z, dx, fmaf(-g.w, dy, c.z)) : c.z;
     // colour and normal (|values| <= 1) take the pair's weight alpha*T as one factor, and so do the extras; the depth
     // image reaches hundreds of units, where 1e-5 absolute is below one ulp, so it keeps the reference's exact
     // association (depth * alpha) * T and stays bit-identical
@@ -113,7 +118,7 @@ render_fwd_warp(const uint2* __restrict__ ranges, const uint32_t* __restrict__ p
       S2 = fmaf(wd, dm, S2);
     }
     C0 = fmaf(f.x, w, C0); C1 = fmaf(f.y, w, C1); C2 = fmaf(f.z, w, C2);
-    Dp = fmaf(c.z * alpha, Ta, Dp);
+    Dp = fmaf(dep * alpha, Ta, Dp);
     N0 = fmaf(f.w, w, N0); N1 = fmaf(g.x, w, N1); N2 = fmaf(g.y, w, N2);
     if constexpr (HAS_EXTRA) {
       const float* ex = extras + (size_t)S.gid[buf][k] * ED;
@@ -173,7 +178,13 @@ render_fwd_warp(const uint2* __restrict__ ranges, const uint32_t* __restrict__ p
     if constexpr (QDEPTH) {
       // the selected record's depth word, read once per pixel: keeping it in a register through the walk as well
       // made the jitter instantiation spill
-      out_depth_q[pix_id] = Pq ? rec[(size_t)point_list[range.x + Pq - 1] * REC_FLOATS + REC_DEPTH] : 0.f;
+      float dq = 0.f;
+      if (Pq) {
+        const float* r = rec + (size_t)point_list[range.x + Pq - 1] * REC_FLOATS;
+        dq = r[REC_DEPTH];
+        if constexpr (RAYD) dq = fmaf(-r[14], r[0] - pixfx, fmaf(-r[15], r[1] - pixfy, dq));
+      }
+      out_depth_q[pix_id] = dq;
       out_depth_q_pos[pix_id] = Pq;
     }
     if constexpr (DIST) {
@@ -195,9 +206,11 @@ enum class FwdOut { LOCAL_OR_PEERS, LOCAL, PEERS };
 // The one blend forward.  Each option is a template argument; a trailing parameter an instantiation does not read
 // (off without JITTER, extras without HAS_EXTRA) costs nothing, and new parameters go at the end of the list.
 // QDEPTH (the depth quantile) and DIST (the depth distortion) are instantiated one at a time, only with local outputs
-// and without extras, with and without jitter.
-template <bool HAS_EXTRA, bool JITTER, FwdOut OUT, bool QDEPTH, bool DIST>
-__global__ void __launch_bounds__(BLEND_THREADS)
+// and without extras, with and without jitter.  RAYD (ray depth) likewise, alone or with QDEPTH, with a bound of three
+// CTAs per SM: left to itself ptxas gave the instantiation without jitter and quantile 64 registers and a 4-byte spill
+// (78-80 registers, no spills, with the bound).
+template <bool HAS_EXTRA, bool JITTER, FwdOut OUT, bool QDEPTH, bool DIST, bool RAYD = false>
+__global__ void __launch_bounds__(BLEND_THREADS, RAYD ? 3 : 0)
 render_fwd_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list,
                   const unsigned char* __restrict__ inst_mask, const uint32_t* __restrict__ hdr, int W, int H,
                   int band0, const float* __restrict__ rec, const float* __restrict__ bg_color,
@@ -209,7 +222,7 @@ render_fwd_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__
                   float* __restrict__ out_dist_state) {
   constexpr bool local = OUT != FwdOut::PEERS;
   const OutPeers none{};
-  render_fwd_warp<HAS_EXTRA, JITTER, QDEPTH, DIST>(ranges, point_list, inst_mask, hdr, W, H, band0, rec, bg_color,
+  render_fwd_warp<HAS_EXTRA, JITTER, QDEPTH, DIST, RAYD>(ranges, point_list, inst_mask, hdr, W, H, band0, rec, bg_color,
                                                    local ? out_color : nullptr, local ? out_depth : nullptr,
                                                    local ? out_norm : nullptr, out_norm_raw,
                                                    local ? out_alpha : nullptr, n_contrib,
@@ -253,10 +266,12 @@ void sfgs_launch_offset_bound(const ImageLayout& im, int W, int H, const float* 
 }
 
 // out_depth_q != NULL: the depth quantile at t = 1 - q; out_dist != NULL: the depth distortion and its state [2,H,W]
-// (the entries' checks leave either no extras, peers or band, and never both)
+// (the entries' checks leave either no extras, peers or band, and never both); ray_depth: ray depth, alone or with the
+// quantile (likewise without extras, peers or band)
 void sfgs_launch_render_fwd(const sfgs_forward_args* a, const GeomLayout& g, const ImageLayout& im,
                             const BinningLayout& b, const float* off, float t, float* out_depth_q,
-                            uint32_t* out_depth_q_pos, float* out_dist, float* out_dist_state, cudaStream_t st) {
+                            uint32_t* out_depth_q_pos, float* out_dist, float* out_dist_state, bool ray_depth,
+                            cudaStream_t st) {
   dim3 grid;
   int band0;
   if (!blend_grid(a->tile_row_begin, a->tile_row_end, im, grid, band0)) return;
@@ -264,7 +279,13 @@ void sfgs_launch_render_fwd(const sfgs_forward_args* a, const GeomLayout& g, con
   if (a->out_peers != nullptr && a->n_out_peers > 0)
     for (op.n = 0; op.n < a->n_out_peers && op.n < 8; op.n++) op.p[op.n] = a->out_peers[op.n];
   // extra_attrs only without offsets (the _subpixel entries reject them)
-  const auto kernel = out_depth_q != nullptr
+  const auto kernel = ray_depth
+                          ? (out_depth_q != nullptr
+                                 ? (off != nullptr ? render_fwd_kernel<false, true, FwdOut::LOCAL, true, false, true>
+                                                   : render_fwd_kernel<false, false, FwdOut::LOCAL, true, false, true>)
+                                 : (off != nullptr ? render_fwd_kernel<false, true, FwdOut::LOCAL, false, false, true>
+                                                   : render_fwd_kernel<false, false, FwdOut::LOCAL, false, false, true>))
+                      : out_depth_q != nullptr
                           ? (off != nullptr ? render_fwd_kernel<false, true, FwdOut::LOCAL, true, false>
                                             : render_fwd_kernel<false, false, FwdOut::LOCAL, true, false>)
                       : out_dist != nullptr

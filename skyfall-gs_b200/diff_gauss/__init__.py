@@ -12,7 +12,9 @@ radii[P] int32, extra[F,H,W] | empty), and with GaussianRasterizer(settings, dep
 depth_q[1,H,W]: the depth at which the pixel's accumulated opacity crosses q (q = 0.5: the median depth), 0 where
 it never does, differentiable like the others; with GaussianRasterizer(settings, depth_distortion=True) a 7th output,
 distortion[1,H,W]: sum_{i<j} w_i w_j (m_i - m_j)^2 over the pixel's blended splats, the distortion loss of Mip-NeRF
-360 / 2DGS, differentiable like the others.  `means2D` is a dummy [P,3] leaf whose
+360 / 2DGS, differentiable like the others.  With GaussianRasterizer(settings, ray_depth=True) the outputs are the
+same, but each splat's depth is taken where the pixel's ray meets it rather than at its centre (in depth and in
+depth_q), so the depth's gradient also reaches rotations and scales.  `means2D` is a dummy [P,3] leaf whose
 .grad receives (dL/dx_ndc * W/2, dL/dy_ndc * H/2, sum |.|) — the densification
 statistics consumed by scene/gaussian_model.py:744-749.
 """
@@ -120,8 +122,8 @@ def _checked_inputs(shs, colors_precomp, scales, rotations, cov3Ds_precomp, norm
 class _RasterizeGaussians(torch.autograd.Function):
     """The rasterizer for the pinhole camera (diff_gauss) and the orthographic one (sfgs.ortho).  Every input slot is
     always passed: the callers resolve the options `fuse_normalize`, `depth_quantile` (q or None), `depth_distortion`,
-    `subpixel_offset` (a [H,W,2] tensor or None) and `ortho`.  With a quantile the outputs end with
-    (depth_q, depth_q_pos); with the distortion, with distortion."""
+    `subpixel_offset` (a [H,W,2] tensor or None), `ortho` and `ray_depth` (the last slot has a default).  With a
+    quantile the outputs end with (depth_q, depth_q_pos); with the distortion, with distortion."""
     # viewmatrix, projmatrix and campos are inputs of their own (the settings tuple is not tracked by autograd), so a
     # camera built from parameters that require grad (scene/cameras.py: Camera(..., optimizing=True)) gets gradients
     CAMERA_INPUTS = slice(12, 15)
@@ -133,9 +135,9 @@ class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                 norm3Ds_precomp, extra_attrs, raster_settings, fuse_normalize, viewmatrix, projmatrix, campos, tanfovx,
-                tanfovy, depth_quantile, depth_distortion, subpixel_offset=None, ortho=False):
+                tanfovy, depth_quantile, depth_distortion, subpixel_offset=None, ortho=False, ray_depth=False):
         rs = raster_settings
-        ctx.depth_q, ctx.dist = depth_quantile is not None, bool(depth_distortion)
+        ctx.depth_q, ctx.dist, ctx.ray_depth = depth_quantile is not None, bool(depth_distortion), bool(ray_depth)
         n_extra = extra_attrs.shape[1] if extra_attrs.shape[0] != 0 else 0
         assert n_extra <= MAX_EXTRA_DIMS
         # under stream capture (torch.cuda.graph) the capture-safe entries run: no host wait, intrinsics that are 0-d
@@ -145,7 +147,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         opts = {}
         if ctx.graph:
             for on, what in ((ctx.depth_q, "the depth quantile"), (ctx.dist, "the depth distortion"),
-                             (ortho, "the orthographic camera")):
+                             (ortho, "the orthographic camera"), (ctx.ray_depth, "ray depth")):
                 if on:
                     raise _C.SfgsError(f"diff_gauss: {what} cannot be captured in a CUDA graph")
             if rs.debug:
@@ -160,6 +162,8 @@ class _RasterizeGaussians(torch.autograd.Function):
             opts["depth_quantile"] = depth_quantile
         if ctx.dist:
             opts["depth_distortion"] = True
+        if ctx.ray_depth:
+            opts["ray_depth"] = True
         native_args = (rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier,
                        cov3Ds_precomp, norm3Ds_precomp, extra_attrs, n_extra, viewmatrix, projmatrix,
                        tanfovx, tanfovy, rs.kernel_size, rs.image_height, rs.image_width, sh, rs.sh_degree,
@@ -214,6 +218,8 @@ class _RasterizeGaussians(torch.autograd.Function):
             opts.update(depth_q_pos=side_state, dL_dout_depth_q=g_side.contiguous())
         if ctx.dist:
             opts.update(distortion_state=side_state, dL_dout_distortion=g_side.contiguous())
+        if ctx.ray_depth:
+            opts["ray_depth"] = True
         bwd = functools.partial(_C.rasterize_gaussians_backward_fused if ctx.fused else
                                 _C.rasterize_gaussians_backward, **opts)
         if ctx.subpixel_offset is not None:
@@ -227,19 +233,23 @@ class _RasterizeGaussians(torch.autograd.Function):
         (g_means2D, g_colors, g_opac, g_means3D, g_cov3D, g_norm3D, g_sh, g_scales, g_rot, g_extra_attrs) = grads[:10]
         # order of forward's inputs; the settings tuple and the options get no gradient
         return ((g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rot, g_cov3D, g_norm3D, g_extra_attrs)
-                + (None, None) + g_camera + g_intrinsics + (None,) * 4)
+                + (None, None) + g_camera + g_intrinsics + (None,) * 5)
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                        norm3Ds_precomp, extra_attrs, raster_settings, depth_quantile=None, depth_distortion=False):
+                        norm3Ds_precomp, extra_attrs, raster_settings, depth_quantile=None, depth_distortion=False,
+                        ray_depth=False):
     rs = raster_settings
     if depth_distortion and depth_quantile is not None:
         raise _C.SfgsError("diff_gauss: depth_distortion and depth_quantile in one call are not supported; render "
                            "them in two calls")
+    if depth_distortion and ray_depth:
+        raise _C.SfgsError("diff_gauss: depth_distortion together with ray_depth is not supported")
     out = _RasterizeGaussians.apply(
         means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, norm3Ds_precomp,
         extra_attrs, rs, FUSE_NORMALIZE, rs.viewmatrix, rs.projmatrix, rs.campos, rs.tanfovx, rs.tanfovy,
-        None if depth_quantile is None else float(depth_quantile), bool(depth_distortion), _subpixel_offset(rs), False)
+        None if depth_quantile is None else float(depth_quantile), bool(depth_distortion), _subpixel_offset(rs), False,
+        bool(ray_depth))
     color, depth, norm, alpha, radii, extra = out[:6]
     if not FUSE_NORMALIZE:
         # the reference normalises the blended normal map in torch, inside the autograd graph (diff_gauss/__init__.py:48)
@@ -251,13 +261,17 @@ class GaussianRasterizer(nn.Module):
     """depth_quantile=q (0 < q < 1): forward() also returns depth_q [1,H,W], the depth at which each pixel's accumulated
     opacity crosses q (include/sfgs.h, sfgs_rasterize_forward_depth_quantile).  depth_distortion=True: forward() also
     returns distortion [1,H,W], sum_{i<j} w_i w_j (m_i - m_j)^2 over each pixel's blended splats in units of depth^2
-    (include/sfgs.h, sfgs_rasterize_forward_distortion).  Not under CUDA-graph capture, and not both in one call."""
+    (include/sfgs.h, sfgs_rasterize_forward_distortion).  Not under CUDA-graph capture, and not both in one call.
+    ray_depth=True: the same outputs, with each splat's depth taken where the pixel's ray meets it, z + g . (p - mu),
+    not at its centre (include/sfgs.h, sfgs_rasterize_forward_ray_depth); combines with depth_quantile, not with
+    depth_distortion or CUDA-graph capture."""
 
-    def __init__(self, raster_settings, depth_quantile=None, depth_distortion=False):
+    def __init__(self, raster_settings, depth_quantile=None, depth_distortion=False, ray_depth=False):
         super().__init__()
         self.raster_settings = raster_settings
         self.depth_quantile = depth_quantile
         self.depth_distortion = depth_distortion
+        self.ray_depth = ray_depth
 
     def markVisible(self, positions):
         """Boolean mask of the points in front of the near plane (view depth > 0.2)."""
@@ -271,4 +285,4 @@ class GaussianRasterizer(nn.Module):
             shs, colors_precomp, scales, rotations, cov3Ds_precomp, norm3Ds_precomp, extra_attrs)
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                                    norm3Ds_precomp, extra_attrs, self.raster_settings, self.depth_quantile,
-                                   self.depth_distortion)
+                                   self.depth_distortion, self.ray_depth)

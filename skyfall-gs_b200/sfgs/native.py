@@ -102,6 +102,7 @@ EXPORTS = [
     "sfgs_rasterize_forward_ortho", "sfgs_rasterize_backward_ortho",
     "sfgs_rasterize_forward_depth_quantile", "sfgs_rasterize_backward_depth_quantile",
     "sfgs_rasterize_forward_distortion", "sfgs_rasterize_backward_distortion",
+    "sfgs_rasterize_forward_ray_depth", "sfgs_rasterize_backward_ray_depth",
 ]
 STAGE_NAMES = ["fwd_zero", "preprocess", "tile_scan", "emit_keys", "tile_sort", "render_fwd", "bwd_zero", "render_bwd",
                "gauss_bwd", "bwd_order"]
@@ -163,6 +164,12 @@ def lib() -> C.CDLL:
     L.sfgs_rasterize_backward_distortion.argtypes = [C.POINTER(BackwardArgs), C.c_void_p, C.c_int, C.c_int,
                                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
     L.sfgs_rasterize_backward_distortion.restype = C.c_int
+    L.sfgs_rasterize_forward_ray_depth.argtypes = [C.POINTER(ForwardArgs), C.c_void_p, C.c_int, C.c_float, C.c_void_p,
+                                                   C.c_void_p]
+    L.sfgs_rasterize_forward_ray_depth.restype = C.c_int
+    L.sfgs_rasterize_backward_ray_depth.argtypes = [C.POINTER(BackwardArgs), C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+                                                    C.c_void_p, C.c_void_p, C.c_int]
+    L.sfgs_rasterize_backward_ray_depth.restype = C.c_int
     L.sfgs_capacity_estimate.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int]
     L.sfgs_capacity_estimate.restype = C.c_longlong
     L.sfgs_mark_visible.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]

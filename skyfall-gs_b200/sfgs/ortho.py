@@ -100,13 +100,16 @@ class OrthoRasterizer(nn.Module):
     .grad receives (dL/dx_ndc W/2, dL/dy_ndc H/2, sum |.|), the densification statistics.  There are no camera
     gradients: a viewmatrix or projmatrix that requires grad raises.  With depth_quantile=q (0 < q < 1) a 7th output,
     depth_q [1,H,W], as for diff_gauss.GaussianRasterizer; with depth_distortion=True a 7th output, distortion [1,H,W],
-    likewise (not both in one call)."""
+    likewise (not both in one call).  ray_depth=True: the same outputs with each splat's depth taken where the pixel's
+    ray meets it (as for diff_gauss.GaussianRasterizer); with depth_quantile, not with depth_distortion."""
 
-    def __init__(self, raster_settings: OrthoRasterizationSettings, depth_quantile=None, depth_distortion=False):
+    def __init__(self, raster_settings: OrthoRasterizationSettings, depth_quantile=None, depth_distortion=False,
+                 ray_depth=False):
         super().__init__()
         self.raster_settings = raster_settings
         self.depth_quantile = depth_quantile
         self.depth_distortion = depth_distortion
+        self.ray_depth = ray_depth
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
                 cov3Ds_precomp=None, norm3Ds_precomp=None, extra_attrs=None):
@@ -128,6 +131,8 @@ class OrthoRasterizer(nn.Module):
         if self.depth_distortion and self.depth_quantile is not None:
             raise N.SfgsError("OrthoRasterizer: depth_distortion and depth_quantile in one call are not supported; "
                               "render them in two calls")
+        if self.depth_distortion and self.ray_depth:
+            raise N.SfgsError("OrthoRasterizer: depth_distortion together with ray_depth is not supported")
         # the half-extents travel in the tan_fov fields (as numbers: they get no gradient), and campos is not read
         s_x, s_y = float(rs.half_width), float(rs.half_height)
         campos = torch.zeros(3, dtype=torch.float32, device=means3D.device)
@@ -139,18 +144,23 @@ class OrthoRasterizer(nn.Module):
             means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, norm3Ds_precomp,
             extra_attrs, settings, True, rs.viewmatrix, rs.projmatrix, campos, s_x, s_y,
             None if self.depth_quantile is None else float(self.depth_quantile), bool(self.depth_distortion),
-            rs.subpixel_offset, True)
+            rs.subpixel_offset, True, bool(self.ray_depth))
 
 
 def render_height_map(camera: NadirCamera, means3D, opacities, scales, rotations, shs=None, colors_precomp=None,
-                      sh_degree=0, alpha_min=0.5, kernel_size=0.1, scale_modifier=1.0, surface_quantile=None):
+                      sh_degree=0, alpha_min=0.5, kernel_size=0.1, scale_modifier=1.0, surface_quantile=None,
+                      ray_depth=False):
     """The scene's height map [H, W] seen by `camera` (nadir_camera): z_top - depth / alpha where the accumulated
     alpha is >= alpha_min, NaN elsewhere.  depth / alpha is the alpha-normalised expected view depth of the pixel.
     Differentiable with respect to the Gaussians (e.g. an L1 against a DSM over the finite pixels).
 
     surface_quantile=q (0 < q < 1): z_top - depth_q instead, the depth of the one splat at which the pixel's
     accumulated opacity crosses q (q = 0.5: the median depth), where a splat was selected and alpha >= alpha_min.  It
-    does not blend a roof edge with the ground below it; a lower q reports the first surface seen from above."""
+    does not blend a roof edge with the ground below it; a lower q reports the first surface seen from above.
+
+    ray_depth=True: each splat reports its depth where the pixel's ray meets it, not its centre's depth, so a sloped
+    roof of flat splats is rendered as a slope instead of terraces (in both maps), and the map's gradient reaches the
+    splats' rotations and scales."""
     dev = means3D.device
     if shs is None and colors_precomp is None:
         colors_precomp = torch.zeros((means3D.shape[0], 3), dtype=torch.float32, device=dev)
@@ -158,7 +168,7 @@ def render_height_map(camera: NadirCamera, means3D, opacities, scales, rotations
                                     kernel_size, torch.zeros(3, device=dev), scale_modifier,
                                     camera.viewmatrix.to(dev), camera.projmatrix.to(dev), sh_degree, False, False)
     means2D = torch.zeros_like(means3D)
-    out = OrthoRasterizer(rs, depth_quantile=surface_quantile)._rasterize(
+    out = OrthoRasterizer(rs, depth_quantile=surface_quantile, ray_depth=ray_depth)._rasterize(
         means3D, means2D, opacities, shs=shs, colors_precomp=colors_precomp, scales=scales, rotations=rotations)
     depth, alpha = out[1][0], out[3][0]
     if surface_quantile is not None:

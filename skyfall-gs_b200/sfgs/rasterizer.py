@@ -94,6 +94,7 @@ GRAPH = "cannot be captured in a CUDA graph"
 ORTHO = "not supported with an orthographic camera"
 DEPTH_Q = "not supported with the depth quantile"
 DISTORTION = "not supported with the depth distortion"
+RAY_DEPTH = "not supported with ray depth"
 
 
 def _reject(where, tail, **opts):
@@ -126,7 +127,7 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
                         tan_fovx, tan_fovy, kernel_size, image_height, image_width, sh, degree, campos,
                         prefiltered, debug, capacity_hint=0, tile_rows=None, fuse_normalize=False, out_planes=None,
                         out_peers=None, subpixel_offset=None, graph=False, *, ortho=False, depth_quantile=None,
-                        depth_distortion=False):
+                        depth_distortion=False, ray_depth=False):
     """Same positional signature and return tuple as the reference's `_C.rasterize_gaussians`.  With
     `fuse_normalize=True` the returned normal map is already F.normalize(., dim=0) (the reference's torch post-op,
     diff_gauss/__init__.py:48) and the un-normalised blend is appended to the tuple for the backward.
@@ -157,10 +158,19 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
     R = sum_{i<j} w_i w_j (m_i - m_j)^2 over the pixel's blended splats (w = alpha T, m the view depth), the distortion
     loss of Mip-NeRF 360 / 2DGS, in units of depth^2.  The tuple ends with (distortion [1,H,W], distortion_state
     [2,H,W]); the backward takes distortion_state back.  It combines with `ortho` and offsets; depth_quantile, graph,
-    tile_rows, out_peers and extra_attrs raise SfgsError.  Every other output is bit-identical to the call without it."""
+    tile_rows, out_peers and extra_attrs raise SfgsError.  Every other output is bit-identical to the call without it.
+
+    `ray_depth=True` (sfgs_rasterize_forward_ray_depth, include/sfgs.h): each splat's depth is taken where the pixel's
+    ray meets it, d(p) = z + g . (p - mu) with g its depth slope, not its centre's depth z, in out_depth and (with
+    `depth_quantile`) in depth_q.  The backward must be given `ray_depth=True` too.  It combines with `ortho`, offsets
+    and `depth_quantile`; depth_distortion, graph, tile_rows, out_peers and extra_attrs raise SfgsError.  Every other
+    output is bit-identical to the call without it."""
     if means3D.ndim != 2 or means3D.shape[1] != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")
     banded = dict(tile_rows=tile_rows is not None, out_peers=out_peers is not None)
+    if ray_depth:
+        _reject("rasterize_gaussians(ray_depth=True)", RAY_DEPTH, depth_distortion=depth_distortion, graph=graph,
+                **banded, extra_attrs=int(attr_degree) > 0)
     if depth_distortion:
         _reject("rasterize_gaussians(depth_distortion=True)", DISTORTION, depth_quantile=depth_quantile is not None,
                 graph=graph, **banded, extra_attrs=int(attr_degree) > 0)
@@ -251,7 +261,13 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
                 a.tile_row_begin, a.tile_row_end = _band(tile_rows)
             # the entry and its arguments after the struct, in the order of precedence of the options
             off = _ptr(subpixel_offset, keep)
-            if depth_quantile is not None:
+            if ray_depth:
+                q = depth_quantile is not None
+                entry, args = "sfgs_rasterize_forward_ray_depth", (off, int(bool(ortho)),
+                                                                   float(depth_quantile) if q else 0.0,
+                                                                   side[0].data_ptr() if q else None,
+                                                                   side[1].data_ptr() if q else None)
+            elif depth_quantile is not None:
                 entry, args = "sfgs_rasterize_forward_depth_quantile", (off, int(bool(ortho)), float(depth_quantile),
                                                                         side[0].data_ptr(), side[1].data_ptr())
             elif depth_distortion:
@@ -311,7 +327,7 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
                                  gauss_range=None, acc_peers=None, peer_slice=0, subpixel_offset=None,
                                  camera_grad=False, intrinsics_grad=False, graph=False, *, ortho=False,
                                  depth_q_pos=None, dL_dout_depth_q=None, distortion_state=None,
-                                 dL_dout_distortion=None):
+                                 dL_dout_distortion=None, ray_depth=False):
     """Same positional signature and return tuple as the reference's `_C.rasterize_gaussians_backward`.  With
     `norm_raw` (the extra tensor a `fuse_normalize=True` forward returned) `dL_dout_norm` is taken w.r.t. the unit
     normal map and the adjoint of F.normalize is applied inside the blend-adjoint kernel.
@@ -361,9 +377,19 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     `distortion_state` (the forward's, with `depth_distortion=True`) and `dL_dout_distortion` ([1,H,W]): the backward of
     a depth-distortion forward (sfgs_rasterize_backward_distortion), which adds dL/dR to the blend adjoint's alpha and
     depth terms.  It takes offsets, `ortho`, the deterministic mode, phase 1, and camera and focal gradients (not with
-    `ortho`); depth_q_pos, graph, tile_rows, acc_peers and extra_attrs raise SfgsError."""
+    `ortho`); depth_q_pos, graph, tile_rows, acc_peers and extra_attrs raise SfgsError.
+
+    `ray_depth=True`: the backward of a `ray_depth=True` forward (sfgs_rasterize_backward_ray_depth), with or without
+    its depth quantile's `depth_q_pos` / `dL_dout_depth_q`; the depth cotangents then also reach each splat's depth
+    slope, and through it its rotation, scale and covariance.  It takes offsets, `ortho`, the deterministic mode,
+    phase 1, and camera and focal gradients (not with `ortho`); distortion_state, graph, tile_rows, acc_peers and
+    extra_attrs raise SfgsError."""
     banded = dict(tile_rows=tile_rows is not None, acc_peers=acc_peers is not None)
     has_extra = extra_attrs is not None and extra_attrs.numel() != 0
+    if ray_depth:
+        _reject("rasterize_gaussians_backward(ray_depth=True)", RAY_DEPTH,
+                distortion_state=distortion_state is not None or dL_dout_distortion is not None, graph=graph, **banded,
+                extra_attrs=has_extra)
     dist = _given_together("distortion_state", distortion_state, "dL_dout_distortion", dL_dout_distortion)
     if dist:
         _reject("rasterize_gaussians_backward(distortion_state=...)", DISTORTION,
@@ -414,7 +440,7 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
             pos += pad(P * w)
         dL_dsh = alloc((P, M, 3), **fopt)
         dL_dextra = alloc((P, F), **fopt) if F > 0 else torch.empty(0, **fopt)
-        f64 = partial and (P == 0 or not (depth_q or dist))
+        f64 = partial and (P == 0 or not (depth_q or dist or ray_depth))
         dL_dcamera = alloc((ncam,), dtype=torch.float64 if f64 else torch.float32, device=dev) if ncam else None
         if P > 0:
             with torch.cuda.device(dev):
@@ -489,7 +515,12 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
                 off = _ptr(subpixel_offset, keep)
                 det = int(deterministic)
                 cam = dL_dcamera.data_ptr() if ncam else None
-                if depth_q:
+                if ray_depth:
+                    entry, args = "sfgs_rasterize_backward_ray_depth", (off, int(bool(ortho)), det,
+                                                                        _ptr(depth_q_pos, keep) if depth_q else None,
+                                                                        _ptr(dL_dout_depth_q, keep) if depth_q else None,
+                                                                        cam, ncam)
+                elif depth_q:
                     entry, args = "sfgs_rasterize_backward_depth_quantile", (off, int(bool(ortho)), det,
                                                                              _ptr(depth_q_pos, keep),
                                                                              _ptr(dL_dout_depth_q, keep), cam, ncam)
