@@ -461,6 +461,42 @@ int sfgs_rasterize_backward_ray_depth(const sfgs_backward_args* a, const float* 
                                       int deterministic, const uint32_t* depth_q_pos, const float* dL_dpix_depth_q,
                                       float* dL_dcamera, int ncam);
 
+/* ---- Plane normals -----------------------------------------------------------------------------------------------
+ * Ray depth (above) whose normals are those of the plane its depths lie on, and the backward that differentiates
+ * them.  The shortest-axis normal of the other entries ignores the depth the rasterizer renders, jumps where two scales
+ * cross and has a gradient that reaches the rotation only; this one is the normal of the surface out_depth describes,
+ * so a depth-normal consistency loss can make the two agree.
+ *   - For record i, with g_i its ray-depth slope (record words 14-15), T0, T1 the two rows of T = J W in world
+ *     coordinates (the J, with its 1.3 tan clamp, and the W from which the 2D covariance and s are formed) and
+ *     w3 = (view[2], view[6], view[10]):
+ *         u_i = w3 - g_x T0 - g_y T1,   n_i = sigma_i u_i / |u_i|,
+ *         sigma_i = -1 where (m_i - campos) . u_i > 0 (orthographic: where w3 . u_i > 0), else +1
+ *     the shortest-axis normal's flip, so the normals face the camera.  A world displacement dX moves the pixel by
+ *     T dX and the depth by w3 . dX, so the plane d(p) = z + g . (p - mu) is {dX : w3 . dX = g . T dX} and u is its
+ *     normal.  |u|^2 >= 1 / (1 + (t_x/t_z)^2 + (t_y/t_z)^2) (pinhole, clamped t_x, t_y) and >= 1 (orthographic).
+ *   - Record words 11-13 hold n_i in place of the shortest-axis normal; out_norm = sum n_i alpha_i T_i, and the fused or
+ *     torch normalisation, are as before.  Colour, alpha, out_depth, out_depth_q, n_contrib, radii, binning and
+ *     record words 0-10 and 14-15 are bit-identical to sfgs_rasterize_forward_ray_depth.
+ *   - kernel_size = 0 and a flat splat (rank-2 Sigma): n_i is the splat's shortest-axis normal up to sign.  With
+ *     kernel_size > 0 the dilation shrinks g, as it shrinks the ray depth's slope, and n_i tilts toward the camera
+ *     (most for footprints whose smaller 2D eigenvalue is below a pixel^2): it is the normal of the depth rendered.
+ *   - Gradient, with c = dL/dn_i (acc words 4-6, the blend adjoint's normal sums): dL/du = sigma (I - n n^T) c / |u|,
+ *     sigma recovered from the sign of u . (record words 11-13).  dL/dg gains -(T0 . dL/du, T1 . dL/du) beside acc
+ *     words 14-15 before the ray-depth chain; dL/dT0 gains -g_x dL/du and dL/dT1 gains -g_y dL/du before dL/dJ (t,
+ *     means3D, the focal terms); with camera gradients dL/dview[2, 6, 10] gains dL/du.  dL_dnorm3D is 0 and the
+ *     rotation gets no shortest-axis term.  With every normal cotangent 0 the deterministic gradients are those of
+ *     sfgs_rasterize_backward_ray_depth to float32 rounding: dL_dmean3D, dL_dcov3D, dL_dscale, dL_drot and the camera
+ *     terms are summed from products the compiler contracts into FMAs differently, the other six are equal.  No
+ *     gradient with respect to kernel_size.
+ * Arguments as for the ray-depth entries; the backward must be given the forward's option.  Before any CUDA work, in
+ * ray depth's order with its messages naming plane normals, and then norm3D_precomp given (SFGS_E_UNSUPPORTED).
+ * Not available under graph capture, with tile-row sharding, with extra_attrs or together with the depth distortion. */
+int sfgs_rasterize_forward_plane_normals(const sfgs_forward_args* a, const float* subpixel_offset, int ortho,
+                                         float quantile, float* out_depth_q, uint32_t* out_depth_q_pos);
+int sfgs_rasterize_backward_plane_normals(const sfgs_backward_args* a, const float* subpixel_offset, int ortho,
+                                          int deterministic, const uint32_t* depth_q_pos,
+                                          const float* dL_dpix_depth_q, float* dL_dcamera, int ncam);
+
 /* ---- markVisible --------------------------------------------------------- */
 int sfgs_mark_visible(int P, const float* means3D, const float* viewmatrix,
                       const float* projmatrix, unsigned char* present, void* stream);

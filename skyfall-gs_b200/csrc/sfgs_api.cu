@@ -26,7 +26,7 @@ std::atomic<long long> g_sfgs_launches{0};
 
 void sfgs_launch_preprocess(const sfgs_forward_args* a, const GeomLayout& g, const ImageLayout& im,
                             const BinningLayout& b, unsigned long long capacity, float focal_x, float focal_y,
-                            const float* tan_fov, bool ortho, bool ray_depth, cudaStream_t st);
+                            const float* tan_fov, bool ortho, bool ray_depth, bool plane_normals, cudaStream_t st);
 void sfgs_launch_mark_visible(int P, const float* means3D, const float* viewmatrix, unsigned char* present,
                               cudaStream_t st);
 void sfgs_launch_tile_scan(const ImageLayout& im, unsigned long long capacity, cudaStream_t st);
@@ -63,7 +63,7 @@ int sfgs_launch_activations_bwd(int P, const float* opacity_raw, const float* sc
                                 float* g_rotation_raw, cudaStream_t st);
 void sfgs_launch_gauss_bwd(const sfgs_backward_args* a, const GeomLayout& g, float focal_x, float focal_y,
                            const float* acc, int g_begin, int g_end, int acc_row0, double* cam_part, int ncam,
-                           const float* tan_fov, bool ortho, bool ray_depth, cudaStream_t st);
+                           const float* tan_fov, bool ortho, bool ray_depth, bool plane_normals, cudaStream_t st);
 size_t sfgs_camera_scratch_bytes(int P, int ncam);
 void sfgs_launch_camera_reduce(int P, int ncam, const double* cam_part, float* dL_dcamera, cudaStream_t st);
 void sfgs_launch_camera_partial_reduce(int n, int ncam, const double* cam_part, double* dL_dcamera, cudaStream_t st);
@@ -227,6 +227,7 @@ struct FwdCall {
   float* out_distortion = nullptr;
   float* out_distortion_state = nullptr;   // ... and the state (mu, M2) [2,H,W] its adjoint reads
   bool ray_depth = false;             // ray depth (sfgs_rasterize_forward_ray_depth), with or without depth_q
+  bool plane_normals = false;         // plane normals (sfgs_rasterize_forward_plane_normals), with ray_depth
 };
 
 struct BwdCall {
@@ -247,6 +248,7 @@ struct BwdCall {
   const float* distortion_state = nullptr;    // ... from the forward's state [2,H,W] ...
   const float* dL_dpix_distortion = nullptr;  // ... and the cotangent of R [H,W]
   bool ray_depth = false;             // ray depth's adjoint (sfgs_rasterize_backward_ray_depth), with or without depth_q
+  bool plane_normals = false;         // plane normals' adjoint (sfgs_rasterize_backward_plane_normals), with ray_depth
 };
 
 int rasterize_forward(const sfgs_forward_args* a, const FwdCall& c);
@@ -425,6 +427,34 @@ int sfgs_rasterize_backward_ray_depth(const sfgs_backward_args* a, const float* 
   return rasterize_backward(a, c);
 }
 
+int sfgs_rasterize_forward_plane_normals(const sfgs_forward_args* a, const float* subpixel_offset, int ortho,
+                                         float quantile, float* out_depth_q, uint32_t* out_depth_q_pos) {
+  FwdCall c{"forward_plane_normals", false, subpixel_offset};
+  c.ortho = ortho != 0;
+  c.ray_depth = true;
+  c.plane_normals = true;
+  c.depth_q = out_depth_q != nullptr;     // NULL: no quantile
+  c.quantile = quantile;
+  c.out_depth_q = out_depth_q;
+  c.out_depth_q_pos = out_depth_q_pos;
+  return rasterize_forward(a, c);
+}
+
+int sfgs_rasterize_backward_plane_normals(const sfgs_backward_args* a, const float* subpixel_offset, int ortho,
+                                          int deterministic, const uint32_t* depth_q_pos,
+                                          const float* dL_dpix_depth_q, float* dL_dcamera, int ncam) {
+  // ncam > 0: the checks and the stages of sfgs_rasterize_backward_camera[_intrinsics] (a bad ncam is rejected first)
+  BwdCall c{"backward_plane_normals", ncam > 0 ? BwdCall::CAMERA : BwdCall::EAGER, subpixel_offset, false,
+            deterministic != 0, ncam, ncam > 0 ? dL_dcamera : nullptr};
+  c.ortho = ortho != 0;
+  c.ray_depth = true;
+  c.plane_normals = true;
+  c.depth_q = depth_q_pos != nullptr || dL_dpix_depth_q != nullptr;   // both NULL: no quantile
+  c.depth_q_pos = depth_q_pos;
+  c.dL_dpix_depth_q = dL_dpix_depth_q;
+  return rasterize_backward(a, c);
+}
+
 }  // extern "C"
 
 namespace {
@@ -460,11 +490,14 @@ int check_forward(const sfgs_forward_args* a, const FwdCall& c) {
   if (!a) return reject(SFGS_E_BADARG, "null args");
   if (c.ray_depth) {
     // with a quantile (out_depth_q given) its own arguments first; every unsupported option is then reported as ray
-    // depth's (the quantile's check below finds nothing left)
+    // depth's, or as plane normals' (the quantile's check below finds nothing left)
+    const char* feature = c.plane_normals ? "plane normals" : "ray depth";
     const char* bad_q = !c.depth_q || quantile_ok(c.quantile) ? nullptr : "the quantile must be finite with 0 < q < 1";
     if (const int rc = check_pixel_output(a, c.name, c.depth_q && !c.out_depth_q_pos, "null out_depth_q_pos", bad_q,
-                                          "ray depth"))
+                                          feature))
       return rc;
+    // the normal is the ray-depth plane's, not an input
+    if (c.plane_normals && a->norm3D_precomp != nullptr) return reject_with(c.name, "norm3D_precomp is", feature);
   }
   if (c.depth_q) {
     const char* bad_q = quantile_ok(c.quantile) ? nullptr : "the quantile must be finite with 0 < q < 1";
@@ -565,7 +598,7 @@ int rasterize_forward(const sfgs_forward_args* a, const FwdCall& c) {
     if (P > 0) {
       PROF_BEGIN(ST_PREPROCESS);
       sfgs_launch_preprocess(a, g, im, b, (unsigned long long)capacity, focal_x, focal_y, c.tan_fov, c.ortho,
-                             c.ray_depth, st);
+                             c.ray_depth, c.plane_normals, st);
       PROF_END();
       STAGE_CHECK("preprocess");
     }
@@ -668,9 +701,11 @@ int check_backward(const sfgs_backward_args* a, const BwdCall& c) {
   const auto reject = [&c](int code, const char* what) { return fail_in(c.name, code, what); };
   if (!a) return reject(SFGS_E_BADARG, "null args");
   if (c.ray_depth) {
+    const char* feature = c.plane_normals ? "plane normals" : "ray depth";
     if (const int rc = check_pixel_output(a, c, c.depth_q && (!c.depth_q_pos || !c.dL_dpix_depth_q),
-                                          "null depth_q_pos or dL_dpix_depth_q", "ray depth"))
+                                          "null depth_q_pos or dL_dpix_depth_q", feature))
       return rc;
+    if (c.plane_normals && a->norm3D_precomp != nullptr) return reject_with(c.name, "norm3D_precomp is", feature);
   }
   if (c.depth_q) {
     if (const int rc = check_pixel_output(a, c, !c.depth_q_pos || !c.dL_dpix_depth_q,
@@ -865,7 +900,7 @@ int rasterize_backward(const sfgs_backward_args* a, const BwdCall& c) {
   if (do_gauss) {
     PROF_BEGIN(ST_GAUSS_BWD);
     sfgs_launch_gauss_bwd(a, g, focal_x, focal_y, acc, g_begin, g_end, phase == 2 ? g_begin : 0, cam_part, ncam,
-                          c.tan_fov, c.ortho, c.ray_depth, st);
+                          c.tan_fov, c.ortho, c.ray_depth, c.plane_normals, st);
     if (dL_dcamera) sfgs_launch_camera_reduce(P, ncam, cam_part, dL_dcamera, st);
     // an empty slice has no spans: the reduction writes zeros
     if (dL_dcamera_partial) sfgs_launch_camera_partial_reduce(g_end - g_begin, ncam, cam_part, dL_dcamera_partial, st);

@@ -111,7 +111,12 @@ __device__ __forceinline__ float3 dnormvdv3(float3 v, float3 dv) {
 // off-diagonal derivative) before the conic -> cov2D chain; dL/dSigma gains sym(w3 (dL/ds T)) and dL/dT gains
 // dL/ds (Sigma w3), which reach cov3D, scales, rotations, t, means3D and the focal terms; w3 itself gives direct
 // viewmatrix terms.  C is formed again from the 2D covariance (the stage holds record words 4-15 only).
-template <int NCAM, bool ORTHO, bool RAYD, class SH>
+// PLANE: plane normals (sfgs_rasterize_backward_plane_normals), with RAYD only.  The record's normal (words 11-13) is
+// n = sigma u / |u|, u = w3 - g_x T0 - g_y T1 (T0, T1 the rows of T = J W); with c = dL/dn (A1.xyz),
+// dL/du = sigma (I - n n^T) c / |u|, u formed again here and sigma recovered from the sign of u . (words 11-13).  dL/dg
+// gains -(T0 . dL/du, T1 . dL/du) before the ray-depth chain, dL/dT_i gains -g_i dL/du before dL/dJ, and dL/dw3 gains
+// dL/du (viewmatrix entries 2, 6, 10).  dL_dnorm3D is 0 and the rotation gets no shortest-axis term.
+template <int NCAM, bool ORTHO, bool RAYD, bool PLANE, class SH>
 __device__ __forceinline__ void gauss_adjoint(
     int D, float mx, float my, float mz, bool has_scales, float4 q_in, float scx, float scy, float scz,
     float scale_modifier, bool has_sh, unsigned cm, SH sh, const float* cov3D, bool norm_precomp, float4 A0,
@@ -130,7 +135,7 @@ __device__ __forceinline__ void gauss_adjoint(
   for (int q = 0; q < 16; q++) dsh_scale[q] = 0.f;
   float dL_dRGB[3] = {0, 0, 0};
   o_color[0] = A0.x; o_color[1] = A0.y; o_color[2] = A0.z; o_depth = A0.w;
-  o_norm[0] = A1.x; o_norm[1] = A1.y; o_norm[2] = A1.z;
+  if constexpr (!PLANE) { o_norm[0] = A1.x; o_norm[1] = A1.y; o_norm[2] = A1.z; }   // PLANE: dL_dnorm3D is 0
   o_mean2D[0] = A1.w; o_mean2D[1] = A2.x; o_mean2D[2] = A2.y;
   o_conic[0] = A2.z; o_conic[1] = A2.w; o_conic[3] = A3.x;
   o_opac = A3.y;
@@ -190,12 +195,30 @@ __device__ __forceinline__ void gauss_adjoint(
     // RAYD: dL/ds and w3, and the conic cotangent of g = C s
     float dLds0 = 0.f, dLds1 = 0.f;
     const float w3[3] = {view[2], view[6], view[10]};
+    // PLANE: dL/du of the plane normal
+    float dLdu[3] = {0.f, 0.f, 0.f};
+    if constexpr (PLANE) {
+      static_assert(RAYD, "plane normals are the normals of the ray-depth plane");
+      float uv[3];
+#pragma unroll
+      for (int r = 0; r < 3; r++) uv[r] = w3[r] - rec3.z * T[0][r] - rec3.w * T[1][r];
+      const float inv_len = 1.f / sqrtf(uv[0] * uv[0] + uv[1] * uv[1] + uv[2] * uv[2]);
+      const float nh[3] = {uv[0] * inv_len, uv[1] * inv_len, uv[2] * inv_len};
+      const float cn[3] = {A1.x, A1.y, A1.z};
+      const float nc = nh[0] * cn[0] + nh[1] * cn[1] + nh[2] * cn[2];
+      // sigma: the forward's flip, read off the record's normal
+      const float f = uv[0] * rec2.w + uv[1] * rec3.x + uv[2] * rec3.y < 0.f ? -inv_len : inv_len;
+#pragma unroll
+      for (int r = 0; r < 3; r++) dLdu[r] = f * (cn[r] - nh[r] * nc);
+    }
     if constexpr (RAYD) {
       const float s0 = w3[0] * X[0][0] + w3[1] * X[1][0] + w3[2] * X[2][0];
       const float s1 = w3[0] * X[0][1] + w3[1] * X[1][1] + w3[2] * X[2][1];
       const float inv = 1.f / denom;
       const float Cx = c * inv, Cy = -b * inv, Cz = a * inv;
-      const float dgx = A3.z, dgy = A3.w;
+      // PLANE: u moves with g by -(T0, T1) . dL/du
+      const float dgx = PLANE ? A3.z - (T[0][0] * dLdu[0] + T[0][1] * dLdu[1] + T[0][2] * dLdu[2]) : A3.z;
+      const float dgy = PLANE ? A3.w - (T[1][0] * dLdu[0] + T[1][1] * dLdu[1] + T[1][2] * dLdu[2]) : A3.w;
       dLds0 = Cx * dgx + Cy * dgy;
       dLds1 = Cy * dgx + Cz * dgy;
       dLcx += s0 * dgx;
@@ -255,6 +278,11 @@ __device__ __forceinline__ void gauss_adjoint(
       dL_dT00 += dLds0 * v[0]; dL_dT01 += dLds0 * v[1]; dL_dT02 += dLds0 * v[2];
       dL_dT10 += dLds1 * v[0]; dL_dT11 += dLds1 * v[1]; dL_dT12 += dLds1 * v[2];
     }
+    if constexpr (PLANE) {
+      // u = w3 - g_x T0 - g_y T1: dL/dT_i += -g_i dL/du
+      dL_dT00 -= rec3.z * dLdu[0]; dL_dT01 -= rec3.z * dLdu[1]; dL_dT02 -= rec3.z * dLdu[2];
+      dL_dT10 -= rec3.w * dLdu[0]; dL_dT11 -= rec3.w * dLdu[1]; dL_dT12 -= rec3.w * dLdu[2];
+    }
     const float dL_dJ00 = Wm[0][0] * dL_dT00 + Wm[0][1] * dL_dT01 + Wm[0][2] * dL_dT02;
     const float dL_dJ02 = Wm[2][0] * dL_dT00 + Wm[2][1] * dL_dT01 + Wm[2][2] * dL_dT02;
     const float dL_dJ11 = Wm[1][0] * dL_dT10 + Wm[1][1] * dL_dT11 + Wm[1][2] * dL_dT12;
@@ -291,6 +319,11 @@ __device__ __forceinline__ void gauss_adjoint(
         // s_i = w3^T Sigma T_i^T: dL/dw3 = Sigma u
 #pragma unroll
         for (int k = 0; k < 3; k++) cam[C_VIEW + 4 * k + 2] += Vrk[k][0] * u[0] + Vrk[k][1] * u[1] + Vrk[k][2] * u[2];
+      }
+      if constexpr (PLANE) {
+        // u = w3 - ...: dL/dw3 += dL/du
+#pragma unroll
+        for (int k = 0; k < 3; k++) cam[C_VIEW + 4 * k + 2] += dLdu[k];
       }
     }
     if constexpr (NCAM > C_TANY) {
@@ -468,7 +501,7 @@ __device__ __forceinline__ void gauss_adjoint(
     o_rot[2] = 2 * x * (dMt[1][0] + dMt[0][1]) + 2 * r * (dMt[2][0] - dMt[0][2]) + 2 * z * (dMt[1][2] + dMt[2][1]) - 4 * y * (dMt[2][2] + dMt[0][0]);
     o_rot[3] = 2 * r * (dMt[0][1] - dMt[1][0]) + 2 * x * (dMt[2][0] + dMt[0][2]) + 2 * y * (dMt[1][2] + dMt[2][1]) - 4 * z * (dMt[1][1] + dMt[0][0]);
 
-    if (!norm_precomp) {
+    if (!PLANE && !norm_precomp) {
       // normal -> rotation (computeNorm3D bwd, backward.cu:380-428); the raw (unscaled) scales pick the axis
       float ax0, ax1, ax2;
       if (scx > scz && scy > scz) { ax0 = 0.f; ax1 = 0.f; ax2 = 1.f; }
@@ -572,8 +605,9 @@ static_assert(sizeof(float) * (GB_CAM_STAGE + GB_CAM * GB_SLOTS) <= sizeof(GbInp
 // H / (2 tan_fovy)), as in preprocess_kernel<DEV_FOV>.  A trailing parameter an instantiation does not read costs
 // nothing, and new parameters go at the end of the list.  ORTHO: the orthographic camera's adjoint (gauss_adjoint); only
 // <0, false, true> is instantiated.  RAYD: ray depth (gauss_adjoint), with host intrinsics: <0 | 35 | 37, false, false,
-// true> and <0, false, true, true>.
-template <int NCAM, bool DEV_FOV, bool ORTHO, bool RAYD = false>
+// true> and <0, false, true, true>.  PLANE: plane normals (gauss_adjoint), with RAYD: <0 | 35 | 37, false, false, true,
+// true> and <0, false, true, true, true>.
+template <int NCAM, bool DEV_FOV, bool ORTHO, bool RAYD = false, bool PLANE = false>
 __global__ void __launch_bounds__(GB_THREADS, GB_CTAS_PER_SM)
 gauss_bwd_kernel(int g_begin, int g_end, int spans_per_cta, int acc_row0, int D, int M,
                  const float* __restrict__ means3D, const int* __restrict__ radii, const float* __restrict__ shs,
@@ -709,7 +743,7 @@ gauss_bwd_kernel(int g_begin, int g_end, int spans_per_cta, int acc_row0, int D,
       const float* shk = reinterpret_cast<const float*>(&in.sh[0][k]);   // float j at word (j >> 2) * 4 * SLOTS + (j & 3)
       const float cov3D[6] = {in.cov[0][k], in.cov[1][k], in.cov[2][k], in.cov[3][k], in.cov[4][k], in.cov[5][k]};
       const unsigned cm = has_sh ? (in.clamped[k] >> (8 * (S.gidx[b][k] & 3))) & 0xffu : 0u;
-      gauss_adjoint<NCAM, ORTHO, RAYD>(D, in.mean[0][k], in.mean[1][k], in.mean[2][k], has_scales,
+      gauss_adjoint<NCAM, ORTHO, RAYD, PLANE>(D, in.mean[0][k], in.mean[1][k], in.mean[2][k], has_scales,
                     has_scales ? in.rot[k] : make_float4(0.f, 0.f, 0.f, 0.f),
                     has_scales ? in.scale[0][k] : 0.f, has_scales ? in.scale[1][k] : 0.f,
                     has_scales ? in.scale[2][k] : 0.f, scale_modifier, has_sh, cm,
@@ -862,15 +896,20 @@ void sfgs_launch_camera_partial_reduce(int n, int ncam, const double* cam_part, 
 // tan_fov: NULL (the launch parameters a->tan_fovx / a->tan_fovy, focal_x, focal_y are used) or DEVICE float [2], read
 // by the kernel (DEV_FOV)
 // ortho: the orthographic adjoint (focal_x / focal_y are its pixel scales); cam_part and tan_fov are then NULL
-// ray_depth: the ray-depth adjoint (tan_fov NULL)
+// ray_depth: the ray-depth adjoint (tan_fov NULL); plane_normals: the plane-normal adjoint (implies ray_depth)
 void sfgs_launch_gauss_bwd(const sfgs_backward_args* a, const GeomLayout& g, float focal_x, float focal_y,
                            const float* acc, int g_begin, int g_end, int acc_row0, double* cam_part, int ncam,
-                           const float* tan_fov, bool ortho, bool ray_depth, cudaStream_t st) {
+                           const float* tan_fov, bool ortho, bool ray_depth, bool plane_normals, cudaStream_t st) {
   if (g_end <= g_begin) return;
   const bool dev_fov = tan_fov != nullptr;
   const size_t smem = sizeof(GbShared);
   const auto kernel =
-      ray_depth ? (ortho                ? sfgs_smem_kernel<gauss_bwd_kernel<0, false, true, true>>(smem)
+      plane_normals
+          ? (ortho                 ? sfgs_smem_kernel<gauss_bwd_kernel<0, false, true, true, true>>(smem)
+             : cam_part == nullptr ? sfgs_smem_kernel<gauss_bwd_kernel<0, false, false, true, true>>(smem)
+             : ncam == GB_CAM      ? sfgs_smem_kernel<gauss_bwd_kernel<GB_CAM, false, false, true, true>>(smem)
+                                   : sfgs_smem_kernel<gauss_bwd_kernel<GB_CAM_POSE, false, false, true, true>>(smem))
+      : ray_depth ? (ortho                ? sfgs_smem_kernel<gauss_bwd_kernel<0, false, true, true>>(smem)
                    : cam_part == nullptr ? sfgs_smem_kernel<gauss_bwd_kernel<0, false, false, true>>(smem)
                    : ncam == GB_CAM      ? sfgs_smem_kernel<gauss_bwd_kernel<GB_CAM, false, false, true>>(smem)
                                          : sfgs_smem_kernel<gauss_bwd_kernel<GB_CAM_POSE, false, false, true>>(smem))

@@ -90,12 +90,13 @@ __device__ __forceinline__ void normal_from_scale_rot(float sx, float sy, float 
 // scales h = W / (2 s)): no clamp and no t dependence; everything after J is the perspective code.
 // RAYD: also s = (w3^T Sigma T0^T, w3^T Sigma T1^T) into *s_out, w3 = (vm[2], vm[6], vm[10]) the view's depth row: the
 // covariance of view depth with the two pixel coordinates, from the products X = T Sigma the 2D covariance is formed of.
-template <bool ORTHO, bool RAYD = false>
+// PLANE: also the two rows T0, T1 of T = J W (world coordinates) into t_out[0..2], t_out[3..5].
+template <bool ORTHO, bool RAYD = false, bool PLANE = false>
 __device__ __forceinline__ float4 cov2d_project(float mx, float my, float mz,
                                                 float focal_x, float focal_y,
                                                 float tan_fovx, float tan_fovy, float kernel_size,
                                                 const Sym3& V, const float* __restrict__ vm,
-                                                float2* s_out = nullptr) {
+                                                float2* s_out = nullptr, float* t_out = nullptr) {
   float a0, a2, b1, b2;   // J columns: (a0, 0, a2), (0, b1, b2), 0
   if constexpr (ORTHO) {
     a0 = focal_x; a2 = 0.0f; b1 = focal_y; b2 = 0.0f;
@@ -137,6 +138,10 @@ __device__ __forceinline__ float4 cov2d_project(float mx, float my, float mz,
   float c11 = X1[0] * T1[0] + X1[1] * T1[1] + X1[2] * T1[2];
   if constexpr (RAYD)
     *s_out = make_float2(vm[2] * X0[0] + vm[6] * X0[1] + vm[10] * X0[2], vm[2] * X1[0] + vm[6] * X1[1] + vm[10] * X1[2]);
+  if constexpr (PLANE) {
+#pragma unroll
+    for (int r = 0; r < 3; r++) { t_out[r] = T0[r]; t_out[3 + r] = T1[r]; }
+  }
 
   const float det_0 = fmax(1e-6, (double)(c00 * c11 - c01 * c01));
   const float det_1 = fmax(1e-6, (double)((c00 + kernel_size) * (c11 + kernel_size) - c01 * c01));
@@ -227,7 +232,12 @@ __device__ __forceinline__ float radius_bound(float trace_sigma, float view_z, f
 // RAYD: ray depth (sfgs_rasterize_forward_ray_depth).  Record words 14-15 get the depth slope g = C s in depth units
 // per pixel, C = (con.x, con.y, con.z) the record's conic and s from cov2d_project<ORTHO, true>; without it they are
 // 0.  Nothing else changes.  Instantiated with host intrinsics only.
-template <bool DEV_FOV, bool ORTHO, bool RAYD = false>
+// PLANE: plane normals (sfgs_rasterize_forward_plane_normals), with RAYD only.  Record words 11-13 get the normal of
+// the record's ray-depth plane in place of the shortest-axis normal: u = w3 - g_x T0 - g_y T1 (T0, T1 the rows of
+// T = J W from cov2d_project<ORTHO, true, true>, g the slope above), n = sigma u / |u| with sigma = -1 where
+// (m - cam_pos) . u > 0 (orthographic: w3 . u > 0), the shortest-axis normal's flip.  |u| >= 1 / |(t_x, t_y, t_z) /
+// t_z| > 0 (clamped t), so the division needs no guard.  norm3D_precomp is not read (the entries reject it).
+template <bool DEV_FOV, bool ORTHO, bool RAYD = false, bool PLANE = false>
 __global__ void __launch_bounds__(PRE_THREADS, 3)
 preprocess_kernel(int P, int D, int M,
                   const float* __restrict__ means3D, const float* __restrict__ scales, float scale_modifier,
@@ -377,6 +387,7 @@ preprocess_kernel(int P, int D, int M,
     float4 q = make_float4(0.f, 0.f, 0.f, 0.f);
     float g_pix_x = 0.f, g_pix_y = 0.f, g_conx = 0.f, g_cony = 0.f, g_conz = 0.f, g_coef = 0.f;
     float g_slx = 0.f, g_sly = 0.f;      // RAYD: the depth slope
+    float g_n0 = 0.f, g_n1 = 0.f, g_n2 = 0.f;   // PLANE: the plane normal
     Sym3 g_V = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
 
     if (in_range) {
@@ -416,8 +427,9 @@ preprocess_kernel(int P, int D, int M,
         }
 
         float2 s = make_float2(0.f, 0.f);
-        const float4 cov =
-            cov2d_project<ORTHO, RAYD>(px, py, pz, focal_x, focal_y, tan_fovx, tan_fovy, kernel_size, V, vm, &s);
+        float tt[6];   // PLANE: T0, T1
+        const float4 cov = cov2d_project<ORTHO, RAYD, PLANE>(px, py, pz, focal_x, focal_y, tan_fovx, tan_fovy,
+                                                             kernel_size, V, vm, &s, tt);
         const float det = (cov.x * cov.z - cov.y * cov.y);
         if (det != 0.0f) {
           const float det_inv = 1.f / det;
@@ -441,6 +453,17 @@ preprocess_kernel(int P, int D, int M,
             if constexpr (RAYD) {
               g_slx = s.x * conx + s.y * cony;
               g_sly = s.x * cony + s.y * conz;
+            }
+            if constexpr (PLANE) {
+              static_assert(RAYD, "plane normals are the normals of the ray-depth plane");
+              const float ux = vm[2] - g_slx * tt[0] - g_sly * tt[3];
+              const float uy = vm[6] - g_slx * tt[1] - g_sly * tt[4];
+              const float uz = vm[10] - g_slx * tt[2] - g_sly * tt[5];
+              const float inv_len = 1.f / sqrtf(ux * ux + uy * uy + uz * uz);
+              const float dx = ORTHO ? vm[2] : px - cam_pos[0], dy = ORTHO ? vm[6] : py - cam_pos[1];
+              const float dz = ORTHO ? vm[10] : pz - cam_pos[2];
+              const float f = dx * ux + dy * uy + dz * uz > 0 ? -inv_len : inv_len;
+              g_n0 = ux * f; g_n1 = uy * f; g_n2 = uz * f;
             }
             out_radius = iradius;
             out_tiles = ntiles;
@@ -469,7 +492,9 @@ preprocess_kernel(int P, int D, int M,
 #define VIEW_DIR ORTHO ? vm[2] : px, ORTHO ? vm[6] : py, ORTHO ? vm[10] : pz, ORTHO ? 0.f : cam_pos[0], \
                  ORTHO ? 0.f : cam_pos[1], ORTHO ? 0.f : cam_pos[2]
         float n[3];
-        if (norm3D_precomp != nullptr) {
+        if constexpr (PLANE) {
+          n[0] = g_n0; n[1] = g_n1; n[2] = g_n2;
+        } else if (norm3D_precomp != nullptr) {
           n[0] = norm3D_precomp[3 * (size_t)idx]; n[1] = norm3D_precomp[3 * (size_t)idx + 1]; n[2] = norm3D_precomp[3 * (size_t)idx + 2];
         } else {
           normal_from_scale_rot(sx, sy, sz, q.x, q.y, q.z, q.w, VIEW_DIR, n);
@@ -548,7 +573,7 @@ __global__ void mark_visible_kernel(int P, const float* __restrict__ means3D,
 
 void sfgs_launch_preprocess(const sfgs_forward_args* a, const GeomLayout& g, const ImageLayout& im,
                             const BinningLayout& b, unsigned long long capacity, float focal_x, float focal_y,
-                            const float* tan_fov, bool ortho, bool ray_depth, cudaStream_t st) {
+                            const float* tan_fov, bool ortho, bool ray_depth, bool plane_normals, cudaStream_t st) {
   const int blocks = (a->P + PRE_SPAN - 1) / PRE_SPAN;
   constexpr size_t smem = PRE_THREADS * (12 * sizeof(float4) + sizeof(uint32_t) + sizeof(int4) + sizeof(uint32_t)) +
                           PRE_SPAN * sizeof(unsigned short);
@@ -559,13 +584,19 @@ void sfgs_launch_preprocess(const sfgs_forward_args* a, const GeomLayout& g, con
     cudaFuncSetAttribute(preprocess_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     cudaFuncSetAttribute(preprocess_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     cudaFuncSetAttribute(preprocess_kernel<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(preprocess_kernel<false, false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                         (int)smem);
+    cudaFuncSetAttribute(preprocess_kernel<false, true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                         (int)smem);
   }
   const SfgsBand band = sfgs_band(a->tile_row_begin, a->tile_row_end, im.tiles_y);
   const int band0 = band.b0, band1 = band.b1;
   SFGS_COUNT_LAUNCH();
-  // ortho: tan_fov is NULL (the orthographic entries take the intrinsics as launch parameters); ray depth: likewise
-  // (its entries are not capturable)
-  const auto kernel = ray_depth ? (ortho ? preprocess_kernel<false, true, true> : preprocess_kernel<false, false, true>)
+  // ortho: tan_fov is NULL (the orthographic entries take the intrinsics as launch parameters); ray depth and plane
+  // normals (which imply ray depth): likewise (their entries are not capturable)
+  const auto kernel = plane_normals ? (ortho ? preprocess_kernel<false, true, true, true>
+                                             : preprocess_kernel<false, false, true, true>)
+                      : ray_depth ? (ortho ? preprocess_kernel<false, true, true> : preprocess_kernel<false, false, true>)
                       : ortho   ? preprocess_kernel<false, true>
                       : tan_fov != nullptr ? preprocess_kernel<true, false> : preprocess_kernel<false, false>;
   kernel<<<blocks, PRE_THREADS, smem, st>>>(

@@ -14,7 +14,9 @@ it never does, differentiable like the others; with GaussianRasterizer(settings,
 distortion[1,H,W]: sum_{i<j} w_i w_j (m_i - m_j)^2 over the pixel's blended splats, the distortion loss of Mip-NeRF
 360 / 2DGS, differentiable like the others.  With GaussianRasterizer(settings, ray_depth=True) the outputs are the
 same, but each splat's depth is taken where the pixel's ray meets it rather than at its centre (in depth and in
-depth_q), so the depth's gradient also reaches rotations and scales.  `means2D` is a dummy [P,3] leaf whose
+depth_q), so the depth's gradient also reaches rotations and scales; GaussianRasterizer(settings, ray_depth=True,
+plane_normals=True) also replaces each splat's shortest-axis normal by the normal of its ray-depth plane, so the
+normal map describes the surface the depth map renders.  `means2D` is a dummy [P,3] leaf whose
 .grad receives (dL/dx_ndc * W/2, dL/dy_ndc * H/2, sum |.|) — the densification
 statistics consumed by scene/gaussian_model.py:744-749.
 """
@@ -122,8 +124,8 @@ def _checked_inputs(shs, colors_precomp, scales, rotations, cov3Ds_precomp, norm
 class _RasterizeGaussians(torch.autograd.Function):
     """The rasterizer for the pinhole camera (diff_gauss) and the orthographic one (sfgs.ortho).  Every input slot is
     always passed: the callers resolve the options `fuse_normalize`, `depth_quantile` (q or None), `depth_distortion`,
-    `subpixel_offset` (a [H,W,2] tensor or None), `ortho` and `ray_depth` (the last slot has a default).  With a
-    quantile the outputs end with (depth_q, depth_q_pos); with the distortion, with distortion."""
+    `subpixel_offset` (a [H,W,2] tensor or None), `ortho`, `ray_depth` and `plane_normals` (the last three slots have
+    defaults).  With a quantile the outputs end with (depth_q, depth_q_pos); with the distortion, with distortion."""
     # viewmatrix, projmatrix and campos are inputs of their own (the settings tuple is not tracked by autograd), so a
     # camera built from parameters that require grad (scene/cameras.py: Camera(..., optimizing=True)) gets gradients
     CAMERA_INPUTS = slice(12, 15)
@@ -135,9 +137,11 @@ class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                 norm3Ds_precomp, extra_attrs, raster_settings, fuse_normalize, viewmatrix, projmatrix, campos, tanfovx,
-                tanfovy, depth_quantile, depth_distortion, subpixel_offset=None, ortho=False, ray_depth=False):
+                tanfovy, depth_quantile, depth_distortion, subpixel_offset=None, ortho=False, ray_depth=False,
+                plane_normals=False):
         rs = raster_settings
         ctx.depth_q, ctx.dist, ctx.ray_depth = depth_quantile is not None, bool(depth_distortion), bool(ray_depth)
+        ctx.plane_normals = bool(plane_normals)
         n_extra = extra_attrs.shape[1] if extra_attrs.shape[0] != 0 else 0
         assert n_extra <= MAX_EXTRA_DIMS
         # under stream capture (torch.cuda.graph) the capture-safe entries run: no host wait, intrinsics that are 0-d
@@ -147,7 +151,8 @@ class _RasterizeGaussians(torch.autograd.Function):
         opts = {}
         if ctx.graph:
             for on, what in ((ctx.depth_q, "the depth quantile"), (ctx.dist, "the depth distortion"),
-                             (ortho, "the orthographic camera"), (ctx.ray_depth, "ray depth")):
+                             (ortho, "the orthographic camera"), (ctx.plane_normals, "plane normals"),
+                             (ctx.ray_depth, "ray depth")):
                 if on:
                     raise _C.SfgsError(f"diff_gauss: {what} cannot be captured in a CUDA graph")
             if rs.debug:
@@ -164,6 +169,8 @@ class _RasterizeGaussians(torch.autograd.Function):
             opts["depth_distortion"] = True
         if ctx.ray_depth:
             opts["ray_depth"] = True
+        if ctx.plane_normals:
+            opts["plane_normals"] = True
         native_args = (rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier,
                        cov3Ds_precomp, norm3Ds_precomp, extra_attrs, n_extra, viewmatrix, projmatrix,
                        tanfovx, tanfovy, rs.kernel_size, rs.image_height, rs.image_width, sh, rs.sh_degree,
@@ -220,6 +227,8 @@ class _RasterizeGaussians(torch.autograd.Function):
             opts.update(distortion_state=side_state, dL_dout_distortion=g_side.contiguous())
         if ctx.ray_depth:
             opts["ray_depth"] = True
+        if ctx.plane_normals:
+            opts["plane_normals"] = True
         bwd = functools.partial(_C.rasterize_gaussians_backward_fused if ctx.fused else
                                 _C.rasterize_gaussians_backward, **opts)
         if ctx.subpixel_offset is not None:
@@ -233,23 +242,27 @@ class _RasterizeGaussians(torch.autograd.Function):
         (g_means2D, g_colors, g_opac, g_means3D, g_cov3D, g_norm3D, g_sh, g_scales, g_rot, g_extra_attrs) = grads[:10]
         # order of forward's inputs; the settings tuple and the options get no gradient
         return ((g_means3D, g_means2D, g_sh, g_colors, g_opac, g_scales, g_rot, g_cov3D, g_norm3D, g_extra_attrs)
-                + (None, None) + g_camera + g_intrinsics + (None,) * 5)
+                + (None, None) + g_camera + g_intrinsics + (None,) * 6)
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                         norm3Ds_precomp, extra_attrs, raster_settings, depth_quantile=None, depth_distortion=False,
-                        ray_depth=False):
+                        ray_depth=False, plane_normals=False):
     rs = raster_settings
     if depth_distortion and depth_quantile is not None:
         raise _C.SfgsError("diff_gauss: depth_distortion and depth_quantile in one call are not supported; render "
                            "them in two calls")
+    if plane_normals and not ray_depth:
+        raise _C.SfgsError("diff_gauss: plane_normals are the normals of the ray-depth plane and need ray_depth=True")
+    if depth_distortion and plane_normals:
+        raise _C.SfgsError("diff_gauss: depth_distortion together with plane_normals is not supported")
     if depth_distortion and ray_depth:
         raise _C.SfgsError("diff_gauss: depth_distortion together with ray_depth is not supported")
     out = _RasterizeGaussians.apply(
         means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, norm3Ds_precomp,
         extra_attrs, rs, FUSE_NORMALIZE, rs.viewmatrix, rs.projmatrix, rs.campos, rs.tanfovx, rs.tanfovy,
         None if depth_quantile is None else float(depth_quantile), bool(depth_distortion), _subpixel_offset(rs), False,
-        bool(ray_depth))
+        bool(ray_depth), bool(plane_normals))
     color, depth, norm, alpha, radii, extra = out[:6]
     if not FUSE_NORMALIZE:
         # the reference normalises the blended normal map in torch, inside the autograd graph (diff_gauss/__init__.py:48)
@@ -264,14 +277,18 @@ class GaussianRasterizer(nn.Module):
     (include/sfgs.h, sfgs_rasterize_forward_distortion).  Not under CUDA-graph capture, and not both in one call.
     ray_depth=True: the same outputs, with each splat's depth taken where the pixel's ray meets it, z + g . (p - mu),
     not at its centre (include/sfgs.h, sfgs_rasterize_forward_ray_depth); combines with depth_quantile, not with
-    depth_distortion or CUDA-graph capture."""
+    depth_distortion or CUDA-graph capture.  plane_normals=True (with ray_depth=True): the same outputs, with each
+    splat's normal that of its ray-depth plane rather than its shortest axis (include/sfgs.h,
+    sfgs_rasterize_forward_plane_normals); norm3Ds_precomp raises with it."""
 
-    def __init__(self, raster_settings, depth_quantile=None, depth_distortion=False, ray_depth=False):
+    def __init__(self, raster_settings, depth_quantile=None, depth_distortion=False, ray_depth=False,
+                 plane_normals=False):
         super().__init__()
         self.raster_settings = raster_settings
         self.depth_quantile = depth_quantile
         self.depth_distortion = depth_distortion
         self.ray_depth = ray_depth
+        self.plane_normals = plane_normals
 
     def markVisible(self, positions):
         """Boolean mask of the points in front of the near plane (view depth > 0.2)."""
@@ -285,4 +302,4 @@ class GaussianRasterizer(nn.Module):
             shs, colors_precomp, scales, rotations, cov3Ds_precomp, norm3Ds_precomp, extra_attrs)
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                                    norm3Ds_precomp, extra_attrs, self.raster_settings, self.depth_quantile,
-                                   self.depth_distortion, self.ray_depth)
+                                   self.depth_distortion, self.ray_depth, self.plane_normals)

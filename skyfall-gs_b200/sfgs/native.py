@@ -103,6 +103,7 @@ EXPORTS = [
     "sfgs_rasterize_forward_depth_quantile", "sfgs_rasterize_backward_depth_quantile",
     "sfgs_rasterize_forward_distortion", "sfgs_rasterize_backward_distortion",
     "sfgs_rasterize_forward_ray_depth", "sfgs_rasterize_backward_ray_depth",
+    "sfgs_rasterize_forward_plane_normals", "sfgs_rasterize_backward_plane_normals",
 ]
 STAGE_NAMES = ["fwd_zero", "preprocess", "tile_scan", "emit_keys", "tile_sort", "render_fwd", "bwd_zero", "render_bwd",
                "gauss_bwd", "bwd_order"]
@@ -170,6 +171,12 @@ def lib() -> C.CDLL:
     L.sfgs_rasterize_backward_ray_depth.argtypes = [C.POINTER(BackwardArgs), C.c_void_p, C.c_int, C.c_int, C.c_void_p,
                                                     C.c_void_p, C.c_void_p, C.c_int]
     L.sfgs_rasterize_backward_ray_depth.restype = C.c_int
+    L.sfgs_rasterize_forward_plane_normals.argtypes = [C.POINTER(ForwardArgs), C.c_void_p, C.c_int, C.c_float,
+                                                       C.c_void_p, C.c_void_p]
+    L.sfgs_rasterize_forward_plane_normals.restype = C.c_int
+    L.sfgs_rasterize_backward_plane_normals.argtypes = [C.POINTER(BackwardArgs), C.c_void_p, C.c_int, C.c_int,
+                                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
+    L.sfgs_rasterize_backward_plane_normals.restype = C.c_int
     L.sfgs_capacity_estimate.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int]
     L.sfgs_capacity_estimate.restype = C.c_longlong
     L.sfgs_mark_visible.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]

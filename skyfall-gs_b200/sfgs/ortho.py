@@ -101,15 +101,18 @@ class OrthoRasterizer(nn.Module):
     gradients: a viewmatrix or projmatrix that requires grad raises.  With depth_quantile=q (0 < q < 1) a 7th output,
     depth_q [1,H,W], as for diff_gauss.GaussianRasterizer; with depth_distortion=True a 7th output, distortion [1,H,W],
     likewise (not both in one call).  ray_depth=True: the same outputs with each splat's depth taken where the pixel's
-    ray meets it (as for diff_gauss.GaussianRasterizer); with depth_quantile, not with depth_distortion."""
+    ray meets it (as for diff_gauss.GaussianRasterizer); with depth_quantile, not with depth_distortion.
+    plane_normals=True (with ray_depth=True): each splat's normal is that of its ray-depth plane (as for
+    diff_gauss.GaussianRasterizer); norm3Ds_precomp raises with it."""
 
     def __init__(self, raster_settings: OrthoRasterizationSettings, depth_quantile=None, depth_distortion=False,
-                 ray_depth=False):
+                 ray_depth=False, plane_normals=False):
         super().__init__()
         self.raster_settings = raster_settings
         self.depth_quantile = depth_quantile
         self.depth_distortion = depth_distortion
         self.ray_depth = ray_depth
+        self.plane_normals = plane_normals
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
                 cov3Ds_precomp=None, norm3Ds_precomp=None, extra_attrs=None):
@@ -131,6 +134,11 @@ class OrthoRasterizer(nn.Module):
         if self.depth_distortion and self.depth_quantile is not None:
             raise N.SfgsError("OrthoRasterizer: depth_distortion and depth_quantile in one call are not supported; "
                               "render them in two calls")
+        if self.plane_normals and not self.ray_depth:
+            raise N.SfgsError("OrthoRasterizer: plane_normals are the normals of the ray-depth plane and need "
+                              "ray_depth=True")
+        if self.depth_distortion and self.plane_normals:
+            raise N.SfgsError("OrthoRasterizer: depth_distortion together with plane_normals is not supported")
         if self.depth_distortion and self.ray_depth:
             raise N.SfgsError("OrthoRasterizer: depth_distortion together with ray_depth is not supported")
         # the half-extents travel in the tan_fov fields (as numbers: they get no gradient), and campos is not read
@@ -144,7 +152,7 @@ class OrthoRasterizer(nn.Module):
             means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, norm3Ds_precomp,
             extra_attrs, settings, True, rs.viewmatrix, rs.projmatrix, campos, s_x, s_y,
             None if self.depth_quantile is None else float(self.depth_quantile), bool(self.depth_distortion),
-            rs.subpixel_offset, True, bool(self.ray_depth))
+            rs.subpixel_offset, True, bool(self.ray_depth), bool(self.plane_normals))
 
 
 def render_height_map(camera: NadirCamera, means3D, opacities, scales, rotations, shs=None, colors_precomp=None,

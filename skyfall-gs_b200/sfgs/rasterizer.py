@@ -95,6 +95,16 @@ ORTHO = "not supported with an orthographic camera"
 DEPTH_Q = "not supported with the depth quantile"
 DISTORTION = "not supported with the depth distortion"
 RAY_DEPTH = "not supported with ray depth"
+PLANE_NORMALS = "not supported with plane normals"
+
+
+def _check_plane_normals(where, ray_depth, norm3Ds_precomp, **opts):
+    """plane_normals=True: it needs ray_depth=True, and norm3Ds_precomp and each option of `opts` that is set raise
+    SfgsError, before any native call."""
+    if not ray_depth:
+        raise N.SfgsError(f"{where}: plane normals are the normals of the ray-depth plane and need ray_depth=True")
+    _reject(where, PLANE_NORMALS, **opts,
+            norm3Ds_precomp=norm3Ds_precomp is not None and norm3Ds_precomp.numel() != 0)
 
 
 def _reject(where, tail, **opts):
@@ -127,7 +137,7 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
                         tan_fovx, tan_fovy, kernel_size, image_height, image_width, sh, degree, campos,
                         prefiltered, debug, capacity_hint=0, tile_rows=None, fuse_normalize=False, out_planes=None,
                         out_peers=None, subpixel_offset=None, graph=False, *, ortho=False, depth_quantile=None,
-                        depth_distortion=False, ray_depth=False):
+                        depth_distortion=False, ray_depth=False, plane_normals=False):
     """Same positional signature and return tuple as the reference's `_C.rasterize_gaussians`.  With
     `fuse_normalize=True` the returned normal map is already F.normalize(., dim=0) (the reference's torch post-op,
     diff_gauss/__init__.py:48) and the un-normalised blend is appended to the tuple for the backward.
@@ -164,10 +174,20 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
     ray meets it, d(p) = z + g . (p - mu) with g its depth slope, not its centre's depth z, in out_depth and (with
     `depth_quantile`) in depth_q.  The backward must be given `ray_depth=True` too.  It combines with `ortho`, offsets
     and `depth_quantile`; depth_distortion, graph, tile_rows, out_peers and extra_attrs raise SfgsError.  Every other
-    output is bit-identical to the call without it."""
+    output is bit-identical to the call without it.
+
+    `plane_normals=True` (with `ray_depth=True`; sfgs_rasterize_forward_plane_normals, include/sfgs.h): the normal
+    map blends the normal of each splat's ray-depth plane, u = w3 - g_x T0 - g_y T1 flipped toward the camera, in place
+    of its shortest axis, so the normals describe the surface the depth map renders.  The backward must be given
+    `plane_normals=True` too.  Without ray_depth it raises, and so do norm3Ds_precomp and everything ray depth rejects,
+    naming plane normals.  Every other output is bit-identical to the `ray_depth=True` call."""
     if means3D.ndim != 2 or means3D.shape[1] != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")
     banded = dict(tile_rows=tile_rows is not None, out_peers=out_peers is not None)
+    if plane_normals:
+        _check_plane_normals("rasterize_gaussians(plane_normals=True)", ray_depth, norm3Ds_precomp,
+                             depth_distortion=depth_distortion, graph=graph, **banded,
+                             extra_attrs=int(attr_degree) > 0)
     if ray_depth:
         _reject("rasterize_gaussians(ray_depth=True)", RAY_DEPTH, depth_distortion=depth_distortion, graph=graph,
                 **banded, extra_attrs=int(attr_degree) > 0)
@@ -263,10 +283,10 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
             off = _ptr(subpixel_offset, keep)
             if ray_depth:
                 q = depth_quantile is not None
-                entry, args = "sfgs_rasterize_forward_ray_depth", (off, int(bool(ortho)),
-                                                                   float(depth_quantile) if q else 0.0,
-                                                                   side[0].data_ptr() if q else None,
-                                                                   side[1].data_ptr() if q else None)
+                entry = "sfgs_rasterize_forward_plane_normals" if plane_normals else "sfgs_rasterize_forward_ray_depth"
+                args = (off, int(bool(ortho)),
+                        float(depth_quantile) if q else 0.0, side[0].data_ptr() if q else None,
+                        side[1].data_ptr() if q else None)
             elif depth_quantile is not None:
                 entry, args = "sfgs_rasterize_forward_depth_quantile", (off, int(bool(ortho)), float(depth_quantile),
                                                                         side[0].data_ptr(), side[1].data_ptr())
@@ -327,7 +347,7 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
                                  gauss_range=None, acc_peers=None, peer_slice=0, subpixel_offset=None,
                                  camera_grad=False, intrinsics_grad=False, graph=False, *, ortho=False,
                                  depth_q_pos=None, dL_dout_depth_q=None, distortion_state=None,
-                                 dL_dout_distortion=None, ray_depth=False):
+                                 dL_dout_distortion=None, ray_depth=False, plane_normals=False):
     """Same positional signature and return tuple as the reference's `_C.rasterize_gaussians_backward`.  With
     `norm_raw` (the extra tensor a `fuse_normalize=True` forward returned) `dL_dout_norm` is taken w.r.t. the unit
     normal map and the adjoint of F.normalize is applied inside the blend-adjoint kernel.
@@ -383,9 +403,18 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     its depth quantile's `depth_q_pos` / `dL_dout_depth_q`; the depth cotangents then also reach each splat's depth
     slope, and through it its rotation, scale and covariance.  It takes offsets, `ortho`, the deterministic mode,
     phase 1, and camera and focal gradients (not with `ortho`); distortion_state, graph, tile_rows, acc_peers and
-    extra_attrs raise SfgsError."""
+    extra_attrs raise SfgsError.
+
+    `plane_normals=True` (with `ray_depth=True`): the backward of a `plane_normals=True` forward
+    (sfgs_rasterize_backward_plane_normals); the normal cotangent reaches each splat's plane normal, and through it its
+    depth slope, covariance, rotation, scale, mean and the camera and focal terms.  dL_dnorm3D is 0.  It takes what
+    `ray_depth=True` takes; without ray_depth it raises, and so do norm3Ds_precomp and everything ray depth rejects."""
     banded = dict(tile_rows=tile_rows is not None, acc_peers=acc_peers is not None)
     has_extra = extra_attrs is not None and extra_attrs.numel() != 0
+    if plane_normals:
+        _check_plane_normals("rasterize_gaussians_backward(plane_normals=True)", ray_depth, norm3Ds_precomp,
+                             distortion_state=distortion_state is not None or dL_dout_distortion is not None,
+                             graph=graph, **banded, extra_attrs=has_extra)
     if ray_depth:
         _reject("rasterize_gaussians_backward(ray_depth=True)", RAY_DEPTH,
                 distortion_state=distortion_state is not None or dL_dout_distortion is not None, graph=graph, **banded,
@@ -516,10 +545,10 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
                 det = int(deterministic)
                 cam = dL_dcamera.data_ptr() if ncam else None
                 if ray_depth:
-                    entry, args = "sfgs_rasterize_backward_ray_depth", (off, int(bool(ortho)), det,
-                                                                        _ptr(depth_q_pos, keep) if depth_q else None,
-                                                                        _ptr(dL_dout_depth_q, keep) if depth_q else None,
-                                                                        cam, ncam)
+                    entry = ("sfgs_rasterize_backward_plane_normals" if plane_normals
+                             else "sfgs_rasterize_backward_ray_depth")
+                    args = (off, int(bool(ortho)), det, _ptr(depth_q_pos, keep) if depth_q else None,
+                            _ptr(dL_dout_depth_q, keep) if depth_q else None, cam, ncam)
                 elif depth_q:
                     entry, args = "sfgs_rasterize_backward_depth_quantile", (off, int(bool(ortho)), det,
                                                                              _ptr(depth_q_pos, keep),
